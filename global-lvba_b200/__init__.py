@@ -41,6 +41,8 @@ EXPORTS = [
     "lvba_tracks_triangulate", "lvba_tracks_mean_reproj",
     "lvba_fuse_default_opts", "lvba_tracks_fuse_create", "lvba_tracks_fuse_summary", "lvba_tracks_fuse_export", "lvba_tracks_fuse_destroy",
     "lvba_anchor_clouds_create", "lvba_anchor_clouds_export", "lvba_anchor_clouds_destroy",
+    "lvba_colorizer_create", "lvba_colorizer_begin", "lvba_colorizer_add_images", "lvba_colorizer_finish",
+    "lvba_colorizer_export", "lvba_colorizer_destroy",
     "lvba_env_solve", "lvba_lidar_owned_rows", "lvba_visual_owned_rows", "lvba_comm_bytes_sent",
     "lvba_comm_unique_id", "lvba_comm_init", "lvba_comm_destroy", "lvba_comm_info", "lvba_shard_owner",
 ]
@@ -576,6 +578,91 @@ class DepthGrid:
                                               _p(it, C.c_double), C.c_int32(width), C.c_int32(height), _p(kp, C.c_int64), _p(uv, C.c_float),
                                               _p(Xw, C.c_double), _p(valid, C.c_uint8), C.byref(s)))
         return Xw, valid, s.as_dict()
+
+
+# ------------------------------------------------------------------ B8: coloured LiDAR map
+class ColorizeSummary(C.Structure):
+    _fields_ = [(k, C.c_int64) for k in ("n_points", "n_images", "n_listed", "n_projections", "n_landed", "n_survivors", "n_out")] + \
+               [("ms_device", C.c_double), ("ms_total", C.c_double)] + \
+               [(k, C.c_int64) for k in ("kernel_launches", "h2d_bytes", "d2h_bytes", "peak_device_bytes")]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+class Colorizer:
+    """The coloured LiDAR map of VisualizeOptComparison (lvba_system.cpp:1932-2143) on the device: scans uploaded once, then one
+    begin() .. add_images() .. finish() per pose set (the optimised poses, then the poses from before the optimisation)."""
+
+    def __init__(self, scans, frame_ts, device=-1, scan_ptr=None):
+        lib = load_library()
+        self._lib = lib
+        ts = _f64(frame_ts)
+        if scan_ptr is None:
+            F = len(scans)
+            sp = np.zeros(F + 1, np.int64)
+            sp[1:] = np.cumsum([len(s) for s in scans])
+            xyz = (np.concatenate([np.asarray(s, np.float32).reshape(-1, 3) for s in scans]) if F else np.zeros((0, 3), np.float32))
+        else:
+            sp = np.ascontiguousarray(scan_ptr, np.int64); F = len(sp) - 1
+            xyz = np.asarray(scans, np.float32)
+        xyz = np.ascontiguousarray(xyz, np.float32)
+        stride = xyz.shape[1] if xyz.ndim == 2 else 3
+        self.F = F
+        self._h = C.c_void_p()
+        _chk(lib.lvba_colorizer_create(C.c_int32(F), _p(sp, C.c_int64), _p(xyz, C.c_float), C.c_int32(stride), _p(ts, C.c_double),
+                                       C.c_int32(device), C.byref(self._h)))
+
+    def close(self):
+        if self._h:
+            self._lib.lvba_colorizer_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def begin(self, frame_poses, leaf, half_window=0.5):
+        ps = _f64(frame_poses).reshape(-1, 12)
+        _chk(self._lib.lvba_colorizer_begin(self._h, _p(ps, C.c_double), C.c_double(half_window), C.c_double(leaf)))
+
+    def add_images(self, image_ts, cams, intr, width, height, rgb=None):
+        """cams (n, 12) = Rcw row-major, tcw; rgb (n, height, width, 3) uint8 in R, G, B order or None (grey).
+        Returns listed (n,) uint8: 1 where the image has LiDAR in its window."""
+        cams = _f64(cams).reshape(-1, 12); its = _f64(image_ts); it = _f64(intr)
+        n = len(cams)
+        listed = np.zeros(n, np.uint8)
+        img = None
+        if rgb is not None:
+            img = np.ascontiguousarray(rgb, np.uint8)
+            if img.shape != (n, height, width, 3):
+                raise ValueError(f"rgb has shape {img.shape}, expected {(n, height, width, 3)}")
+        _chk(self._lib.lvba_colorizer_add_images(self._h, C.c_int32(n), _p(its, C.c_double), _p(cams, C.c_double), _p(it, C.c_double),
+                                                 C.c_int32(width), C.c_int32(height), _p(img, C.c_uint8) if img is not None else None,
+                                                 _p(listed, C.c_uint8)))
+        return listed
+
+    def finish(self):
+        """Returns (xyz (n, 3) float32, rgb (n, 3) uint8, summary dict)."""
+        n = C.c_int64(); s = ColorizeSummary()
+        _chk(self._lib.lvba_colorizer_finish(self._h, C.byref(n), C.byref(s)))
+        xyz = np.zeros((n.value, 3), np.float32); rgb = np.zeros((n.value, 3), np.uint8)
+        _chk(self._lib.lvba_colorizer_export(self._h, _p(xyz, C.c_float), _p(rgb, C.c_uint8)))
+        return xyz, rgb, s.as_dict()
+
+    def run(self, frame_poses, image_ts, cams, intr, width, height, rgb=None, leaf=0.01, half_window=0.5, batch=None):
+        """One pose set end to end; `batch` images per add_images call (None: all at once).  Returns (xyz, rgb, listed, summary)."""
+        self.begin(frame_poses, leaf, half_window)
+        cams = _f64(cams).reshape(-1, 12); its = _f64(image_ts)
+        n = len(cams); step = n if not batch else int(batch)
+        listed = [np.zeros(0, np.uint8)]
+        for k0 in range(0, n, max(step, 1)):
+            sl = slice(k0, k0 + step)
+            listed.append(self.add_images(its[sl], cams[sl], intr, width, height, None if rgb is None else rgb[sl]))
+        xyz, col, s = self.finish()
+        return xyz, col, np.concatenate(listed), s
 
 
 # ------------------------------------------------------------------ B5: per-track numerics of the track fusion

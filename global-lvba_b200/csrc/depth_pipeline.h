@@ -61,15 +61,16 @@ LVBA_HD void affine3(const double* m, const double* x, double* y) {
     y[k] = add_(add_(add_(mul_(m[3 * k], x[0]), mul_(m[3 * k + 1], x[1])), mul_(m[3 * k + 2], x[2])), m[9 + k]);
 }
 
-// generateDepthWithVoxel's inner loop (:885-901) for one world point: returns the pixel index or -1, and (float)Z.
-LVBA_HD int64_t project_pixel(const double* cam, const double* intr, int width, int height, const double* pw, float* zf) {
+// projectCameraToPixel / projectWorldToPixel (include/utils.hpp:169-205) for one world point: false when the point is not in
+// front of the camera or an intermediate is non-finite, else the distorted pixel (uu, vv) and the camera depth Z.  Shared by the
+// depth z-buffer (B4) and the colour z-buffer (B8, color_pipeline.h), which differ only in the gate on Z and the pixel rounding.
+LVBA_HD bool project_uv(const double* cam, const double* intr, const double* pw, double* u_out, double* v_out, double* Z_out) {
   double pc[3];
   affine3(cam, pw, pc);
   const double Z = pc[2];
-  if (Z < 1e-3) return -1;                                                    // :889
-  if (!(finite_(pc[0]) && finite_(pc[1]) && finite_(pc[2])) || !(Z > 1e-12)) return -1;   // utils.hpp:186-188
+  if (!(finite_(pc[0]) && finite_(pc[1]) && finite_(pc[2])) || !(Z > 1e-12)) return false;   // utils.hpp:186-188
   const double x = pc[0] / Z, y = pc[1] / Z;
-  if (!(finite_(x) && finite_(y))) return -1;
+  if (!(finite_(x) && finite_(y))) return false;
   const double fx = intr[0], fy = intr[1], cx = intr[2], cy = intr[3], k1 = intr[4], k2 = intr[5], p1 = intr[6], p2 = intr[7];
   const double r2 = add_(mul_(x, x), mul_(y, y));                             // utils.hpp:173-179
   const double r4 = mul_(r2, r2);
@@ -77,9 +78,17 @@ LVBA_HD int64_t project_pixel(const double* cam, const double* intr, int width, 
   const double x_tan = add_(mul_(mul_(mul_(2.0, p1), x), y), mul_(p2, add_(r2, mul_(mul_(2.0, x), x))));
   const double y_tan = add_(mul_(p1, add_(r2, mul_(mul_(2.0, y), y))), mul_(mul_(mul_(2.0, p2), x), y));
   const double xd = add_(mul_(x, radial), x_tan), yd = add_(mul_(y, radial), y_tan);
-  if (!(finite_(xd) && finite_(yd))) return -1;
+  if (!(finite_(xd) && finite_(yd))) return false;
   const double uu = add_(mul_(fx, xd), cx), vv = add_(mul_(fy, yd), cy);      // utils.hpp:193-194
-  if (!(finite_(uu) && finite_(vv))) return -1;
+  if (!(finite_(uu) && finite_(vv))) return false;
+  *u_out = uu; *v_out = vv; *Z_out = Z;
+  return true;
+}
+
+// generateDepthWithVoxel's inner loop (:885-901) for one world point: returns the pixel index or -1, and (float)Z.
+LVBA_HD int64_t project_pixel(const double* cam, const double* intr, int width, int height, const double* pw, float* zf) {
+  double uu, vv, Z;
+  if (!project_uv(cam, intr, pw, &uu, &vv, &Z) || Z < 1e-3) return -1;      // :889 (a pure rejection, so its place is free)
   if (!(fabs(uu) < 2147483648.0 && fabs(vv) < 2147483648.0)) return -1;       // the (int) cast below is only defined in range
   const int u = (int)uu, v = (int)vv;                                          // :894-895 truncation toward zero
   if (u < 0 || u >= width || v < 0 || v >= height) return -1;

@@ -9,6 +9,7 @@
 #include "track_api.cuh"
 #include "anchor_api.cuh"
 #include "fuse_api.cuh"
+#include "color_api.cuh"
 
 extern "C" {
 

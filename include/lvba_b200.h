@@ -358,6 +358,52 @@ int lvba_depth_backproject(lvba_depth_grid* g, int32_t n_images, const double* c
 int lvba_depth_grid_destroy(lvba_depth_grid* g);
 
 /* ======================================================================================
+ * B8  coloured LiDAR map — the numeric part of VisualizeOptComparison, src/lvba_system.cpp:1932-2143:
+ *     per image (in the order given): the scans with |x_buf[idx].t - id| <= half_window (a linear scan over all frames, any
+ *     timestamp order, :1973-1977), every point moved to the world as (float)(R p + t) (:1983-1990); an image whose window holds
+ *     no point is not listed (:1993-1996, the skip precedes its images.txt line); a z-buffer in cloud order (scan, then point):
+ *     projectWorldToPixel (include/utils.hpp:183-205), round() to the pixel, `if (zc + 1e-6f < zbuf) { zbuf = (float)zc; keep }`
+ *     (:2037-2060, order dependent); the kept points in pixel order coloured from the image (:2051-2055, :2062-2069); after
+ *     all images down_sampling_voxel2(merged, leaf) (include/BALM/tools.hpp:301-359; leaf < 0.001 keeps every point).
+ *   create: the scans once (n_frames, scan_ptr, xyz, xyz_stride_floats as for B3; frame_ts [n_frames] = x_buf[i].t)
+ *   begin:  one pose set: frame_poses [n_frames*12], half_window 0.5, leaf colmap_output/filter_size_points3D.  The two
+ *           clouds of the reference pair poses and cameras as follows (:1983-1990, :1998-2001, :2041, :2079):
+ *             after  (points3D.txt, colored_merged_after.pcd):  frame_poses = x_buf_,         cams = Rcw_all_optimized_ / tcw_all_optimized_
+ *             before (colored_merged_before.pcd):               frame_poses = x_buf_before_,  cams = Rcw_all_ / tcw_all_
+ *           With leaf >= 0.001 every FINITE world point of every scan — not only those in some image's window — must lie within
+ *           2^30 leaf voxels of the origin, else LVBA_ERR_INVALID_ARG (the rule of B6); the voxel-key range is taken over them too.
+ *           Non-finite pose or camera entries are LVBA_ERR_INVALID_ARG.  The reference would instead drop the points they touch
+ *           (projectWorldToPixel's allFinite) and still list the image; this stage refuses such input rather than guess.
+ *   add_images (any number of calls): image_ts [n], cams [n*12] Rcw row-major then tcw, intr fx fy cx cy k1 k2 p1 p2, the
+ *           image size after any resize, rgb [n][height][width][3] in R, G, B order (NULL: every point (128, 128, 128)),
+ *           listed [n] out: 1 when the image has LiDAR in its window.  The library cuts the images into device batches itself.
+ *   finish: n_out; export: xyz [n_out*3] float, rgb [n_out*3], in ascending (kx, ky, kz) leaf-voxel order (x-major, signed)
+ *           — the reference's unordered_map order is unspecified — or, with leaf < 0.001, in merged order.
+ *   Device memory is bounded by the scans, the thinned table and one batch, not by the number of images.
+ * ====================================================================================== */
+typedef struct lvba_colorize_summary {
+  int64_t n_points;          /* LiDAR points of the scans */
+  int64_t n_images, n_listed;
+  int64_t n_projections;     /* (image, window point) pairs projected */
+  int64_t n_landed;          /* of those, inside their image */
+  int64_t n_survivors;       /* z-buffer survivors of all images = size of the merged cloud before thinning */
+  int64_t n_out;
+  double ms_device, ms_total;
+  int64_t kernel_launches, h2d_bytes, d2h_bytes;
+  int64_t peak_device_bytes; /* the stage's own device buffers at their largest (sort scratch aside) */
+} lvba_colorize_summary;
+
+typedef struct lvba_colorizer lvba_colorizer;
+int lvba_colorizer_create(int32_t n_frames, const int64_t* scan_ptr, const float* xyz, int32_t xyz_stride_floats,
+                          const double* frame_ts, int32_t device, lvba_colorizer** out);
+int lvba_colorizer_begin(lvba_colorizer* c, const double* frame_poses, double half_window, double leaf);
+int lvba_colorizer_add_images(lvba_colorizer* c, int32_t n_images, const double* image_ts, const double* cams, const double intr[8],
+                              int32_t width, int32_t height, const uint8_t* rgb /* may be NULL */, uint8_t* listed);
+int lvba_colorizer_finish(lvba_colorizer* c, int64_t* n_out, lvba_colorize_summary* summary /* may be NULL */);
+int lvba_colorizer_export(lvba_colorizer* c, float* xyz, uint8_t* rgb);
+int lvba_colorizer_destroy(lvba_colorizer* c);
+
+/* ======================================================================================
  * B5  per-track numerics of the track fusion (BuildTracksAndFuse3D, src/lvba_system.cpp:921-1263), many tracks at once:
  *       TriangulateTrackDLT   src/lvba_system.cpp:52-111    lvba_tracks_triangulate
  *       ComputeMeanReproj     src/lvba_system.cpp:8-50      lvba_tracks_mean_reproj
