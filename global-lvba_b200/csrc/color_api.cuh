@@ -1,5 +1,5 @@
 // color_api.cuh — boundary B8: the coloured LiDAR map of VisualizeOptComparison (src/lvba_system.cpp:1932-2143) on the device.
-// Passes: color_pipeline.h; execution policy: CudaExec (voxel_api.cuh).  No host path.
+// Passes: color_pipeline.h; execution policy: CudaExec (exec.cuh).  No host path.
 #pragma once
 #include "color_pipeline.h"
 #include "voxel_api.cuh"

@@ -1,5 +1,5 @@
 // depth_api.cuh — boundary B4 (SURVEY.md §8f N3, first half): depth images rendered from the world point grid on the device.
-// Passes: depth_pipeline.h; execution policy: CudaExec (voxel_api.cuh).  No host path.
+// Passes: depth_pipeline.h; execution policy: CudaExec (exec.cuh).  No host path.
 #pragma once
 #include "depth_pipeline.h"
 #include "voxel_api.cuh"

@@ -5,8 +5,9 @@
 //   PointCluster::transform            reference include/BALM/tools.hpp:450-456
 //
 // Work decomposition (GPU-first, not the reference's 16 std::threads over dense W-slot vectors):
-//   * the non-empty (voxel, pose) slots are stored CSR and cut on the host into *batches* of
-//     consecutive voxels holding <= kSlots slots; one CTA of kSlots threads owns one batch;
+//   * the non-empty (voxel, pose) slots are stored CSR, the voxels in the order of their lowest pose (lidar_tiles.h);
+//   * the Hessian build cuts them into *tiles* of consecutive voxels holding <= kTileSlots slots, one CTA of kTileSlots
+//     threads per tile; the residual pass cuts the same order into batches of <= kSlots slots, one 128-thread CTA each;
 //   * phase 1: one thread per slot — coalesced double2 loads of the SoA cluster record, gathered pose,
 //              rigid transform of the cluster, staged in shared memory;
 //   * phase 2: one thread per voxel — merge the staged clusters, 3x3 Jacobi eigen-solve;
@@ -14,20 +15,26 @@
 //              f1 = A_i^T u1, f2 = A_i^T u2, b = [v_i x R_i^T u0 ; n_i u0]; the off-diagonal block of any
 //              pose pair is the rank-3 product  c1 f1_i f1_j^T + c2 f2_i f2_j^T - 2/N^2 b_i b_j^T
 //              (algebraically identical to bavoxel.hpp:159-163, re-associated);
-//   * phase 4: every warp takes 8 pose pairs at a time: 8*36 = 288 block elements = 9 per lane, each a
-//              3-FMA product of factors followed by one RED.ADD.F64 into the block-envelope Hessian.  Four lanes share a
-//              pair and write one aligned 32-byte sector per instruction; a lane reads the 27 factor values of its 9
-//              elements from shared memory once.  Diagonal blocks and g_i are staged in shared memory and flushed with
-//              32 consecutive doubles per warp instruction.
+//   * phase 4: every distinct H block and gradient row of the tile is summed on chip and written with one RED.ADD.F64 per
+//              element.  A destination table built once per structure (lidar_tiles.h) lists the tile's pose pairs grouped
+//              by H block and its slots grouped by pose.  Off-diagonal blocks: four lanes per block, each summing 9 elements
+//              (3-FMA products of the factors) over the pairs of the block in registers, one aligned 32-byte sector per RED
+//              instruction.  Diagonal blocks and g_i: staged in shared memory and summed per pose.
+//              Sorted voxels share pose pairs: at config C a 256-slot tile holds 2.5 pairs per distinct block and 8 slots
+//              per pose, and the element REDs per build fall from 246 M (one per pair and slot) to 83 M.  512-slot tiles
+//              (4.2 pairs per block, 48 M REDs) measured slower on the H100: one CTA per SM, and 128 registers at 512 threads.
 // FP64 throughout: lambda0 ~ 1e-4 m^2 is a difference of O(1e4) m^2 terms (P/N - vbar vbar^T).
 #pragma once
 #include "common.cuh"
 #include "envelope.cuh"
+#include "lidar_tiles.h"
 
 namespace lvba {
 
-constexpr int kSlots = 128;            // slots (threads) per batch CTA
-constexpr int kMaxVoxPerBatch = 64;    // K >= 2 per voxel  =>  <= kSlots/2 voxels per batch
+using tiles::kTileSlots;
+using tiles::kMaxVoxPerTile;
+constexpr int kSlots = 128;            // slots (threads) per batch CTA of the residual pass and of the visual kernels; the most poses a
+                                       // voxel of the tiles may have (more: lidar_big.h)
 constexpr int kStageStride = 37;       // visual build: doubles per slot in the staging buffer (36 + 1 pad: odd => no LDS.64 bank conflicts)
 constexpr int kLStage = 19;            // LiDAR build: 10 cluster values, then HALF a diagonal block (18 + 1 pad)
 constexpr int kFStride = 19;           // 18 factor doubles + 1 pad
@@ -35,14 +42,20 @@ constexpr int kVoxParams = 16;
 
 struct LidarView {
   int W;
-  int n_batches;
   const double2* cl;        // [5][nnz_pad] SoA pairs: (Pxx,Pxy) (Pxz,Pyy) (Pyz,Pzz) (vx,vy) (vz,N)
   long long nnz_pad;
   const int* pidx;          // [nnz] pose index per slot
   const int* vox_ptr;       // [V_local+1] slot offsets
+  int n_batches;            // residual pass: batches of <= kSlots slots
   const int* batch_vox;     // [n_batches+1] voxel range per batch
-  const long long* batch_pair;  // [n_batches+1] pair range per batch
-  const unsigned* pairs;    // packed (li | lj<<8 | lv<<16), li<lj local slot ids, lv local voxel id
+  int n_tiles;              // Hessian build: tiles of <= kTileSlots slots (lidar_tiles.h)
+  const int* tile_vox;      // [n_tiles+1] voxel range per tile
+  const int64_t* tile_prun; // [n_tiles+1] pair runs of every tile
+  const int64_t* prun_ptr;  // run r = pairs[prun_ptr[r] .. prun_ptr[r+1]): the pose pairs of one H block
+  const unsigned* pairs;    // li | lj << 16, li < lj slots local to the tile
+  const int64_t* tile_drun; // [n_tiles+1] pose runs of every tile
+  const int64_t* drun_ptr;  // run r = dslot[drun_ptr[r] .. drun_ptr[r+1]): the slots of one pose
+  const unsigned* dslot;    // slots local to the tile; a tile's items are dslot[s0 .. s0 + ns)
 };
 
 struct SlotData {
@@ -156,25 +169,30 @@ lidar_residual_kernel(LidarView lv, const double* __restrict__ poses, double* __
 }
 
 // ------------------------------------------------------------------------------------------------
-// Hessian + gradient + residual build
-__global__ void __launch_bounds__(kSlots, 4)
+// Hessian + gradient + residual build: one CTA of kTileSlots threads per tile
+__global__ void __launch_bounds__(kTileSlots, 512 / kTileSlots)
 lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, double* __restrict__ H,
                    double* __restrict__ g, double* __restrict__ batch_res) {
+  constexpr int S = kTileSlots;
   extern __shared__ double sm[];
-  double* stage = sm;                                   // [kSlots][kLStage]
-  double* sF = stage + kSlots * kLStage;           // [kSlots][kFStride]
-  double* sG = sF + kSlots * kFStride;                  // [kSlots][6]
-  double* sV = sG + kSlots * 6;                         // [kMaxVoxPerBatch][kVoxParams]
-  double* red = sV + kMaxVoxPerBatch * kVoxParams;      // [32]
-  long long* sDiag = reinterpret_cast<long long*>(red + 32);   // [kSlots] element offset of the slot's diagonal block
-  long long* sRowRS = sDiag + kSlots;                   // [kSlots] envelope row_start of the slot's pose row
-  int* sPose = reinterpret_cast<int*>(sRowRS + kSlots); // [kSlots]
-  int* sRowFirst = sPose + kSlots;                      // [kSlots] envelope first[] of the slot's pose row
-  unsigned char* sVoxOf = reinterpret_cast<unsigned char*>(sRowFirst + kSlots);   // [kSlots]
+  double* stage = sm;                                   // [S][kLStage]
+  double* sF = stage + S * kLStage;                     // [S][kFStride]
+  double* sG = sF + S * kFStride;                       // [S][6]
+  double* sV = sG + S * 6;                              // [kMaxVoxPerTile][kVoxParams]
+  double* red = sV + kMaxVoxPerTile * kVoxParams;       // [32]
+  long long* sDiag = reinterpret_cast<long long*>(red + 32);   // [S] element offset of the slot's diagonal block
+  long long* sRowRS = sDiag + S;                        // [S] envelope row_start of the slot's pose row
+  int* sPose = reinterpret_cast<int*>(sRowRS + S);      // [S]
+  int* sRowFirst = sPose + S;                           // [S] envelope first[] of the slot's pose row
+  unsigned short* sVoxOf = reinterpret_cast<unsigned short*>(sRowFirst + S);   // [S] tile-local voxel of the slot
+  unsigned short* sDSlot = sVoxOf + S;                  // [S] the tile's slots grouped by pose
+  unsigned short* sDRun = sDSlot + S;                   // [S + 1] pose run r = sDSlot[sDRun[r] .. sDRun[r + 1])
 
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int v0 = lv.batch_vox[b], v1 = lv.batch_vox[b + 1], nv = v1 - v0;
+  const int v0 = lv.tile_vox[b], v1 = lv.tile_vox[b + 1], nv = v1 - v0;
   const int s0 = lv.vox_ptr[v0], ns = lv.vox_ptr[v1] - s0;
+  const int64_t d0 = lv.tile_drun[b];
+  const int nd = (int)(lv.tile_drun[b + 1] - d0);
 
   // ---- phase 1: load + transform
   SlotData s;
@@ -191,7 +209,9 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
     const int fr = env.first[pose];
     sRowRS[tid] = rs; sRowFirst[tid] = fr;
     sDiag[tid] = (rs + (pose - fr)) * 36;
+    sDSlot[tid] = (unsigned short)lv.dslot[s0 + tid];   // the tile's slot items are dslot[s0 .. s0 + ns), grouped by pose
   }
+  for (int r = tid; r <= nd; r += S) sDRun[r] = (unsigned short)(lv.drun_ptr[d0 + r] - s0);
   __syncthreads();
 
   // ---- phase 2: per voxel merge + eigen solve (bavoxel.hpp:97-110)
@@ -209,9 +229,9 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
     p[9] = 2.0 / (lam[0] - lam[1]);       // umumT weights, bavoxel.hpp:110
     p[10] = 2.0 / (lam[0] - lam[2]);
     p[11] = (double)(int)Nsum;            // int NN = sig.N, bavoxel.hpp:101
-    for (int q = lo; q < hi; ++q) sVoxOf[q] = (unsigned char)tid;
+    for (int q = lo; q < hi; ++q) sVoxOf[q] = (unsigned short)tid;
   }
-  const double tot = block_sum<kSlots>(lam0, red);   // contains __syncthreads
+  const double tot = block_sum<S>(lam0, red);   // contains __syncthreads
   if (tid == 0) batch_res[b] = tot;
   __syncthreads();
 
@@ -300,8 +320,8 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
     sf[15] = s3n * uk[0]; sf[16] = s3n * uk[1]; sf[17] = s3n * uk[2];
   }
 
-  // ---- phase 4a: flush diagonal blocks (two halves through the staging buffer: 18 doubles per slot keep the CTA at
-  //      55 kB of shared memory = 4 CTAs per SM) and gradients, 32 consecutive doubles per warp instruction
+  // ---- phase 4a: diagonal blocks and gradient rows, summed per pose of the tile (nd runs) and written with one RED per
+  //      element.  The blocks go through the staging buffer in two halves of 18 doubles per slot.
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     __syncthreads();                                      // half 0: phase 2 is done with the clusters; half 1: flush 0 is done
@@ -311,47 +331,49 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
       for (int q = 0; q < 18; ++q) st[q] = Hb[18 * half + q];
     }
     __syncthreads();
-    for (int e = tid; e < ns * 18; e += kSlots) {
-      const int sl = e / 18, el = e - sl * 18;
-      atomicAdd(H + sDiag[sl] + 18 * half + el, stage[sl * kLStage + el]);
+    for (int e = tid; e < nd * 18; e += S) {
+      const int r = e / 18, el = e - r * 18;
+      const int qa = sDRun[r], qb = sDRun[r + 1];
+      double v = 0.0;
+      for (int q = qa; q < qb; ++q) v += stage[sDSlot[q] * kLStage + el];
+      atomicAdd(H + sDiag[sDSlot[qa]] + 18 * half + el, v);
     }
   }
-  for (int e = tid; e < ns * 6; e += kSlots) {
-    const int sl = e / 6, el = e - sl * 6;
-    atomicAdd(g + 6 * (long long)sPose[sl] + el, sG[e]);
+  for (int e = tid; e < nd * 6; e += S) {
+    const int r = e / 6, el = e - r * 6;
+    const int qa = sDRun[r], qb = sDRun[r + 1];
+    double v = 0.0;
+    for (int q = qa; q < qb; ++q) v += sG[sDSlot[q] * 6 + el];
+    atomicAdd(g + 6 * (long long)sPose[sDSlot[qa]] + el, v);
   }
 
-  // ---- phase 4b: off-diagonal blocks, 8 pairs (288 elements) per warp iteration.
-  // Lane (pq, k) = (lane >> 2, lane & 3) owns the elements 4 m + k, m = 0..8, of pair pq: every RED instruction of the warp
-  // writes one aligned 32-byte sector per pair (8 full sectors, as a linear mapping would), but a lane stays inside one pair,
-  // so its factors are read from shared memory once — 27 loads for 9 elements instead of 6 per element.  With el = 4 m + k,
-  // row = el / 6 and column = el % 6 depend on the lane only through k:
+  // ---- phase 4b: off-diagonal blocks.  The tile's pose pairs come grouped by destination block (runs); every warp takes 8
+  // runs at a time, sums each block in registers over the pairs of its run and writes it with 9 REDs per lane.
+  // Lane (pq, k) = (lane >> 2, lane & 3) owns the elements 4 m + k, m = 0..8, of run pq: every RED instruction of the warp
+  // writes one aligned 32-byte sector per run (8 full sectors, as a linear mapping would), and a lane reads the 27 factor values
+  // of its 9 elements of a pair from shared memory once.  With el = 4 m + k, row = el / 6 and column = el % 6 depend on the
+  // lane only through k:
   //   m % 3 == 0: row 2j,                 column k
   //   m % 3 == 1: row 2j + (k >= 2),      column k < 2 ? 4 + k : k - 2
   //   m % 3 == 2: row 2j + 1,             column 2 + k                      (j = m / 3)
   // so the three columns sit in registers indexed by m % 3 (compile time) and the row of the middle case is a select.
-  const long long p0 = lv.batch_pair[b], np = lv.batch_pair[b + 1] - p0;
+  const int64_t r0 = lv.tile_prun[b], nr = lv.tile_prun[b + 1] - r0;
   const int pq = lane >> 2, k = lane & 3;
   const bool hi = k >= 2;
   const int col0 = k, col1 = hi ? k - 2 : 4 + k, col2 = 2 + k;
-  unsigned code_next = 0;
-  {
-    const long long c0 = (long long)warp * 8;
-    if (c0 + pq < np) code_next = lv.pairs[p0 + c0 + pq];
-  }
-  for (long long c = (long long)warp * 8; c < np; c += (kSlots / 32) * 8) {
-    const bool live = c + pq < np;
-    const unsigned code = code_next;
-    {                                                     // prefetch the next chunk's pair codes
-      const long long cn = c + (kSlots / 32) * 8;
-      code_next = (cn + pq < np) ? lv.pairs[p0 + cn + pq] : 0u;
-    }
-    if (live) {
-      const int li = code & 0xff, lj = (code >> 8) & 0xff;
-      // lower-triangle block: row = larger pose (slot lj, ascending order inside a voxel), col = slot li
-      double* dst = H + (sRowRS[lj] + (sPose[li] - sRowFirst[lj])) * 36 + k;
-      const double* fi = sF + li * kFStride;               // column factors
-      const double* fj = sF + lj * kFStride;               // row factors
+  for (int64_t c = (int64_t)warp * 8; c < nr; c += (S / 32) * 8) {
+    if (c + pq >= nr) continue;
+    const int64_t qa = lv.prun_ptr[r0 + c + pq], qb = lv.prun_ptr[r0 + c + pq + 1];
+    unsigned code = lv.pairs[qa];
+    // lower-triangle block: row = larger pose (slot lj, ascending order inside a voxel), col = slot li
+    double* dst = H + (sRowRS[code >> 16] + (sPose[code & 0xffff] - sRowFirst[code >> 16])) * 36 + k;
+    double acc[9];
+#pragma unroll
+    for (int m = 0; m < 9; ++m) acc[m] = 0.0;
+    for (int64_t q = qa; q < qb; ++q) {
+      const unsigned code_next = q + 1 < qb ? lv.pairs[q + 1] : 0u;
+      const double* fi = sF + (code & 0xffff) * kFStride;   // column factors
+      const double* fj = sF + (code >> 16) * kFStride;      // row factors
       double ci[3][3], rj[6][3];
 #pragma unroll
       for (int t = 0; t < 3; ++t) { ci[0][t] = fi[6 * t + col0]; ci[1][t] = fi[6 * t + col1]; ci[2][t] = fi[6 * t + col2]; }
@@ -362,21 +384,24 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
 #pragma unroll
       for (int m = 0; m < 9; ++m) {
         const int j2 = 2 * (m / 3), ph = m % 3;
-        double r0, r1, r2;
-        if (ph == 0) { r0 = rj[j2][0]; r1 = rj[j2][1]; r2 = rj[j2][2]; }
-        else if (ph == 2) { r0 = rj[j2 + 1][0]; r1 = rj[j2 + 1][1]; r2 = rj[j2 + 1][2]; }
-        else { r0 = hi ? rj[j2 + 1][0] : rj[j2][0]; r1 = hi ? rj[j2 + 1][1] : rj[j2][1]; r2 = hi ? rj[j2 + 1][2] : rj[j2][2]; }
-        const double val = -(ci[ph][0] * r0 + ci[ph][1] * r1 + ci[ph][2] * r2);
-        atomicAdd(dst + 4 * m, val);
+        double x0, x1, x2;
+        if (ph == 0) { x0 = rj[j2][0]; x1 = rj[j2][1]; x2 = rj[j2][2]; }
+        else if (ph == 2) { x0 = rj[j2 + 1][0]; x1 = rj[j2 + 1][1]; x2 = rj[j2 + 1][2]; }
+        else { x0 = hi ? rj[j2 + 1][0] : rj[j2][0]; x1 = hi ? rj[j2 + 1][1] : rj[j2][1]; x2 = hi ? rj[j2 + 1][2] : rj[j2][2]; }
+        acc[m] -= ci[ph][0] * x0 + ci[ph][1] * x1 + ci[ph][2] * x2;
       }
+      code = code_next;
     }
+#pragma unroll
+    for (int m = 0; m < 9; ++m) atomicAdd(dst + 4 * m, acc[m]);
   }
 }
 
 constexpr size_t lidar_build_smem_bytes() {
-  return sizeof(double) * (kSlots * kLStage + kSlots * kFStride + kSlots * 6 + kMaxVoxPerBatch * kVoxParams + 32)
-       + sizeof(long long) * 2 * kSlots + sizeof(int) * 2 * kSlots + kSlots /*u8*/ + 64;
+  return sizeof(double) * (kTileSlots * (kLStage + kFStride + 6) + kMaxVoxPerTile * kVoxParams + 32)
+       + sizeof(long long) * 2 * kTileSlots + sizeof(int) * 2 * kTileSlots + sizeof(unsigned short) * (3 * kTileSlots + 1) + 64;
 }
+static_assert(lidar_build_smem_bytes() <= 227 * 1024, "lidar_build_kernel: shared memory above the 227 kB an H100 CTA may hold");
 
 // ------------------------------------------------------------------------------------------------
 // small LM helpers

@@ -5,9 +5,10 @@
 #include <unordered_set>
 
 #include "runtime.cuh"   // (pulls comm.cuh in)
+#include "exec.cuh"
 #include "lidar.cuh"
 #include "lidar_big.h"
-#include "runtime.cuh"
+#include "lidar_tiles.h"
 
 namespace lvba {
 
@@ -21,7 +22,7 @@ __global__ void lidar_aos_to_soa_kernel(long long nnz, long long nnz_pad, const 
 }
 
 // ---- batched window BA (LvbaSystem::runWindowBA, reference src/lvba_system.cpp:232-302): per-window reductions.
-// One CTA per window; ranges are contiguous because batches and poses are ordered by window.
+// One CTA per window; ranges are contiguous because tiles, batches and poses are ordered by window.
 __global__ void lidar_group_sum_kernel(const double* __restrict__ part, const int* __restrict__ rng /*[G+1]*/, double* __restrict__ out, int slot) {
   __shared__ double red[32];
   const int g = blockIdx.x;
@@ -60,20 +61,23 @@ __global__ void lidar_select_poses_kernel(int W, const int* __restrict__ pose_gr
   if (i < 12 * W && accept[pose_grp[i / 12]]) poses[i] = trial[i];
 }
 
-// sharded problems: the rank's slots are scattered through the caller's array; the whole array goes up in ONE copy
-// and the kernel picks the owned slots (src[i] = global slot of local slot i)
-__global__ void lidar_aos_to_soa_gather_kernel(long long nnz, long long nnz_pad, const double* __restrict__ aos,
-                                               const int* __restrict__ src, double2* __restrict__ soa) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= nnz) return;
-  const double2* r = reinterpret_cast<const double2*>(aos + 10 * (long long)src[i]);
+// the local voxel order is not the caller's (voxels ordered by lowest pose, or a shard's share): the caller's records and pose
+// indices are on the device as they are, and every local slot w picks its own.  Local voxel i of w by binary search in the
+// local CSR; slot0[i] = its first slot in the caller's arrays.
+__global__ void lidar_gather_slots_kernel(long long nnz, long long nnz_pad, int n_vox, const int* __restrict__ l_vox_ptr,
+                                          const int* __restrict__ slot0, const int* __restrict__ caller_pidx,
+                                          const double* __restrict__ aos, int* __restrict__ pidx, double2* __restrict__ soa) {
+  const long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (w >= nnz) return;
+  int lo = 0, hi = n_vox;
+  while (hi - lo > 1) { const int m = (lo + hi) >> 1; if (l_vox_ptr[m] <= w) lo = m; else hi = m; }
+  const long long q = slot0[lo] + (w - l_vox_ptr[lo]);
+  pidx[w] = caller_pidx[q];
+  const double2* r = reinterpret_cast<const double2*>(aos + 10 * q);
 #pragma unroll
-  for (int q = 0; q < 5; ++q) soa[q * nnz_pad + i] = r[q];
+  for (int k = 0; k < 5; ++k) soa[k * nnz_pad + w] = r[k];
 }
 
-// Pair table of the Hessian build (one word per pose pair of every voxel: li | lj << 8 | lv << 16), generated on the
-// device from the voxel CSR: thread = local slot x of the batch, it writes the pairs (x, y), y > x, of its voxel in the
-// order the build kernel walks them.  (5.2 M words for config C: 6 ms of host loops + a 21 MB upload otherwise.)
 // out[i] = aos[src[i]]   (10-double cluster records)
 __global__ void lidar_gather_aos_kernel(long long n, const int* __restrict__ src, const double* __restrict__ aos, double* __restrict__ out) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -83,39 +87,13 @@ __global__ void lidar_gather_aos_kernel(long long n, const int* __restrict__ src
   for (int k = 0; k < 10; ++k) out[10 * i + k] = a[k];
 }
 
-__global__ void __launch_bounds__(kSlots)
-lidar_pairs_kernel(int n_batches, const int* __restrict__ vox_ptr, const int* __restrict__ batch_vox,
-                   const long long* __restrict__ batch_pair, unsigned* __restrict__ pairs) {
-  __shared__ long long off[kMaxVoxPerBatch + 1];
-  __shared__ int vlo[kMaxVoxPerBatch + 1];
-  const int b = blockIdx.x;
-  const int v0 = batch_vox[b], v1 = batch_vox[b + 1], sbase = vox_ptr[v0];
-  if (threadIdx.x == 0) {
-    long long o = batch_pair[b];
-    for (int i = 0; i < v1 - v0; ++i) {
-      const int lo = vox_ptr[v0 + i] - sbase, K = vox_ptr[v0 + i + 1] - vox_ptr[v0 + i];
-      off[i] = o; vlo[i] = lo;
-      o += (long long)K * (K - 1) / 2;
-    }
-    vlo[v1 - v0] = vox_ptr[v1] - sbase;
-  }
-  __syncthreads();
-  const int x = threadIdx.x;
-  if (x >= vlo[v1 - v0]) return;
-  int lv = 0;
-  while (vlo[lv + 1] <= x) ++lv;
-  const int lo = vlo[lv], hi = vlo[lv + 1], K = hi - lo, j = x - lo;
-  unsigned* dst = pairs + off[lv] + (long long)j * (K - 1) - (long long)j * (j - 1) / 2;
-  for (int y = x + 1; y < hi; ++y) *dst++ = (unsigned)x | ((unsigned)y << 8) | ((unsigned)lv << 16);
-}
-
 }  // namespace lvba
 
 struct lvba_lidar_problem {
   int W = 0;
   long long V_total = 0;          // voxels of the whole problem (the AVG_THR divisor, bavoxel.hpp:635)
   long long V_local = 0, nnz_local = 0, n_pairs = 0;
-  int n_batches = 0;
+  int n_batches = 0, n_tiles = 0;
   int device = 0;
   // host copies kept for counters / structure queries
   std::vector<long long> h_vox_ptr_all;
@@ -123,9 +101,8 @@ struct lvba_lidar_problem {
   bool have_structure = false;
   cudaStream_t stream = nullptr;
   lvba::DevBuf<double2> cl;
-  lvba::DevBuf<int> pidx, vox_ptr, batch_vox;
-  lvba::DevBuf<long long> batch_pair;
-  lvba::DevBuf<unsigned> pairs;
+  lvba::DevBuf<int> pidx, vox_ptr, batch_vox, tile_vox;
+  lvba::tiles::Runs<lvba::CudaExec> prun, drun;   // the build's destination table: pose pairs by H block, slots by pose
   lvba::DevBuf<double> poses, poses0, trial, H, g, diag, dadd, dx, batch_res, scal;
   lvba::Envelope env;
   lvba::EnvSolver solver;
@@ -143,7 +120,7 @@ struct lvba_lidar_problem {
   int n_groups = 0;
   std::vector<int> grp_ptr;            // [G+1] pose offsets
   std::vector<long long> grp_V;        // voxels per window (AVG_THR divisor of each window)
-  lvba::DevBuf<int> d_grp_ptr, d_pose_grp, d_grp_batch, d_accept;
+  lvba::DevBuf<int> d_grp_ptr, d_pose_grp, d_grp_batch, d_grp_tile, d_accept;   // d_grp_batch / d_grp_tile: batch / tile range per window
   lvba::DevBuf<double> d_u_grp, d_grp_scal;
   double* h_grp_scal = nullptr;        // pinned [4G]: r1 sum, q1, bad flag, r2 sum per window
   size_t h_grp_scal_bytes = 0;
@@ -158,9 +135,12 @@ struct lvba_lidar_problem {
 
   lvba::LidarView view() const {
     lvba::LidarView v_;
-    v_.W = W; v_.n_batches = n_batches; v_.cl = cl.p; v_.nnz_pad = (long long)(cl.n / 5);
-    v_.pidx = pidx.p; v_.vox_ptr = vox_ptr.p; v_.batch_vox = batch_vox.p; v_.batch_pair = batch_pair.p;
-    v_.pairs = pairs.p;
+    v_.W = W; v_.cl = cl.p; v_.nnz_pad = (long long)(cl.n / 5);
+    v_.pidx = pidx.p; v_.vox_ptr = vox_ptr.p;
+    v_.n_batches = n_batches; v_.batch_vox = batch_vox.p;
+    v_.n_tiles = n_tiles; v_.tile_vox = tile_vox.p;
+    v_.tile_prun = prun.tile_run.p; v_.prun_ptr = prun.run_ptr.p; v_.pairs = prun.code.p;
+    v_.tile_drun = drun.tile_run.p; v_.drun_ptr = drun.run_ptr.p; v_.dslot = drun.code.p;
     return v_;
   }
   ~lvba_lidar_problem() {
@@ -299,37 +279,28 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
 
   // ---- shard: voxel -> owner of its lowest pose index (SURVEY.md §8e)
   Comm& cm = comm();
-  bool sorted_voxels = false;
-  std::vector<int64_t> mine;
-  if (!cm.active()) {                                          // one rank: every voxel, in the caller's order
-    mine.resize((size_t)V);
-    for (int64_t a = 0; a < V; ++a) mine[(size_t)a] = a;        // ~0.1 ms at 200 k voxels: cheaper than waking the helpers
-  } else {
-    mine.reserve((size_t)V);
+  // the voxels this rank holds (all of them on one rank: `owned` stays empty and stands for 0..V-1)
+  std::vector<int64_t> owned;
+  const bool sharded = cm.active();
+  if (sharded) {
+    owned.reserve((size_t)V);
     for (int64_t a = 0; a < V; ++a)
       if ((P->solver.dist() ? P->solver.dist_owner(pose_idx[vox_ptr[a]]) : shard_owner(pose_idx[vox_ptr[a]], W, cm.n_ranks)) == cm.rank)
-        mine.push_back(a);
+        owned.push_back(a);
   }
-  {
-    // voxels in the order of their lowest pose: a batch CTA then touches ~30 consecutive pose rows of H (its diagonal blocks and
-    // gradient rows can be reduced per pose before they leave the SM, and its REDs stay inside a few hundred kB of L2)
-    const char* sv = getenv("LVBA_SORT_VOXELS");
-    sorted_voxels = n_groups == 0 && sv && sv[0] == '1';
-    if (sorted_voxels)
-      std::stable_sort(mine.begin(), mine.end(), [&](int64_t x, int64_t y) { return pose_idx[vox_ptr[x]] < pose_idx[vox_ptr[y]]; });
-  }
-  if (n_groups > 0)      // windows in order: batches and their partial sums become contiguous per window
-    std::stable_sort(mine.begin(), mine.end(), [&](int64_t x, int64_t y) { return pose_grp[pose_idx[vox_ptr[x]]] < pose_grp[pose_idx[vox_ptr[y]]]; });
-  // voxels seen from more than kSlots poses do not fit a batch CTA: they leave `mine` and take the passes of lidar_big.h
+  // voxels seen from more than kSlots poses do not fit a batch CTA: they leave `owned` and take the passes of lidar_big.h
   std::vector<int64_t> bigv;
   {
-    std::vector<int64_t> small;
+    const int64_t n_own = sharded ? (int64_t)owned.size() : V;
     bool has_big = false;
-    for (size_t i = 0; i < mine.size() && !has_big; ++i) has_big = vox_ptr[mine[i] + 1] - vox_ptr[mine[i]] > kSlots;
-    if (has_big) for (int64_t a : mine) if (vox_ptr[a + 1] - vox_ptr[a] > kSlots) bigv.push_back(a);
-    if (!bigv.empty()) {
-      for (int64_t a : mine) if (vox_ptr[a + 1] - vox_ptr[a] <= kSlots) small.push_back(a);
-      mine.swap(small);
+    for (int64_t j = 0; j < n_own && !has_big; ++j) { const int64_t a = sharded ? owned[j] : j; has_big = vox_ptr[a + 1] - vox_ptr[a] > kSlots; }
+    if (has_big) {
+      std::vector<int64_t> small;
+      for (int64_t j = 0; j < n_own; ++j) {
+        const int64_t a = sharded ? owned[j] : j;
+        (vox_ptr[a + 1] - vox_ptr[a] > kSlots ? bigv : small).push_back(a);
+      }
+      owned.swap(small);
     }
     // the batched window LM (lidar_batch_lm_impl) has no big-voxel passes: such a voxel would silently drop out of H, g and the
     // residual sums while still counting in the AVG_THR divisor.  A window holds <= 31 poses (prepare_batch), so this cannot
@@ -338,30 +309,38 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
       return fail(LVBA_ERR_UNSUPPORTED, "batched window BA: voxel %lld is seen from %lld poses (more than %d)", (long long)bigv[0],
                   (long long)(vox_ptr[bigv[0] + 1] - vox_ptr[bigv[0]]), kSlots);
   }
-  const int64_t Vl = (int64_t)mine.size();
-  std::vector<int> l_vox_ptr(Vl + 1, 0);
-  for (int64_t i = 0; i < Vl; ++i) l_vox_ptr[i + 1] = l_vox_ptr[i] + (int)(vox_ptr[mine[i] + 1] - vox_ptr[mine[i]]);
-  const long long nnz = l_vox_ptr[Vl];
-  P->V_local = Vl; P->nnz_local = nnz;
-
-  // ---- batches of consecutive voxels, <= kSlots slots and <= kMaxVoxPerBatch voxels each
-  std::vector<int> batch_vox{0};
-  {
-    int ns = 0, nv = 0;
-    for (int64_t i = 0; i < Vl; ++i) {
-      const int K = l_vox_ptr[i + 1] - l_vox_ptr[i];
-      const bool new_grp = n_groups > 0 && i > 0 && pose_grp[pose_idx[vox_ptr[mine[i]]]] != pose_grp[pose_idx[vox_ptr[mine[i - 1]]]];
-      if (nv > 0 && (ns + K > kSlots || nv + 1 > kMaxVoxPerBatch || new_grp)) { batch_vox.push_back((int)i); ns = 0; nv = 0; }
-      ns += K; ++nv;
-    }
-    if (Vl > 0) batch_vox.push_back((int)Vl);
+  const bool all = !sharded && bigv.empty();
+  // voxels in the order of their lowest pose: the voxels of a build tile then share pose pairs, whose H blocks the tile sums on
+  // chip (lidar_tiles.h); the windows of the batched window BA, consecutive pose ranges, come out contiguous and in order
+  std::vector<int> slot0, l_vox_ptr;                           // first caller slot / first local slot of every local voxel
+  const int64_t Vl = all ? V : (int64_t)owned.size();
+  const long long nnz = tiles::order_by_lowest_pose(W, all ? nullptr : owned.data(), Vl, vox_ptr, pose_idx, slot0, l_vox_ptr);
+  bool identity = all;                                         // the caller's voxels, in the caller's order
+  long long np = 0;                                            // pose pairs
+  for (int64_t i = 0; i < Vl; ++i) {
+    const long long K = l_vox_ptr[i + 1] - l_vox_ptr[i];
+    np += K * (K - 1) / 2;
+    identity = identity && slot0[i] == l_vox_ptr[i];
   }
+  P->V_local = Vl; P->nnz_local = nnz; P->n_pairs = np;
+
+  // ---- residual batches (<= kSlots slots) and build tiles (<= kTileSlots slots): consecutive voxels, never across a window
+  std::vector<int> vox_grp(n_groups > 0 ? (size_t)Vl : (size_t)0);
+  for (int64_t i = 0; i < (int64_t)vox_grp.size(); ++i) vox_grp[i] = pose_grp[pose_idx[slot0[i]]];
+  const int* grp = n_groups > 0 ? vox_grp.data() : nullptr;
+  const std::vector<int> batch_vox = tiles::cut_ranges(Vl, l_vox_ptr.data(), grp, kSlots, kSlots);
+  const std::vector<int> tile_vox = tiles::cut_ranges(Vl, l_vox_ptr.data(), grp, kTileSlots, kMaxVoxPerTile);
   P->n_batches = (int)batch_vox.size() - 1;
+  P->n_tiles = (int)tile_vox.size() - 1;
   if (n_groups > 0) {
-    std::vector<int> grp_batch((size_t)n_groups + 1, 0);       // batch range of every window
-    for (int b = 0; b < P->n_batches; ++b) ++grp_batch[pose_grp[pose_idx[vox_ptr[mine[batch_vox[b]]]]] + 1];
-    for (int g = 0; g < n_groups; ++g) grp_batch[g + 1] += grp_batch[g];
-    LVBA_TRY(P->d_grp_batch.upload(grp_batch, s, &P->h2d));
+    auto per_window = [&](const std::vector<int>& cut) {      // range of batches / tiles of every window
+      std::vector<int> r((size_t)n_groups + 1, 0);
+      for (size_t k = 0; k + 1 < cut.size(); ++k) ++r[(size_t)vox_grp[cut[k]] + 1];
+      for (int g = 0; g < n_groups; ++g) r[g + 1] += r[g];
+      return r;
+    };
+    LVBA_TRY(P->d_grp_batch.upload(per_window(batch_vox), s, &P->h2d));
+    LVBA_TRY(P->d_grp_tile.upload(per_window(tile_vox), s, &P->h2d));
     LVBA_TRY(P->d_grp_ptr.upload(P->grp_ptr, s, &P->h2d));
     LVBA_TRY(P->d_pose_grp.upload(pose_grp, s, &P->h2d));
     LVBA_TRY(P->d_accept.alloc((size_t)n_groups));
@@ -372,48 +351,30 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
     LVBA_TRY(pinned_pool().take(P->h_grp_scal_bytes, (void**)&P->h_grp_scal));
     LVBA_CUDA(cudaStreamSynchronize(s));                       // local vectors
   }
-  // ---- pair table
-  std::vector<long long> batch_pair(P->n_batches + 1, 0);
-  parallel_chunks(P->n_batches, 1 << 10, [&](int64_t b0, int64_t b1, int) {
-    for (int64_t b = b0; b < b1; ++b) {
-      long long c = 0;
-      for (int i = batch_vox[(size_t)b]; i < batch_vox[(size_t)b + 1]; ++i) {
-        const long long K = l_vox_ptr[i + 1] - l_vox_ptr[i];
-        c += K * (K - 1) / 2;
-      }
-      batch_pair[(size_t)b + 1] = c;
-    }
-  });
-  for (int b = 0; b < P->n_batches; ++b) batch_pair[b + 1] += batch_pair[b];
-  const long long np = batch_pair[P->n_batches];
-  P->n_pairs = np;
 
-  lap("batches+pair table");
+  lap("order+batches+tiles");
   // ---- upload.  Clusters: the caller's AoS records go up in ONE copy and are transposed to the SoA double2 layout
-  //      by a kernel (which also picks the owned slots when the problem is sharded or window-sorted).
+  //      by a kernel (which also picks the slots in the local voxel order unless that is the caller's).
   const long long nnz_pad = ((nnz + 31) / 32) * 32 + 32;
   LVBA_TRY(P->cl.alloc((size_t)5 * nnz_pad));
   LVBA_TRY(P->cl.zero(s));
-  const bool contiguous = Vl == V && n_groups == 0 && !sorted_voxels;       // single rank, caller's order: the records and pose indices are used as they are
-  std::vector<int> l_pidx(contiguous ? (size_t)0 : (size_t)nnz);
+  LVBA_TRY(P->vox_ptr.upload(l_vox_ptr, s, &P->h2d));
   if (lane.done) LVBA_CUDA(cudaStreamWaitEvent(s, lane.done, 0));            // the kernels below read the records
   {
-    if (contiguous) {
+    if (identity) {
       if (nnz > 0) {
         lidar_aos_to_soa_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(nnz, nnz_pad, aos_dev, P->cl.p);
         ++P->launches;
       }
     } else {
-      // a shard (or a window-sorted batch) owns scattered voxels: the ONE copy of the caller's array + a device-side gather
-      // (one copy per run of contiguous voxels would mean ~100k small copies on a 2-rank split of config C)
-      std::vector<int> src((size_t)nnz);
-      long long w = 0;
-      for (int64_t i = 0; i < Vl; ++i)
-        for (int64_t q = vox_ptr[mine[i]]; q < vox_ptr[mine[i] + 1]; ++q, ++w) { src[w] = (int)q; l_pidx[w] = pose_idx[q]; }
-      DevBuf<int> d_src;
+      // reordered (or a shard's scattered) voxels: the ONE copy of the caller's records and pose indices + a device-side gather
+      DevBuf<int> d_slot0, d_caller_pidx;
       if (nnz > 0) {
-        LVBA_TRY(d_src.upload(src, s, &P->h2d));
-        lidar_aos_to_soa_gather_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(nnz, nnz_pad, aos_dev, d_src.p, P->cl.p);
+        LVBA_TRY(d_slot0.upload(slot0, s, &P->h2d));
+        LVBA_TRY(d_caller_pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)vox_ptr[V], s, &P->h2d));
+        LVBA_TRY(P->pidx.alloc((size_t)nnz));
+        lidar_gather_slots_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(nnz, nnz_pad, (int)Vl, P->vox_ptr.p, d_slot0.p, d_caller_pidx.p,
+                                                                                aos_dev, P->pidx.p, P->cl.p);
         ++P->launches;
       }
       if (!bigv.empty()) {                   // the big voxels' records stay AoS (lidar_big.h reads them slot by slot)
@@ -439,21 +400,29 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
         ++P->launches;
         LVBA_CUDA(cudaStreamSynchronize(s)); // the host vectors and d_bsrc go out of scope
       }
-      LVBA_CUDA(cudaStreamSynchronize(s));   // src and d_src are freed on scope exit
+      LVBA_CUDA(cudaStreamSynchronize(s));   // d_slot0 and d_caller_pidx are freed on scope exit
     }
   }
   if (tlog) { cudaStreamSynchronize(s); } lap("cluster upload+SoA");
   static_assert(sizeof(int) == sizeof(int32_t), "pose_idx is uploaded as it is");
-  if (contiguous) LVBA_TRY(P->pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)nnz, s, &P->h2d));
-  else LVBA_TRY(P->pidx.upload(l_pidx, s, &P->h2d));
-  LVBA_TRY(P->vox_ptr.upload(l_vox_ptr, s, &P->h2d));
+  if (identity) LVBA_TRY(P->pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)nnz, s, &P->h2d));
   LVBA_TRY(P->batch_vox.upload(batch_vox, s, &P->h2d));
-  LVBA_TRY(P->batch_pair.upload(batch_pair, s, &P->h2d));
-  if (np > 0) {                                                // pair table: generated on the device from the CSR just uploaded
-    LVBA_TRY(P->pairs.alloc((size_t)np));
-    lidar_pairs_kernel<<<P->n_batches, kSlots, 0, s>>>(P->n_batches, P->vox_ptr.p, P->batch_vox.p, P->batch_pair.p, P->pairs.p);
-    ++P->launches;
+  LVBA_TRY(P->tile_vox.upload(tile_vox, s, &P->h2d));
+  if (P->n_tiles > 0) {                                        // destination table of the build, on the device from the CSR just uploaded
+    CudaExec ex;
+    ex.stream = s;
+    DevBuf<long long> d_pair_cnt, d_vox_pair;                  // pose pairs before every local voxel
+    LVBA_TRY(d_pair_cnt.alloc((size_t)Vl + 1));
+    LVBA_TRY(d_vox_pair.alloc((size_t)Vl + 1));
+    LVBA_TRY(ex.for_each(Vl + 1, tiles::PairCountF{P->vox_ptr.p, Vl, d_pair_cnt.p}));
+    LVBA_TRY(ex.exclusive_scan(d_pair_cnt.p, d_vox_pair.p, Vl + 1));
+    const tiles::TableIn tin{P->n_tiles, W, P->env.nblocks, P->tile_vox.p, P->vox_ptr.p, P->pidx.p, d_vox_pair.p,
+                             P->env.d_first.p, P->env.d_row_start.p};
+    LVBA_TRY(tiles::build_runs(ex, tin, /*by_slot=*/false, np, P->prun));
+    LVBA_TRY(tiles::build_runs(ex, tin, /*by_slot=*/true, nnz, P->drun));
+    P->launches += ex.launches;
   }
+  lap("destination table");
   LVBA_TRY(P->poses.upload(poses, (size_t)W * 12, s, &P->h2d));
   LVBA_TRY(P->poses0.upload(poses, (size_t)W * 12, s));
   LVBA_TRY(P->trial.alloc((size_t)W * 12));
@@ -462,7 +431,7 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   LVBA_TRY(P->diag.alloc((size_t)W * 6));
   LVBA_TRY(P->dadd.alloc((size_t)W * 6));
   LVBA_TRY(P->dx.alloc((size_t)W * 6));
-  LVBA_TRY(P->batch_res.alloc((size_t)std::max<long long>(P->n_batches + P->n_big, 1)));
+  LVBA_TRY(P->batch_res.alloc((size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1)));
   LVBA_TRY(P->scal.alloc(8));
   LVBA_TRY(P->scal.zero(s));
   LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
@@ -475,9 +444,10 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   return LVBA_OK;
 }
 
-// voxels seen from more than kSlots poses (lidar_big.h): lambda_0 of voxel b -> batch_res[n_batches + b]; with the Hessian,
-// their gradient / diagonal-block / pair-block contributions are added to g and H by atomics
-inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool residual_only) {
+// voxels seen from more than kSlots poses (lidar_big.h): lambda_0 of voxel b -> batch_res[n_before + b] (after the partials of
+// the tiles or batches); with the Hessian, their gradient / diagonal-block / pair-block contributions are added to g and H by
+// atomics
+inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool residual_only, int n_before) {
   cudaStream_t s = P->stream;
   const big::View bv = P->big_view();
   auto launch = [&](int64_t items, const auto& f) {
@@ -485,7 +455,7 @@ inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool r
     env_wide_pass_kernel<<<grid, 128, 0, s>>>(items, f);
     ++P->launches;
   };
-  launch((int64_t)P->n_big, big::ParamsF{bv, d_poses, P->big_params.p, P->batch_res.p + P->n_batches});
+  launch((int64_t)P->n_big, big::ParamsF{bv, d_poses, P->big_params.p, P->batch_res.p + n_before});
   if (!residual_only) {
     launch((int64_t)P->n_big_slots, big::SlotsF{bv, d_poses, P->big_params.p, P->big_feat.p, P->H.p, P->g.p});
     launch((int64_t)P->n_big_pairs, big::PairsF{bv, P->big_params.p, P->big_feat.p, P->H.p});
@@ -499,12 +469,12 @@ inline int lidar_build_dev(lvba_lidar_problem* P, const double* d_poses, int slo
   cudaStream_t s = P->stream;
   LVBA_TRY(P->H.zero(s));
   LVBA_TRY(P->g.zero(s));
-  if (P->n_batches > 0) {
-    lidar_build_kernel<<<P->n_batches, kSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->H.p, P->g.p, P->batch_res.p);
+  if (P->n_tiles > 0) {
+    lidar_build_kernel<<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->H.p, P->g.p, P->batch_res.p);
     ++P->launches;
   }
-  if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/false));
-  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_res.p, (int)(P->n_batches + P->n_big), P->scal.p + slot);
+  if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/false, P->n_tiles));
+  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_res.p, (int)(P->n_tiles + P->n_big), P->scal.p + slot);
   ++P->launches;
   LVBA_CUDA(cudaGetLastError());
   Comm& cm = comm();
@@ -525,7 +495,7 @@ inline int lidar_residual_dev(lvba_lidar_problem* P, const double* d_poses, int 
     lidar_residual_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), d_poses, P->batch_res.p);
     ++P->launches;
   }
-  if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/true));
+  if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/true, P->n_batches));
   reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_res.p, (int)(P->n_batches + P->n_big), P->scal.p + slot);
   ++P->launches;
   LVBA_CUDA(cudaGetLastError());
@@ -663,11 +633,11 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
     P->timers.begin(PH_BUILD);
     LVBA_TRY(P->H.zero(s));
     LVBA_TRY(P->g.zero(s));
-    if (P->n_batches > 0) {
-      lidar_build_kernel<<<P->n_batches, kSlots, lidar_build_smem_bytes(), s>>>(P->view(), ev, P->poses.p, P->H.p, P->g.p, P->batch_res.p);
+    if (P->n_tiles > 0) {
+      lidar_build_kernel<<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), ev, P->poses.p, P->H.p, P->g.p, P->batch_res.p);
       ++P->launches;
     }
-    lidar_group_sum_kernel<<<G, 128, 0, s>>>(P->batch_res.p, P->d_grp_batch.p, P->d_grp_scal.p, 0);
+    lidar_group_sum_kernel<<<G, 128, 0, s>>>(P->batch_res.p, P->d_grp_tile.p, P->d_grp_scal.p, 0);
     ++P->launches;
     P->timers.end();
     ++P->builds;

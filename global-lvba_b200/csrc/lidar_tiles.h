@@ -1,0 +1,179 @@
+// lidar_tiles.h — voxel order, tiles and destination table of the LiDAR Hessian build (lidar_build_kernel, lidar.cuh).
+//
+// The build sums every distinct H block and gradient row of a tile on chip and writes it with one RED per element, so the
+// RED count falls with the number of voxels of a tile that share a pose pair.  Three pieces set that up once per structure:
+//   * order_by_lowest_pose: the voxels in the order of their lowest pose (stable counting sort, O(V + W)).  Neighbouring
+//     voxels then share poses, and windows of the batched window BA (consecutive pose ranges) come out contiguous.
+//   * cut_ranges: consecutive voxels into tiles of <= max_slots slots and <= max_vox voxels, never across a window.
+//   * build_runs: per tile, the (slot i, slot j) pose pairs grouped by destination H block, and the slots grouped by pose
+//     (diagonal blocks and gradient rows).  Functors over items run by an execution policy: CudaExec (exec.cuh) in the
+//     library, the host policy of tests/emu in the CPU tests.
+#pragma once
+#include <math.h>
+#include <stdint.h>
+
+#include <vector>
+
+#if defined(__CUDACC__)
+#define LVBA_THD __host__ __device__ __forceinline__
+#else
+#define LVBA_THD inline
+#endif
+
+namespace lvba {
+namespace tiles {
+
+constexpr int kTileSlots = 256;              // slots (threads) per tile CTA of the Hessian build (faster than 512 on the H100)
+constexpr int kMaxVoxPerTile = kTileSlots / 2;
+
+// The voxels `in[0..n)` (all voxels 0..n-1 when `in` is null), stably ordered by their lowest pose index (pose_idx is ascending
+// inside a voxel), as a local CSR: slot0[i] = first slot of local voxel i in the caller's arrays, l_vox_ptr[i] = its first local
+// slot (l_vox_ptr has n + 1 entries).  Returns the number of slots.  Two sequential passes over the caller's CSR.
+inline int64_t order_by_lowest_pose(int W, const int64_t* in, int64_t n, const int64_t* vox_ptr, const int32_t* pose_idx,
+                                    std::vector<int>& slot0, std::vector<int>& l_vox_ptr) {
+  std::vector<int64_t> at((size_t)W + 1, 0);
+  for (int64_t j = 0; j < n; ++j) ++at[(size_t)pose_idx[vox_ptr[in ? in[j] : j]] + 1];
+  for (int r = 0; r < W; ++r) at[(size_t)r + 1] += at[(size_t)r];
+  slot0.resize((size_t)n); l_vox_ptr.assign((size_t)n + 1, 0);
+  for (int64_t j = 0; j < n; ++j) {
+    const int64_t a = in ? in[j] : j;
+    const size_t i = (size_t)at[(size_t)pose_idx[vox_ptr[a]]]++;
+    slot0[i] = (int)vox_ptr[a]; l_vox_ptr[i + 1] = (int)(vox_ptr[a + 1] - vox_ptr[a]);
+  }
+  for (int64_t i = 0; i < n; ++i) l_vox_ptr[(size_t)i + 1] += l_vox_ptr[(size_t)i];
+  return l_vox_ptr[(size_t)n];
+}
+
+// voxel ranges [r[k], r[k+1]) of consecutive voxels with <= max_slots slots and <= max_vox voxels each; with `grp` (window
+// of every voxel) a range never holds two windows.  A voxel has <= max_slots slots.
+inline std::vector<int> cut_ranges(int64_t V, const int* vox_ptr, const int* grp, int max_slots, int max_vox) {
+  std::vector<int> r{0};
+  int ns = 0, nv = 0;
+  for (int64_t i = 0; i < V; ++i) {
+    const int K = vox_ptr[i + 1] - vox_ptr[i];
+    const bool new_grp = grp && i > 0 && grp[i] != grp[i - 1];
+    if (nv > 0 && (ns + K > max_slots || nv + 1 > max_vox || new_grp)) { r.push_back((int)i); ns = 0; nv = 0; }
+    ns += K; ++nv;
+  }
+  if (V > 0) r.push_back((int)V);
+  return r;
+}
+
+struct TableIn {
+  int64_t n_tiles;
+  int W;
+  long long nblocks;            // blocks of the envelope
+  const int* tile_vox;          // [n_tiles + 1] voxel range of every tile
+  const int* vox_ptr;           // [V + 1] slot offsets (the tiles' voxel order)
+  const int* pidx;              // [nnz] pose of every slot
+  const long long* vox_pair;    // [V + 1] prefix sums of K (K - 1) / 2
+  const int* first;             // envelope first[] per pose row
+  const long long* row_start;   // envelope row_start[] per pose row
+};
+
+// items 0..V: cnt[i] = pose pairs of local voxel i (0 for i = V); its exclusive scan is TableIn::vox_pair
+struct PairCountF {
+  const int* vox_ptr; int64_t V; long long* cnt;
+  LVBA_THD void operator()(int64_t i) const {
+    const long long K = i < V ? vox_ptr[i + 1] - vox_ptr[i] : 0;
+    cnt[i] = K * (K - 1) / 2;
+  }
+};
+
+// one item per pose pair (i < j) of a voxel: key = (tile, lower-envelope block (pose_j, pose_i)), code = li | lj << 16 (slots
+// local to the tile)
+struct PairKeyF {
+  TableIn in; uint64_t* key; uint32_t* code;
+  LVBA_THD void operator()(int64_t p) const {
+    const TableIn& q = in;
+    int64_t t = 0, hi = q.n_tiles;                            // tile: the last one starting at or before p
+    while (hi - t > 1) { const int64_t m = (t + hi) >> 1; if (q.vox_pair[q.tile_vox[m]] <= p) t = m; else hi = m; }
+    int64_t a = q.tile_vox[t];                                // voxel: the last one of the tile starting at or before p
+    hi = q.tile_vox[t + 1];
+    while (hi - a > 1) { const int64_t m = (a + hi) >> 1; if (q.vox_pair[m] <= p) a = m; else hi = m; }
+    const int64_t r = p - q.vox_pair[a];                      // strict lower-triangular index: r = j (j - 1) / 2 + i, j > i
+    int64_t j = (int64_t)((sqrt(8.0 * (double)r + 1.0) + 1.0) * 0.5);
+    while (j * (j - 1) / 2 > r) --j;
+    while ((j + 1) * j / 2 <= r) ++j;
+    const int64_t i = r - j * (j - 1) / 2;
+    const int s0 = q.vox_ptr[q.tile_vox[t]];
+    const int si = q.vox_ptr[a] + (int)i, sj = q.vox_ptr[a] + (int)j;
+    const int pi = q.pidx[si], pj = q.pidx[sj];               // ascending inside a voxel: pi < pj
+    key[p] = (uint64_t)t * (uint64_t)q.nblocks + (uint64_t)(q.row_start[pj] + (pi - q.first[pj]));
+    code[p] = (uint32_t)(si - s0) | ((uint32_t)(sj - s0) << 16);
+  }
+};
+
+// one item per slot: key = (tile, pose), code = slot local to the tile
+struct SlotKeyF {
+  TableIn in; uint64_t* key; uint32_t* code;
+  LVBA_THD void operator()(int64_t s) const {
+    const TableIn& q = in;
+    int64_t t = 0, hi = q.n_tiles;
+    while (hi - t > 1) { const int64_t m = (t + hi) >> 1; if (q.vox_ptr[q.tile_vox[m]] <= s) t = m; else hi = m; }
+    key[s] = (uint64_t)t * (uint64_t)q.W + (uint64_t)q.pidx[s];
+    code[s] = (uint32_t)(s - q.vox_ptr[q.tile_vox[t]]);
+  }
+};
+
+// items 0..n: flag[p] = 1 where a run of equal keys starts (flag[n] = 0)
+struct RunFlagF {
+  const uint64_t* key; int64_t n; int64_t* flag;
+  LVBA_THD void operator()(int64_t p) const { flag[p] = (p < n && (p == 0 || key[p] != key[p - 1])) ? 1 : 0; }
+};
+// items 0..n: run_ptr[r] = first item of run r, run_ptr[R] = n
+struct RunStartF {
+  const int64_t* flag; const int64_t* pos; int64_t n; int64_t* run_ptr;
+  LVBA_THD void operator()(int64_t p) const {
+    if (p == n) run_ptr[pos[n]] = n;
+    else if (flag[p]) run_ptr[pos[p]] = p;
+  }
+};
+// items 0..n_tiles: tile_run[t] = first run of tile t (the items of a tile are contiguous: the tile is the key's major part)
+struct TileRunF {
+  TableIn in; const int64_t* pos; bool by_slot; int64_t* tile_run;
+  LVBA_THD void operator()(int64_t t) const {
+    const int v = in.tile_vox[t];
+    tile_run[t] = pos[by_slot ? (int64_t)in.vox_ptr[v] : (int64_t)in.vox_pair[v]];
+  }
+};
+
+// items grouped by destination: run r of tile t (tile_run[t] <= r < tile_run[t + 1]) is code[run_ptr[r] .. run_ptr[r + 1])
+template <class Ex>
+struct Runs {
+  typename Ex::template Buf<uint32_t> code;
+  typename Ex::template Buf<int64_t> run_ptr;    // [n_runs + 1]
+  typename Ex::template Buf<int64_t> tile_run;   // [n_tiles + 1]
+  int64_t n_runs = 0;
+};
+
+// by_slot = false: the pose pairs of every voxel (n = vox_pair[V]) grouped by H block; true: the slots (n = vox_ptr[V])
+// grouped by pose.  Inside a run the items keep their enumeration order (stable sort).
+template <class Ex>
+int build_runs(Ex& ex, const TableIn& in, bool by_slot, int64_t n, Runs<Ex>& out) {
+#define LVBA_TILES_TRY(call) do { int rc__ = (call); if (rc__ != 0) return rc__; } while (0)
+  typename Ex::template Buf<uint64_t> key, key_s;
+  typename Ex::template Buf<uint32_t> code;
+  typename Ex::template Buf<int64_t> flag, pos;
+  LVBA_TILES_TRY(key.alloc((size_t)n)); LVBA_TILES_TRY(key_s.alloc((size_t)n));
+  LVBA_TILES_TRY(code.alloc((size_t)n)); LVBA_TILES_TRY(out.code.alloc((size_t)n));
+  if (by_slot) LVBA_TILES_TRY(ex.for_each(n, SlotKeyF{in, key.p, code.p}));
+  else LVBA_TILES_TRY(ex.for_each(n, PairKeyF{in, key.p, code.p}));
+  const uint64_t max_key = (uint64_t)(in.n_tiles > 0 ? in.n_tiles : 1) * (uint64_t)(by_slot ? in.W : in.nblocks);
+  int bits = 1;
+  while (bits < 64 && (max_key >> bits) != 0) ++bits;
+  LVBA_TILES_TRY(ex.sort_pairs(key.p, key_s.p, code.p, out.code.p, n, bits));
+  LVBA_TILES_TRY(flag.alloc((size_t)n + 1)); LVBA_TILES_TRY(pos.alloc((size_t)n + 1));
+  LVBA_TILES_TRY(ex.for_each(n + 1, RunFlagF{key_s.p, n, flag.p}));
+  LVBA_TILES_TRY(ex.exclusive_scan(flag.p, pos.p, n + 1));
+  LVBA_TILES_TRY(ex.fetch(&out.n_runs, pos.p + n, 1));
+  LVBA_TILES_TRY(out.run_ptr.alloc((size_t)out.n_runs + 1));
+  LVBA_TILES_TRY(ex.for_each(n + 1, RunStartF{flag.p, pos.p, n, out.run_ptr.p}));
+  LVBA_TILES_TRY(out.tile_run.alloc((size_t)in.n_tiles + 1));
+  LVBA_TILES_TRY(ex.for_each(in.n_tiles + 1, TileRunF{in, pos.p, by_slot, out.tile_run.p}));
+  return ex.sync();                                          // the scratch buffers are released on return
+#undef LVBA_TILES_TRY
+}
+
+}  // namespace tiles
+}  // namespace lvba
