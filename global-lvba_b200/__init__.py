@@ -124,7 +124,7 @@ def load_library():
     if _lib is not None:
         return _lib
     path = LIB_PATH
-    if os.environ.get("LVBA_B200_DEV_LIB"):          # development builds of the same library (e.g. with in-kernel clocks): tools/ only
+    if os.environ.get("LVBA_B200_DEV_LIB"):          # another build of the same library (e.g. an older one to compare against): tools/ only
         path = _HERE / os.environ["LVBA_B200_DEV_LIB"]
     if not path.exists():
         raise LvbaError(-2, f"{path} not built: run __graft_entry__.build(); there is no CPU fallback")

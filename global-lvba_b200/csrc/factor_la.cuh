@@ -27,7 +27,7 @@ namespace lvba {
 // warps contend with the look-ahead warps for the issue slots and the shared-memory pipe.
 // Two blocks per thread pay off for the widest windows (P > 24: the look-ahead chain gains most, since half as many
 // pair warps compete with it and it keeps 96 registers); for P <= 24 the pair warps that remain do not spread evenly
-// over the four SMSPs and the 144 accumulator registers cost more than the saved operand fetches (tools/lab/ times both).
+// over the four SMSPs and the 144 accumulator registers cost more than the saved operand fetches.
 constexpr bool la_tile2(int P) { return P > 24; }
 constexpr int la_tile2_threads(int P) { int s = 0; for (int m = 1; m <= P; ++m) s += (m + 1) / 2; return s; }
 template <int P, bool kTile2>
@@ -122,7 +122,7 @@ LVBA_DEV void sym6_block_inverse(const double (&x)[21], double (&K)[21]) {
 // The same inverse computed by a WARP: lanes 0..8 <-> entry (i, j) of the 3 x 3 blocks, stages handed over through 45 doubles of
 // shared memory private to the warp; a lane issues ~120 instructions where one thread working through sym6_block_inverse issues
 // ~280, and 84 registers of the calling warp become free.  It is not faster than
-// the one-thread inverse (in-kernel clocks of the separator kernel: make EXTRA=-DLVBA_DENSE_CLOCKS, LVBA_DENSE_MODE=16/17): the
+// the one-thread inverse (in-kernel clocks of the separator kernel, taken with a development build no longer in the tree): the
 // segment is bound by the latency of the two reciprocals and of the hand-overs, not by the instruction count.  Kept for the
 // registers it frees.  D: 36 doubles row-major, LOWER triangle read.  K: 36 doubles, full, exactly
 // symmetric (the mirror entries are copies).  All 32 lanes must call; `scr` holds >= 48 doubles.
@@ -181,14 +181,9 @@ LVBA_DEV void sym6_block_inverse_warp(const double* __restrict__ D, double* __re
   __syncwarp();
 }
 
-#ifdef LVBA_LAB
-__device__ int g_la_mode = 0;      // solver_lab only: 1 = pair threads skip their update, 2 = look-ahead group skips its math
-#endif
-
-template <int P, bool kTiming, bool kTile2>
+template <int P, bool kTile2>
 __global__ void __launch_bounds__(LaCfg<P, kTile2>::kThreads, 1)
-env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restrict__ pair_map,
-                     long long* __restrict__ dbg_all) {
+env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restrict__ pair_map) {
   using Cfg = LaCfg<P, kTile2>;
   constexpr int S = Cfg::S;
   constexpr int PS = P * S;                       // one parity of sL / sT / sA
@@ -199,9 +194,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
   double* __restrict__ z = J.z;
   const int n_stop = J.n_stop;
   pdl_launch_dependents();
-  long long* dbg = (blockIdx.x == 0) ? dbg_all : nullptr;
-  // optional phase clocks (LVBA_FACTOR_TIMING=1): dbg[(k*8 + role)*4 + stamp]
-#define LVBA_STAMP(role, stamp) do { if (kTiming && dbg && lane == 0) dbg[((long long)k * 8 + (role)) * 4 + (stamp)] = clock64(); } while (0)
 
   extern __shared__ __align__(16) double smem_la[];
   double* sL = smem_la;                          // [2][P][S] L_ik transposed ([q*6+x] = L[x][q]); parity = pivot column & 1
@@ -220,9 +212,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
   const int tid = threadIdx.x, lane = tid & 31;
   const int n = e.n;
   const bool is_la = tid >= Cfg::kPairThreads;                 // warp-uniform
-#ifdef LVBA_LAB
-  const int lab_mode = g_la_mode;
-#endif
 
   // ---------------- prologue: labels and rhs of the first P rows
   for (int r = tid; r < 64; r += Cfg::kThreads) {
@@ -291,7 +280,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
     const double2* tq1 = reinterpret_cast<const double2*>(sT + b1 * S);
     const double2* zero2 = reinterpret_cast<const double2*>(sZero);
     int da = a, db0 = b0, db1 = b1;                            // (slot - c) mod P ; c = k mod P
-    const int prole = (tid < 32) ? 0 : (tid >= Cfg::kPairThreads - 32) ? 1 : -1;
     // after its update (if any) a block either takes the entering block, or hands column k+2 over, or rests
     auto settle = [&](double (&G)[36], int b, int db, int cur) {
       const int lo = da < db ? da : db, hi = da < db ? db : da;
@@ -309,13 +297,8 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
     };
     for (int k = 0; k < n_stop; ++k) {
       const int cur = k & 1;
-      if (kTiming && prole >= 0) LVBA_STAMP(prole, 0);
       if (is_pair) {
-        if (da >= 2
-#ifdef LVBA_LAB
-            && lab_mode != 1
-#endif
-        ) {
+        if (da >= 2) {
           // both blocks in one sweep over L_a; a block that must not change (dead, resting or absent) multiplies by zero
           const double2* lp = lp0 + cur * (PS / 2);
           const double2* t0p = (db0 >= 2) ? tq0 + cur * (PS / 2) : zero2;
@@ -338,14 +321,11 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
             }
           }
         }
-        if (kTiming && prole >= 0) LVBA_STAMP(prole, 1);
         settle(G0, b0, db0, cur);
         if (has1) settle(G1, b1, db1, cur);
       }
-      if (kTiming && prole >= 0) LVBA_STAMP(prole, 2);
       __syncthreads();
-      if (kTiming && prole >= 0) LVBA_STAMP(prole, 3);
-      da = (da == 0) ? P - 1 : da - 1;
+      da =(da == 0) ? P - 1 : da - 1;
       db0 = (db0 == 0) ? P - 1 : db0 - 1;
       db1 = (db1 == 0) ? P - 1 : db1 - 1;
     }
@@ -416,10 +396,8 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
     const double2* lp0 = reinterpret_cast<const double2*>(sL + a * S);
     const double2* tp0 = reinterpret_cast<const double2*>(sT + b * S);
     int da = a, db = b;                                        // (slot - c) mod P ; c = k mod P
-    const int prole = (tid < 32) ? 0 : (tid >= Cfg::kPairThreads - 32) ? 1 : -1;
     for (int k = 0; k < n_stop; ++k) {
       const int cur = k & 1;
-      if (kTiming && prole >= 0) LVBA_STAMP(prole, 0);
       if (is_pair) {
         const int lo = da < db ? da : db, hi = da < db ? db : da;
         if (lo == 0) {
@@ -435,11 +413,7 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
 #pragma unroll
               for (int y2 = 0; y2 < 3; ++y2) { const double2 v = src[x * 3 + y2]; G[(2 * y2) * 6 + x] = v.x; G[(2 * y2 + 1) * 6 + x] = v.y; }
           }
-        } else if (lo >= 2
-#ifdef LVBA_LAB
-                   && lab_mode != 1
-#endif
-        ) {
+        } else if (lo >= 2) {
           const double2* lp = lp0 + cur * (PS / 2);
           const double2* tp = tp0 + cur * (PS / 2);
 #pragma unroll
@@ -455,7 +429,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
             }
           }
         }
-        if (kTiming && prole >= 0) LVBA_STAMP(prole, 1);
         // hand column k+2 (the look-ahead group's column of the NEXT step) over: blocks (k+hi, k+2)
         if (lo != 1 && P > 2 && (da == 2 || db == 2)) {
           double* nA = sA + (cur ^ 1) * PS;
@@ -464,9 +437,7 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
           else publish_N(nA + b * S);                        // slot b is the row: G = A^T
         }
       }
-      if (kTiming && prole >= 0) LVBA_STAMP(prole, 2);
       __syncthreads();
-      if (kTiming && prole >= 0) LVBA_STAMP(prole, 3);
       da = (da == 0) ? P - 1 : da - 1;
       db = (db == 0) ? P - 1 : db - 1;
     }
@@ -586,14 +557,9 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
       int s1 = c + 1; if (s1 >= P) s1 -= P;
       const double* Lc = sL + cur * PS;
       const double* T1 = sT + cur * PS + s1 * S;                    // T_{k+1,k}: [r*6+q] = T[q][r]
-      LVBA_STAMP(4 + aw, 0);
       if (aw == 0) {
         // ---- pivot chain: D_{k+1} = A_{k+1,k+1} - L_{k+1,k} T_{k+1,k}^T (lane <-> lower-triangle element), inverse
-        if (k + 1 < n
-#ifdef LVBA_LAB
-            && lab_mode != 2
-#endif
-        ) {
+        if (k + 1 < n) {
           const double* dg = sDg + cur * 36;
           const double* l1 = Lc + s1 * S;
           const int l21 = lane < 21 ? lane : 0;
@@ -608,9 +574,7 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
           __syncwarp();
           invert_pivot(sDu, sK + nxt * 36, k + 1);
         }
-        LVBA_STAMP(4, 1);
         named_bar_sync(1, Cfg::kLaThreads);                         // K_{k+1} visible to the item warps
-        LVBA_STAMP(4, 2);
         // ---- forward substitution with the final z_k : lane <-> row k+1+lane
         double zk[6];
 #pragma unroll
@@ -635,7 +599,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
         if (lane < 6) sZ[c * 6 + lane] = (k + P < n) ? sZin[((k + P) & 7) * 6 + lane] : 0.0;   // row k+P takes slot c
         // columns 0..k of L were complete in global memory before the block barrier this warp passed at the top of the step
         if (J.progress && lane == 0 && (k & 3) == 3) progress_publish(J.progress, k + 1);
-        LVBA_STAMP(4, 3);
       } else {
         // ---- column items: T_{i,k+1} = A_{i,k+1} - L_{i,k} T_{k+1,k}^T for rows i = k+2 .. k+P, then L = T D_{k+1}^-1
         stream_row(k + 1);                                          // row k+1+P -> sEnter[nxt]
@@ -653,13 +616,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
 #pragma unroll
         for (int rd = 0; rd < Cfg::kRounds; ++rd) {
           const int slot = slot_[rd], x = x_[rd];
-#ifdef LVBA_LAB
-          if (lab_mode == 2) {
-#pragma unroll
-            for (int q = 0; q < 6; ++q) t[rd][q] = 0.0;
-            continue;
-          }
-#endif
           if (ent_[rd]) {
             const double* en = sEnter + (cur * P) * 36 + x * 6;     // block (k+P, k+1): index 0, row-major
 #pragma unroll
@@ -684,21 +640,14 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
             for (int q = 0; q < 6; ++q) tn[q * 6 + x] = t[rd][q];
           }
         }
-        LVBA_STAMP(4 + aw, 1);
         named_bar_sync(1, Cfg::kLaThreads);                         // K_{k+1} ready
-        LVBA_STAMP(4 + aw, 2);
         const double* Kp = sK + nxt * 36;
 #pragma unroll
         for (int rd = 0; rd < Cfg::kRounds; ++rd) {
-          if (act_[rd]
-#ifdef LVBA_LAB
-              && lab_mode != 2
-#endif
-          ) scale_item(Kp, t[rd], slot_[rd], x_[rd], k + h_[rd], k + 1, nxt);
+          if (act_[rd]) scale_item(Kp, t[rd], slot_[rd], x_[rd], k + h_[rd], k + 1, nxt);
           if (++slot_[rd] == P) slot_[rd] = 0;
         }
         cp_async_wait_all();
-        LVBA_STAMP(4 + aw, 3);
       }
       __syncthreads();
       if (++c == P) c = 0;
@@ -711,7 +660,6 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
     }
     if (bad) J.status[0] = 1;
   }
-#undef LVBA_STAMP
   if (J.progress) {                                               // the last global write of the CTA (env_types.h)
     __syncthreads();
     if (tid == 0) progress_publish(J.progress, n_stop);

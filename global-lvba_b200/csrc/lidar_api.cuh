@@ -256,7 +256,6 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
       for (int r = 0; r < W; ++r) first_raw[r] = std::min(first_raw[r], first_w[(size_t)w * (size_t)W + r]);
   }
   LVBA_TRY(P->env.build(first_raw, s, &P->h2d));
-  LVBA_TRY(P->solver.prepare(P->env, s));
   // ---- batched window BA: window of every pose, every voxel inside one window
   std::vector<int> pose_grp;
   if (n_groups > 0) {
@@ -273,8 +272,8 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
         return fail(LVBA_ERR_INVALID_ARG, "voxel %lld spans two windows", (long long)a);
       ++P->grp_V[g];
     }
-    LVBA_TRY(P->solver.prepare_batch(P->env, P->grp_ptr, s));
   }
+  LVBA_TRY(P->solver.prepare(P->env, s, LVBA_SOLVE_AUTO, 0, P->grp_ptr));     // grp_ptr empty: not batched
   lap("envelope+solver alloc");
 
   // ---- shard: voxel -> owner of its lowest pose index (SURVEY.md §8e)
@@ -303,7 +302,7 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
       owned.swap(small);
     }
     // the batched window LM (lidar_batch_lm_impl) has no big-voxel passes: such a voxel would silently drop out of H, g and the
-    // residual sums while still counting in the AVG_THR divisor.  A window holds <= 31 poses (prepare_batch), so this cannot
+    // residual sums while still counting in the AVG_THR divisor.  A window holds <= 31 poses (EnvSolver::prepare), so this cannot
     // happen today; refuse loudly if that ever changes (ADVICE r1).
     if (n_groups > 0 && !bigv.empty())
       return fail(LVBA_ERR_UNSUPPORTED, "batched window BA: voxel %lld is seen from %lld poses (more than %d)", (long long)bigv[0],

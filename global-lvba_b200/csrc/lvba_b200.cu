@@ -53,14 +53,7 @@ int lvba_env_solve(int32_t n, const int32_t* first, const double* blocks, const 
     LVBA_TRY(env.build(fr, s, &bytes));
     EnvSolver sol;
     LVBA_TRY(sol.prepare(env, s, path, chunks));
-    int taken;
-    if (sol.wide) taken = LVBA_SOLVE_ANY_WIDTH;
-    else if (sol.nd_on) taken = LVBA_SOLVE_CHUNKED;
-    else if (sol.tw) taken = LVBA_SOLVE_TWISTED;
-    else if (env.max_col <= 30 && env.n >= 3 && !sol.force_generic) taken = LVBA_SOLVE_ONE_CTA;
-    else taken = LVBA_SOLVE_SHARED_WINDOW;
-    if (path != LVBA_SOLVE_AUTO && taken != path)
-      return fail(LVBA_ERR_UNSUPPORTED, "path %d is not available for this structure (n = %d, tallest column %d blocks): would take path %d", path, n, env.max_col, taken);
+    const bool chunked = sol.path == LVBA_SOLVE_CHUNKED;
     DevBuf<double> dH, dD, dR, dX;
     LVBA_TRY(dH.upload(blocks, (size_t)env.nblocks * 36, s)); LVBA_TRY(dD.upload(dadd, (size_t)n * 6, s));
     LVBA_TRY(dR.upload(rhs, (size_t)n * 6, s)); LVBA_TRY(dX.alloc((size_t)n * 6));
@@ -88,7 +81,7 @@ int lvba_env_solve(int32_t n, const int32_t* first, const double* blocks, const 
       if (st) rc = fail(LVBA_ERR_NUMERIC, "singular / non-finite pivot block");
     }
     if (ms) *ms = best;
-    if (info) { info[0] = taken; info[1] = sol.nd_on ? sol.nd.chunks : 0; info[2] = sol.nd_on ? (int)sol.nd.plan.levels.size() : 0; info[3] = (int)per; }
+    if (info) { info[0] = sol.path; info[1] = chunked ? sol.nd.chunks : 0; info[2] = chunked ? (int)sol.nd.plan.levels.size() : 0; info[3] = (int)per; }
     cudaStreamSynchronize(s);       // nothing of `sol` / the buffers may be in flight when they go back to the pool
   }
   return rc;

@@ -44,12 +44,8 @@ constexpr int kSpikeBufs = 3;                    // rows of L in flight (cp.asyn
 constexpr size_t kSpikeSmem = sizeof(double) * (kSpikeBufs * 32 * kSpikeBS + kSpikeWarps * 33 * kSpikeZStride);
 static_assert(kSpikeC == 4, "the reduce-scatter below is written for 24 values per lane");
 
-// LVBA_SPIKE_MODE (development, results are wrong unless 0): 1 = no block products, 2 = no staging of L, 4 = no E loads / Z stores
-__device__ int g_spike_mode = 0;
-
 __global__ void __launch_bounds__(kSpikeThreads)
 nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
-  const int dbg_mode = g_spike_mode;
   extern __shared__ __align__(16) double smem_spike[];
   double* sRow = smem_spike;                                   // [kSpikeBufs][32][kSpikeBS] blocks of rows k, k+1, k+2
   const nd::SpikeJob J = jobs[blockIdx.y];
@@ -76,7 +72,7 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
     const int nb = jend > f ? jend - f : 0;
     const double* src = J.L + rs * 36;
     double* dst = sRow + (k % kSpikeBufs) * (32 * kSpikeBS);
-    if (tid < 126 && !(dbg_mode & 2))                          // thread -> (block, 16-byte piece): 7 blocks per sweep
+    if (tid < 126)                                             // thread -> (block, 16-byte piece): 7 blocks per sweep
       for (int b = sb0; b < nb; b += 7) cp_async16_zfill(dst + b * kSpikeBS + 2 * sh, src + b * 36 + 2 * sh, true);
   };
   // labels: row k (f0), rows k+1 .. k+3 (f1..f3, rs2, rs3): fetched four rows ahead of their use in the chain
@@ -86,7 +82,7 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
   int f3 = n > 3 ? e.first[3] : 0; long long rs3 = n > 3 ? e.row_start[3] : 0;
   double en[3];                                                // E of the next row: this lane's three outputs
 #pragma unroll
-  for (int q = 0; q < 3; ++q) en[q] = (owner && cw + oc[q] < KS && 0 < J.nE && !(dbg_mode & 4)) ? J.E[((long long)ox[q]) * KS + cw + oc[q]] : 0.0;
+  for (int q = 0; q < 3; ++q) en[q] = (owner && cw + oc[q] < KS && 0 < J.nE) ? J.E[((long long)ox[q]) * KS + cw + oc[q]] : 0.0;
   // side by side with the factorisation (J.progress): row r of L is final once min(r, n_stop) columns are; one thread polls, the
   // block barrier hands the acquired view to the others (the rows are fetched by cp.async.cg: L2, never a stale L1 line)
   int seen = J.progress ? 0 : 0x7fffffff;
@@ -113,13 +109,11 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
     for (int q = 0; q < 3; ++q) ecur[q] = en[q];
 #pragma unroll
     for (int q = 0; q < 3; ++q)
-      en[q] = (owner && cw + oc[q] < KS && k + 1 < J.nE && !(dbg_mode & 4)) ? J.E[((long long)(k + 1) * 6 + ox[q]) * KS + cw + oc[q]] : 0.0;
+      en[q] = (owner && cw + oc[q] < KS && k + 1 < J.nE) ? J.E[((long long)(k + 1) * 6 + ox[q]) * KS + cw + oc[q]] : 0.0;
     const int jend = k < n_stop ? k : n_stop;
     // ---- this lane's block L_{k, f0 + lane} times the four columns of z_{f0 + lane}
     double v[24];
-#pragma unroll
-    for (int o = 0; o < 24; ++o) v[o] = 0.0;
-    if (!(dbg_mode & 1)) {
+    {
       const int j = f0 + lane;
       const int zr = (j < jend) ? (j & 31) : 32;               // no block: the zero row (the L slot holds finite stale data)
       const double2* b2 = reinterpret_cast<const double2*>(sRow + (k % kSpikeBufs) * (32 * kSpikeBS) + lane * kSpikeBS);
@@ -173,7 +167,7 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
       for (int q = 0; q < 3; ++q) {
         const double r = ecur[q] - w3[q];
         sZw[(k & 31) * kSpikeZStride + ox[q] * 4 + oc[q]] = r;       // row k-32 is no longer needed (column height <= 30)
-        if (cw + oc[q] < KS && !(dbg_mode & 4)) J.Z[((long long)k * 6 + ox[q]) * KS + cw + oc[q]] = r;
+        if (cw + oc[q] < KS) J.Z[((long long)k * 6 + ox[q]) * KS + cw + oc[q]] = r;
       }
     }
     __syncwarp();
@@ -193,7 +187,7 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
 constexpr int kSyrkTile = 64;            // scalar columns per tile side
 constexpr int kSyrkThreads = 64;         // 8 x 8 threads, 8 x 8 outputs each
 constexpr int kSyrkChunk = 4;            // block rows per shared-memory chunk (24 scalar rows)
-constexpr int kSyrkSplit = 8;            // block rows per CTA (default; LVBA_SYRK_SPLIT overrides): two chunks, both in flight from the start
+constexpr int kSyrkSplit = 8;            // block rows per CTA: two chunks, both in flight from the start
 constexpr int kSyrkLd = kSyrkTile + 4;   // leading dimension of the shared tiles
 constexpr int kSyrkTileDoubles = kSyrkChunk * 6 * kSyrkLd;
 constexpr size_t kSyrkSmem = sizeof(double) * (5 * kSyrkTileDoubles + 2 * kSyrkChunk * 36 + 2 * kSyrkChunk * 6 + kSyrkChunk * 6);
@@ -366,11 +360,6 @@ static_assert((kDenseColBase) * kDensePairRegs + (kDenseThreads - kDenseColBase)
 constexpr int kDenseS = 38;                  // doubles per operand block in shared memory (bank spread, 16 B aligned)
 constexpr size_t kDenseSmem = sizeof(double) * (6 * kDenseMax * kDenseS + 36 + 72 + kDenseMax * 6 + 8 + 48);
 
-// LVBA_DENSE_MODE (development, results are wrong unless 0): 1 = no trailing update by the pair threads, 2 = the inverting warp skips
-// the inverse (stale K), 4 = the column group skips apply and scale arithmetic; 8 (results stay right) = the pair threads start
-// their trailing update only after the column / inverse chain of the step has finished (no overlap)
-__device__ int g_dense_mode = 0;
-
 __global__ void __launch_bounds__(kDenseThreads, 1)
 nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short* __restrict__ tmap) {
   extern __shared__ __align__(16) double smem_dense[];
@@ -384,14 +373,6 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
   const FactorJob J = jobs[blockIdx.x];
   const int n = J.e.n;
   const int tid = threadIdx.x;
-  const int dense_mode = g_dense_mode;
-#ifdef LVBA_DENSE_CLOCKS                                   // development build only (make EXTRA=-DLVBA_DENSE_CLOCKS): stamps of block 0
-  __shared__ long long sClk[kDenseMax][6];
-  const bool stamp = (dense_mode & 16) && blockIdx.x == 0;
-#define LVBA_DSTAMP(slot, who) do { if (stamp && (who)) sClk[s][slot] = clock64(); } while (0)
-#else
-#define LVBA_DSTAMP(slot, who) do { } while (0)
-#endif
   pdl_launch_dependents();
   for (int o = tid; o < n * 6; o += kDenseThreads) sZ[o] = J.z[o];
   // register re-allocation: one setmaxnreg site per warpgroup-uniform branch (warpgroups 0-3: pair threads + inverting warp)
@@ -406,14 +387,13 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
     __syncthreads();                                               // (P) columns 0 and 1 published by the pair threads
     for (int s = 0; s < n; ++s) {
       const int par = s & 1;
-      LVBA_DSTAMP(0, ct == 0);
       // ---- (1) column s as of pivot s-1: row r of block (i, s), i >= s
       double t[6] = {0, 0, 0, 0, 0, 0};
       if (mine && i >= s) {
         const double2* c2 = reinterpret_cast<const double2*>(sC + (par * kDenseMax + i) * kDenseS + r * 6);
         const double2 q0 = c2[0], q1 = c2[1], q2 = c2[2];
         t[0] = q0.x; t[1] = q0.y; t[2] = q1.x; t[3] = q1.y; t[4] = q2.x; t[5] = q2.y;
-        if (s > 0 && !(dense_mode & 4)) {                          // -= L_{i,s-1}[r][.] T_{s,s-1}^T   (sT holds T^T: [q][y])
+        if (s > 0) {                                               // -= L_{i,s-1}[r][.] T_{s,s-1}^T   (sT holds T^T: [q][y])
           const double2* ts = reinterpret_cast<const double2*>(sT + ((par ^ 1) * kDenseMax + s) * kDenseS);
 #pragma unroll
           for (int q = 0; q < 6; ++q) {
@@ -428,12 +408,10 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
           d2[0] = make_double2(t[0], t[1]); d2[1] = make_double2(t[2], t[3]); d2[2] = make_double2(t[4], t[5]);
         }
       }
-      LVBA_DSTAMP(1, ct == 0);
       if (!idle) {
         named_bar_sync(2, kDenseColThreads + 32);                  // pivot block complete -> the inverting warp
         named_bar_sync(3, kDenseColThreads + 32);                  // D_s^-1 visible
       }
-      LVBA_DSTAMP(3, ct == 0);
       // ---- (2) scale: row r of L_is = T_is D_s^-1, publish T and L, forward substitution
       if (mine && i > s) {
         double lr[6] = {0, 0, 0, 0, 0, 0};
@@ -456,8 +434,6 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
         for (int q = 0; q < 6; ++q) { zs = fma(lr[q], sZ[s * 6 + q], zs); lrow[q] = lr[q]; }
         sZ[i * 6 + r] -= zs;
       }
-      LVBA_DSTAMP(4, ct == 0);
-      if (dense_mode & 8) __syncthreads();                         // (X) the chain of this step is done: now the pair threads may run
       __syncthreads();                                             // (s) L_s, T_s published; column s+2 handed over by the pair threads
       // the two idle warps of this group: D_s^-1 to global memory (the inverting warp left it in sK[par]; it writes that buffer again
       // two pivots from now), and word to a spike kernel running beside this CTA that columns 0..s of L are in global memory
@@ -474,15 +450,11 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
     __syncthreads();                                               // (P)
     for (int s = 0; s < n; ++s) {
       named_bar_sync(2, kDenseColThreads + 32);
-      LVBA_DSTAMP(2, lane == 0);
       double* Kp = sK + (s & 1) * 36;                              // D_s^-1 (full symmetric) for the column group, and for the idle warp that copies it out
-      if (!(dense_mode & 2)) sym6_block_inverse_warp(sD, Kp, sInv, lane);
-      else if (lane < 18) reinterpret_cast<double2*>(Kp)[lane] = reinterpret_cast<const double2*>(sD)[lane];
+      sym6_block_inverse_warp(sD, Kp, sInv, lane);
       __syncwarp();
       if (!isfinite((Kp[0] + Kp[35]) + (Kp[18] + Kp[13]))) bad = 1;
-      LVBA_DSTAMP(5, lane == 0);
       named_bar_sync(3, kDenseColThreads + 32);
-      if (dense_mode & 8) __syncthreads();                         // (X)
       __syncthreads();                                             // (s)
     }
     if (bad && lane == 0) J.status[0] = 1;
@@ -509,9 +481,8 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
     if (live && j <= 1) publish(j);                                // columns 0 and 1 as they are
     __syncthreads();                                               // (P)
     for (int s = 0; s < n; ++s) {
-      if (dense_mode & 8) __syncthreads();                         // (X)
       // the trailing update of pivot s-1 for the columns the pair threads still own (j >= s+1)
-      if (s >= 1 && live && j >= s + 1 && !(dense_mode & 1)) {
+      if (s >= 1 && live && j >= s + 1) {
         const int par = (s - 1) & 1;
         // rank-1 steps over the contraction index q: column q of T_j (six values) and two entries of column q of L_i at a time are
         // live beside the 36 accumulators — 16 operand registers, which is what fits the 96-register budget without spilling G
@@ -538,23 +509,6 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
     }
   }
   __syncthreads();
-#ifdef LVBA_DENSE_CLOCKS
-  if (stamp && tid == 0 && n >= 8) {
-    long long d[6] = {0, 0, 0, 0, 0, 0};
-    for (int s = 2; s + 1 < n; ++s) {
-      d[0] += sClk[s][1] - sClk[s][0];        // column group: load + apply
-      d[1] += sClk[s][2] - sClk[s][1];        // barrier 2
-      d[2] += sClk[s][5] - sClk[s][2];        // inverse (+ writing K)
-      d[3] += sClk[s][3] - sClk[s][5];        // barrier 3
-      d[4] += sClk[s][4] - sClk[s][3];        // scale + publish
-      d[5] += sClk[s + 1][0] - sClk[s][4];    // block barrier (waiting for the pair threads included)
-    }
-    const long long m = n - 3;
-    printf("[dense clocks] n=%d per pivot: apply %lld | bar2 %lld | inverse %lld | bar3 %lld | scale %lld | block barrier %lld | step %lld\n", n,
-           d[0] / m, d[1] / m, d[2] / m, d[3] / m, d[4] / m, d[5] / m, (d[0] + d[1] + d[2] + d[3] + d[4] + d[5]) / m);
-  }
-#endif
-#undef LVBA_DSTAMP
   for (int o = tid; o < n * 6; o += kDenseThreads) J.z[o] = sZ[o];
   if (J.progress) {                                                // the last global write of the CTA
     __syncthreads();

@@ -26,10 +26,8 @@ struct NdDevice {
   int n_ranks = 1, my_rank = 0;
   DevBuf<double> xchg;                     // multi-GPU: rows received from the left neighbour (exchange_rows)
   DevBuf<unsigned short> d_dense_map;      // thread -> block of nd_dense_factor_kernel
-  bool dense_sep = true;                   // separators by nd_dense_factor_kernel (LVBA_ND_DENSE=0: register-window kernel)
   // the spike kernels start while the factorisation they read from is still running and follow its progress counters
-  // (programmatic dependent launch; LVBA_ND_PIPELINE=0: one after the other)
-  bool pipeline = true;
+  // (programmatic dependent launch)
   DevBuf<int> d_prog;                      // [nodes]
   // numeric pools
   DevBuf<double> zs, U, u, Z, E, T, W, w;
@@ -57,8 +55,6 @@ struct NdDevice {
   // number of chunks for a system of n block rows with columns of at most max_col blocks: the chain is
   // (interior) + (tree depth) x (separator width) pivot columns; more chunks shorten the first term and lengthen the second
   static int default_chunks(int n, int max_col) {
-    const char* ev = getenv("LVBA_ND_CHUNKS");
-    if (ev && ev[0]) return atoi(ev);
     // a leaf costs a fixed time per row (factor + spike + substitutions), a tree level a time linear in the separator width
     // w; the twisted pair a (smaller) time per row of the whole system.  Interiors of about three band widths balance the
     // two terms; below ~800 rows the two-CTA twisted solve wins (tools/solver_bench.py measures the crossover).
@@ -86,6 +82,8 @@ struct NdDevice {
         if (plan.rank_row_end[r] - plan.rank_row_begin[r] < max_col + 1) return LVBA_OK;
     }
     {
+      // LVBA_ND_GRAPH=0 runs nd::run eagerly on every solve.  That code is needed anyway (the fall-back when stream capture
+      // fails, and how the multi-GPU solve runs); this switch is the only way a one-GPU test reaches it.
       const char* g = getenv("LVBA_ND_GRAPH");
       use_graph = !(g && g[0] == '0');
     }
@@ -105,10 +103,6 @@ struct NdDevice {
     LVBA_TRY(d_nodes.upload(nodes, s, &dummy));
     const std::vector<unsigned short> dmap = dense_thread_map();
     LVBA_TRY(d_dense_map.upload(dmap, s, &dummy));
-    {
-      const char* g = getenv("LVBA_ND_DENSE");
-      dense_sep = !(g && g[0] == '0');
-    }
     LVBA_TRY(zs.alloc((size_t)n * 6));
     LVBA_TRY(U.alloc((size_t)std::max<long long>(plan.sizeU, 1))); LVBA_TRY(u.alloc((size_t)std::max<long long>(plan.sizeu, 1)));
     LVBA_TRY(Z.alloc((size_t)std::max<long long>(plan.sizeZ, 1))); LVBA_TRY(E.alloc((size_t)std::max<long long>(plan.sizeE, 1)));
@@ -127,18 +121,8 @@ struct NdDevice {
       }
       LVBA_TRY(xchg.alloc((size_t)std::max<long long>(mx, 1)));
     }
-    {
-      const char* pe = getenv("LVBA_ND_PIPELINE");
-      pipeline = !(pe && pe[0] == '0');
-      if (pipeline) LVBA_TRY(d_prog.alloc(plan.nodes.size()));
-    }
+    LVBA_TRY(d_prog.alloc(plan.nodes.size()));
     LVBA_CUDA(cudaFuncSetAttribute(nd_spike_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSpikeSmem));
-    {
-      const char* m = getenv("LVBA_SPIKE_MODE");             // development only (nd_kernels.cuh); the symbol is 0 unless asked
-      if (m) { const int mode = atoi(m); LVBA_CUDA(cudaMemcpyToSymbol(g_spike_mode, &mode, sizeof(int))); }
-      const char* dm = getenv("LVBA_DENSE_MODE");
-      if (dm) { const int mode = atoi(dm); LVBA_CUDA(cudaMemcpyToSymbol(g_dense_mode, &mode, sizeof(int))); }
-    }
     LVBA_CUDA(cudaFuncSetAttribute(nd_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
     LVBA_CUDA(cudaFuncSetAttribute(nd_dense_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDenseSmem));
     LVBA_CUDA(cudaStreamSynchronize(s));                     // local vectors
@@ -159,7 +143,7 @@ struct NdDevice {
     tab.U = U.p; tab.u = U.p; tab.Z = Z.p; tab.E = E.p; tab.T = T.p; tab.W = W.p; tab.w = w.p;
     tab.Hw = n_ranks > 1 ? const_cast<double*>(H) : nullptr;       // multi-GPU: the other ranks' rank-separator rows are written into
     tab.daddw = n_ranks > 1 ? const_cast<double*>(dadd) : nullptr; // the caller's H / dadd (documented at EnvSolver::solve)
-    tab.prog = pipeline ? d_prog.p : nullptr;
+    tab.prog = d_prog.p;
     std::vector<nd::LevelJobs> jobs;
     nd::DenseViewArrays dv{d_zeros.p, d_tri.p, d_last_by_w.p};
     nd::build_level_jobs(plan, tab, d_first_rel.p, d_rs_adj.p, d_last_rel.p, genv.nblocks, dv, status + 1, jobs, my_rank);
@@ -194,8 +178,7 @@ struct NdCudaExec {
   cudaStream_t s;
   std::function<int(int, int, const FactorJob*)> factor_fn;        // (max_col, n_jobs, jobs)
   std::function<void(int, const BacksolveJob*)> back_fn;           // (n_jobs, jobs)
-  const unsigned short* dense_map = nullptr;                       // non-null: separators by nd_dense_factor_kernel
-  bool pipeline = false;                                           // spike kernels by programmatic dependent launch (NdDevice::pipeline)
+  const unsigned short* dense_map = nullptr;                       // thread -> block of nd_dense_factor_kernel (NdDevice::d_dense_map)
   int64_t launches = 0;
   int rc = LVBA_OK;
   template <class F> void pass(long long n, const F& f) {
@@ -213,33 +196,26 @@ struct NdCudaExec {
   }
   void factor_dense(const FactorJob* jobs, int n, int max_col) {
     if (n <= 0) return;
-    if (!dense_map) { factor(jobs, n, max_col); return; }
     nd_dense_factor_kernel<<<n, kDenseThreads, kDenseSmem, s>>>(jobs, dense_map);
     ++launches;
   }
   void spike(const nd::SpikeJob* jobs, int n, int max_ks, int) {
     if (n <= 0 || max_ks <= 0) return;
-    const dim3 grid((max_ks + kSpikeCols - 1) / kSpikeCols, n);
-    if (pipeline) {
-      // the kernel launched just before this one is the factorisation whose L these jobs read: start as soon as all of ITS CTAs run
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = grid; cfg.blockDim = dim3(kSpikeThreads); cfg.dynamicSmemBytes = kSpikeSmem; cfg.stream = s;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      at[0].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      const cudaError_t e = cudaLaunchKernelEx(&cfg, nd_spike_kernel, jobs);
-      if (e != cudaSuccess) rc = fail(LVBA_ERR_CUDA, "cudaLaunchKernelEx(nd_spike_kernel): %s", cudaGetErrorString(e));
-    } else {
-      nd_spike_kernel<<<grid, kSpikeThreads, kSpikeSmem, s>>>(jobs);
-    }
+    // the kernel launched just before this one is the factorisation whose L these jobs read: start as soon as all of ITS CTAs run
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((max_ks + kSpikeCols - 1) / kSpikeCols, n); cfg.blockDim = dim3(kSpikeThreads); cfg.dynamicSmemBytes = kSpikeSmem; cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, nd_spike_kernel, jobs);
+    if (e != cudaSuccess) rc = fail(LVBA_ERR_CUDA, "cudaLaunchKernelEx(nd_spike_kernel): %s", cudaGetErrorString(e));
     ++launches;
   }
   void syrk(const nd::SyrkSeg* segs, int n, int max_ks, int max_rows) {
     if (n <= 0 || max_ks <= 0) return;
     const int nt1 = (max_ks + kSyrkTile - 1) / kSyrkTile, nt = nt1 * (nt1 + 1) / 2;
-    static const int split = [] { const char* e = getenv("LVBA_SYRK_SPLIT"); const int v = e ? atoi(e) : 0; return v > 0 ? ((v + kSyrkChunk - 1) / kSyrkChunk) * kSyrkChunk : kSyrkSplit; }();
-    nd_syrk_kernel<<<dim3(nt, (max_rows + split - 1) / split, n), kSyrkThreads, kSyrkSmem, s>>>(segs, split);
+    nd_syrk_kernel<<<dim3(nt, (max_rows + kSyrkSplit - 1) / kSyrkSplit, n), kSyrkThreads, kSyrkSmem, s>>>(segs, kSyrkSplit);
     ++launches;
   }
   void correct_apply(const nd::Tables& t, const int* ids, int n_ids, int stride) {

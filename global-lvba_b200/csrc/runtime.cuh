@@ -361,15 +361,18 @@ inline std::vector<unsigned> build_pair_map32(int P, bool tile2, int n_threads) 
 namespace lvba {
 
 // ---------------------------------------------------------------- LDL^T solve driver
+// The path is chosen once, by prepare(), from the structure of the system, and solve() follows it.
+constexpr int kSolveBatch = -1;       // EnvSolver::path of a block-diagonal window batch (not an lvba_env_solve path)
 struct EnvSolver {
   DevBuf<double> L, dinv, z;
   DevBuf<int> status;
+  // LVBA_SOLVE_* (include/lvba_b200.h) or kSolveBatch; LVBA_SOLVE_AUTO until prepare() has run
+  int path = LVBA_SOLVE_AUTO;
   // device job tables of the register-window path (built at the first solve, when the solution buffer is known)
   DevBuf<FactorJob> d_fjobs;
   DevBuf<BacksolveJob> d_bjobs;
   const double* jobs_x = nullptr;
   // ---- batched mode (window BA): the system is block diagonal; every group is factorised by its own CTA
-  bool batch = false;
   int n_groups = 0;
   std::vector<int> grp_ptr;     // [n_groups+1] row offsets
   DevBuf<int> first_rel;        // first[r] relative to the first row of r's group
@@ -378,24 +381,18 @@ struct EnvSolver {
   static constexpr int kNumP = 6;
   DevBuf<unsigned> pair_map[kNumP];     // thread -> blocks of the register-window kernel, per P
   bool have_map[kNumP] = {false, false, false, false, false, false};
-  DevBuf<long long> dbg;        // LVBA_FACTOR_TIMING=1: per-step phase clocks of the register-window kernel
-  int dbg_dumped = 0, dbg_max_dumps = 2;
   bool configured = false;
-  bool force_generic = false;   // tests: exercise the wide-envelope kernel on narrow problems
-  // ---- any-width path (envelope_wide.h): columns taller than kEnvMaxCol blocks (loop closures), or forced by the tests
-  bool wide = false;
+  // ---- any-width path (envelope_wide.h): columns taller than kEnvMaxCol blocks (loop closures)
   DevBuf<double> colT;          // [max_col * 36] unscaled copy of the current pivot column
   // ---- twisted (two-ended) factorisation: top half in natural order on one SM, bottom half reversed on another,
   //      joined at a separator of `tw_bs` rows (see envelope.cuh, FactorJob)
   // ---- substructured solve (nd_solver.cuh): p chunk interiors + a tree of separators, one CTA per node; chosen for
   //      systems long enough that  interior + depth x separator  pivot columns beat the two halves of the twisted solve
   NdDevice nd;
-  bool nd_on = false;
-  bool shard = true;            // with an active communicator: cut the system so that its chunks are the multi-GPU unit (SURVEY.md 8(e))
   // multi-GPU, row-owned system: rank r owns the rows dist_begin() .. dist_end()-1 of H / S (its chunks, inner separators and
   // its right rank separator); voxels / tracks are assigned to the owner of their lowest row, so a rank's contributions reach
   // at most max_col rows into the next rank's range: exchange_rows() ships exactly those rows
-  bool dist() const { return nd_on && nd.n_ranks > 1; }
+  bool dist() const { return path == LVBA_SOLVE_CHUNKED && nd.n_ranks > 1; }
   int dist_begin() const { return nd.plan.rank_row_begin[nd.my_rank]; }
   int dist_end() const { return nd.plan.rank_row_end[nd.my_rank]; }
   int dist_owner(int row) const {
@@ -419,7 +416,6 @@ struct EnvSolver {
     }
     return LVBA_OK;
   }
-  bool tw = false;
   int tw_m = 0, tw_send = 0, tw_bs = 0, tw_nb = 0, tw_nbstop = 0;
   Envelope env_bot, env_sep;
   DevBuf<double> Lbot, dinv_bot, zbot, xbot, wtop, wbot, ztopd, zbotd, Lsep, dinv_sep, zsep, xsep;
@@ -427,78 +423,98 @@ struct EnvSolver {
   static int pid(int mc) { return mc <= 7 ? 0 : mc <= 11 ? 1 : mc <= 15 ? 2 : mc <= 20 ? 3 : mc <= 23 ? 4 : 5; }
   static int pval(int id) { return id == 0 ? 8 : id == 1 ? 12 : id == 2 ? 16 : id == 3 ? 21 : id == 4 ? 24 : 31; }
 
-  // path: LVBA_SOLVE_AUTO picks by structure; the others pin one path (lvba_env_solve, tests): see include/lvba_b200.h
-  int prepare(const Envelope& env, cudaStream_t s, int path = LVBA_SOLVE_AUTO, int chunks = 0) {
-    {
-      const char* fg = getenv("LVBA_FORCE_GENERIC_SOLVER");      // tests: run the wide-envelope kernel on narrow problems
-      force_generic = (fg && fg[0] == '1') || path == LVBA_SOLVE_SHARED_WINDOW;
-      const char* fw = getenv("LVBA_FORCE_WIDE_SOLVER");         // tests: run the any-width path on narrow problems
-      wide = env.max_col > kEnvMaxCol || (fw && fw[0] == '1') || path == LVBA_SOLVE_ANY_WIDTH;
-    }
-    if (wide) LVBA_TRY(colT.alloc((size_t)std::max(env.max_col, 1) * 36));
+  // Chooses the path and allocates what it needs.  want = LVBA_SOLVE_AUTO picks by structure (what lvba_lidar_lm /
+  // lvba_visual_lm run); any other LVBA_SOLVE_* value pins that path and fails with LVBA_ERR_UNSUPPORTED if the structure
+  // does not allow it.  chunks: for LVBA_SOLVE_CHUNKED (< 2: default_chunks).  groups (window BA): row offsets
+  // [n_groups + 1] of a block-diagonal system, every group factorised by its own CTA; want must then be LVBA_SOLVE_AUTO.
+  int prepare(const Envelope& env, cudaStream_t s, int want = LVBA_SOLVE_AUTO, int chunks = 0, const std::vector<int>& groups = {}) {
+    path = LVBA_SOLVE_AUTO;
     LVBA_TRY(L.alloc((size_t)env.nblocks * 36));
     LVBA_TRY(dinv.alloc((size_t)env.n * 36));
     LVBA_TRY(z.alloc((size_t)env.n * 6));
     LVBA_TRY(status.alloc(4));
     jobs_x = nullptr;
-    {
-      const char* ft = getenv("LVBA_FACTOR_TIMING");
-      if (ft && ft[0] == '1') { LVBA_TRY(dbg.alloc((size_t)env.n * 32)); }
-    }
     if (!configured) {
       LVBA_CUDA(cudaFuncSetAttribute(env_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)factor_smem()));
-#define LVBA_SET_SMEM(PP, TT) LVBA_CUDA(cudaFuncSetAttribute(env_factor_la_kernel<PP, TT, la_tile2(PP)>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LaCfg<PP, la_tile2(PP)>::kSmem))
-      LVBA_SET_SMEM(8, false); LVBA_SET_SMEM(8, true); LVBA_SET_SMEM(12, false); LVBA_SET_SMEM(12, true);
-      LVBA_SET_SMEM(16, false); LVBA_SET_SMEM(16, true); LVBA_SET_SMEM(21, false); LVBA_SET_SMEM(21, true);
-      LVBA_SET_SMEM(24, false); LVBA_SET_SMEM(24, true); LVBA_SET_SMEM(31, false); LVBA_SET_SMEM(31, true);
+#define LVBA_SET_SMEM(PP) LVBA_CUDA(cudaFuncSetAttribute(env_factor_la_kernel<PP, la_tile2(PP)>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LaCfg<PP, la_tile2(PP)>::kSmem))
+      LVBA_SET_SMEM(8); LVBA_SET_SMEM(12); LVBA_SET_SMEM(16); LVBA_SET_SMEM(21); LVBA_SET_SMEM(24); LVBA_SET_SMEM(31);
 #undef LVBA_SET_SMEM
       LVBA_CUDA(cudaFuncSetAttribute(env_backsolve_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBsSmem));
       configured = true;
     }
-    // ---- twisted split: worthwhile when each half is many pivots long
-    tw = false;
-    const char* nt = getenv("LVBA_NO_TWIST");
-    const bool reg_ok = env.max_col <= 30 && env.n >= 3 && !force_generic && !wide;
-    const bool want_tw = path == LVBA_SOLVE_AUTO ? (env.n >= 256 && !(nt && nt[0] == '1')) : path == LVBA_SOLVE_TWISTED;
-    if (reg_ok && want_tw && env.n >= 8) {
-      const int n = env.n;
-      const int m = n / 2;
-      const int send = env.last[m - 1] + 1;            // rows >= send do not couple to rows < m
-      const int bs = send - m;
-      if (bs >= 3 && bs <= 30 && send < n - 32) {
-        tw_m = m; tw_send = send; tw_bs = bs; tw_nb = n - m; tw_nbstop = n - send;
-        std::vector<int> fb((size_t)tw_nb);
-        for (int rp = 0; rp < tw_nb; ++rp) fb[rp] = n - 1 - env.last[n - 1 - rp];     // reversed row couples up to the original column's last row
-        int64_t dummy = 0;
-        LVBA_TRY(env_bot.build(fb, s, &dummy));
-        std::vector<int> fs((size_t)bs, 0);
-        LVBA_TRY(env_sep.build(fs, s, &dummy));
-        if (env_bot.max_col <= 30) {
-          LVBA_TRY(Lbot.alloc((size_t)env_bot.nblocks * 36)); LVBA_TRY(dinv_bot.alloc((size_t)tw_nb * 36));
-          LVBA_TRY(zbot.alloc((size_t)tw_nb * 6)); LVBA_TRY(xbot.alloc((size_t)tw_nb * 6));
-          LVBA_TRY(wtop.alloc((size_t)bs * bs * 36)); LVBA_TRY(wbot.alloc((size_t)bs * bs * 36));
-          LVBA_TRY(ztopd.alloc((size_t)bs * 6)); LVBA_TRY(zbotd.alloc((size_t)bs * 6));
-          LVBA_TRY(Lsep.alloc((size_t)env_sep.nblocks * 36)); LVBA_TRY(dinv_sep.alloc((size_t)bs * 36));
-          LVBA_TRY(zsep.alloc((size_t)bs * 6)); LVBA_TRY(xsep.alloc((size_t)bs * 6));
-          LVBA_TRY(wtop.zero(s)); LVBA_TRY(wbot.zero(s));
-          tw = true;
+    if (!groups.empty()) {
+      // windows are <= 31 poses: always the register-window kernel, one CTA per window
+      n_groups = (int)groups.size() - 1;
+      grp_ptr = groups;
+      std::vector<int> fr((size_t)env.n);
+      for (int g = 0; g < n_groups; ++g) {
+        if (groups[g + 1] - groups[g] > 31)
+          return fail(LVBA_ERR_UNSUPPORTED, "window %d has %d poses; the batched solve handles <= 31 per window", g, groups[g + 1] - groups[g]);
+        for (int r = groups[g]; r < groups[g + 1]; ++r) {
+          if (env.first[r] < groups[g]) return fail(LVBA_ERR_INVALID_ARG, "row %d couples to a pose outside its window", r);
+          fr[r] = env.first[r] - groups[g];
         }
       }
+      LVBA_TRY(first_rel.upload(fr, s));
+      LVBA_TRY(status.alloc((size_t)std::max(n_groups, 4)));
+      LVBA_CUDA(cudaStreamSynchronize(s));
+      path = kSolveBatch;
+      return LVBA_OK;
     }
-    // ---- substructured split
-    nd_on = false;
-    if (reg_ok && (path == LVBA_SOLVE_AUTO || path == LVBA_SOLVE_CHUNKED)) {
-      const int pw1 = (path == LVBA_SOLVE_CHUNKED && chunks >= 2) ? chunks : NdDevice::default_chunks(env.n, std::max(env.max_col, 1));
-      Comm& cm = comm();
-      const int nr = (cm.active() && shard) ? cm.n_ranks : 1;
-      const int pw = (nr > 1 && pw1 < nr) ? nr : pw1;            // one chunk per rank at least: the chunks are the multi-GPU unit
-      if (pw >= 2) {
-        LVBA_TRY(nd.prepare(env.n, env.first, env.last, env.row_start, env.max_col, pw, s, nr, nr > 1 ? cm.rank : 0));
-        if (nr > 1 && !nd.ready && pw1 >= 2) LVBA_TRY(nd.prepare(env.n, env.first, env.last, env.row_start, env.max_col, pw1, s, 1, 0));   // not cuttable per rank
-        nd_on = nd.ready;
-        if (nd_on) LVBA_TRY(status.alloc((size_t)std::max<size_t>(4, nd.plan.nodes.size() + 1)));
-      }
+    // the register-window kernel holds columns of <= 30 blocks; the shared-memory window those of <= kEnvMaxCol
+    const bool reg_ok = env.max_col <= 30 && env.n >= 3;
+    if (want == LVBA_SOLVE_ANY_WIDTH || env.max_col > kEnvMaxCol) {
+      LVBA_TRY(colT.alloc((size_t)std::max(env.max_col, 1) * 36));
+      path = LVBA_SOLVE_ANY_WIDTH;
+    } else if (want != LVBA_SOLVE_SHARED_WINDOW && reg_ok) {
+      if (want == LVBA_SOLVE_AUTO || want == LVBA_SOLVE_CHUNKED) LVBA_TRY(prepare_chunked(env, s, want == LVBA_SOLVE_CHUNKED ? chunks : 0));
+      if (path == LVBA_SOLVE_AUTO && (want == LVBA_SOLVE_AUTO ? env.n >= 256 : want == LVBA_SOLVE_TWISTED)) LVBA_TRY(prepare_twisted(env, s));
+      if (path == LVBA_SOLVE_AUTO) path = LVBA_SOLVE_ONE_CTA;
     }
+    if (path == LVBA_SOLVE_AUTO) path = LVBA_SOLVE_SHARED_WINDOW;
+    if (want != LVBA_SOLVE_AUTO && path != want)
+      return fail(LVBA_ERR_UNSUPPORTED, "path %d is not available for this structure (n = %d, tallest column %d blocks): would take path %d", want, env.n, env.max_col, path);
+    return LVBA_OK;
+  }
+  // substructured split: p chunks (chunks < 2: default_chunks); sets path = LVBA_SOLVE_CHUNKED if the structure can be cut
+  int prepare_chunked(const Envelope& env, cudaStream_t s, int chunks) {
+    const int pw1 = chunks >= 2 ? chunks : NdDevice::default_chunks(env.n, std::max(env.max_col, 1));
+    Comm& cm = comm();
+    const int nr = cm.active() ? cm.n_ranks : 1;                   // the chunks are the multi-GPU unit (SURVEY.md 8(e))
+    const int pw = (nr > 1 && pw1 < nr) ? nr : pw1;                // one chunk per rank at least
+    if (pw < 2) return LVBA_OK;
+    LVBA_TRY(nd.prepare(env.n, env.first, env.last, env.row_start, env.max_col, pw, s, nr, nr > 1 ? cm.rank : 0));
+    if (nr > 1 && !nd.ready && pw1 >= 2) LVBA_TRY(nd.prepare(env.n, env.first, env.last, env.row_start, env.max_col, pw1, s, 1, 0));   // not cuttable per rank
+    if (!nd.ready) return LVBA_OK;
+    LVBA_TRY(status.alloc((size_t)std::max<size_t>(4, nd.plan.nodes.size() + 1)));
+    path = LVBA_SOLVE_CHUNKED;
+    return LVBA_OK;
+  }
+  // twisted split: top half in natural order, bottom half reversed, joined at a separator of tw_bs rows; worthwhile when each
+  // half is many pivots long.  Sets path = LVBA_SOLVE_TWISTED if the split fits the register window
+  int prepare_twisted(const Envelope& env, cudaStream_t s) {
+    const int n = env.n;
+    if (n < 8) return LVBA_OK;
+    const int m = n / 2;
+    const int send = env.last[m - 1] + 1;            // rows >= send do not couple to rows < m
+    const int bs = send - m;
+    if (bs < 3 || bs > 30 || send >= n - 32) return LVBA_OK;
+    tw_m = m; tw_send = send; tw_bs = bs; tw_nb = n - m; tw_nbstop = n - send;
+    std::vector<int> fb((size_t)tw_nb);
+    for (int rp = 0; rp < tw_nb; ++rp) fb[rp] = n - 1 - env.last[n - 1 - rp];     // reversed row couples up to the original column's last row
+    int64_t dummy = 0;
+    LVBA_TRY(env_bot.build(fb, s, &dummy));
+    std::vector<int> fs((size_t)bs, 0);
+    LVBA_TRY(env_sep.build(fs, s, &dummy));
+    if (env_bot.max_col > 30) return LVBA_OK;
+    LVBA_TRY(Lbot.alloc((size_t)env_bot.nblocks * 36)); LVBA_TRY(dinv_bot.alloc((size_t)tw_nb * 36));
+    LVBA_TRY(zbot.alloc((size_t)tw_nb * 6)); LVBA_TRY(xbot.alloc((size_t)tw_nb * 6));
+    LVBA_TRY(wtop.alloc((size_t)bs * bs * 36)); LVBA_TRY(wbot.alloc((size_t)bs * bs * 36));
+    LVBA_TRY(ztopd.alloc((size_t)bs * 6)); LVBA_TRY(zbotd.alloc((size_t)bs * 6));
+    LVBA_TRY(Lsep.alloc((size_t)env_sep.nblocks * 36)); LVBA_TRY(dinv_sep.alloc((size_t)bs * 36));
+    LVBA_TRY(zsep.alloc((size_t)bs * 6)); LVBA_TRY(xsep.alloc((size_t)bs * 6));
+    LVBA_TRY(wtop.zero(s)); LVBA_TRY(wbot.zero(s));
+    path = LVBA_SOLVE_TWISTED;
     return LVBA_OK;
   }
   static size_t factor_smem() { return sizeof(double) * (2 * kEnvMaxCol * 36 + 36 + 8); }
@@ -522,11 +538,15 @@ struct EnvSolver {
   int launch_factor(int id, int grid, const FactorJob* jobs, cudaStream_t s, int64_t* launches) {
     LVBA_TRY(ensure_map(id, s));
     const unsigned* pm = pair_map[id].p;
-#define LVBA_LAUNCH_LA(PP, TT) env_factor_la_kernel<PP, TT, la_tile2(PP)><<<grid, LaCfg<PP, la_tile2(PP)>::kThreads, LaCfg<PP, la_tile2(PP)>::kSmem, s>>>(jobs, pm, dbg.p)
-#define LVBA_LAUNCH_ID(TT) do { switch (id) { case 0: LVBA_LAUNCH_LA(8, TT); break; case 1: LVBA_LAUNCH_LA(12, TT); break; case 2: LVBA_LAUNCH_LA(16, TT); break; \
-                                   case 3: LVBA_LAUNCH_LA(21, TT); break; case 4: LVBA_LAUNCH_LA(24, TT); break; default: LVBA_LAUNCH_LA(31, TT); } } while (0)
-    if (dbg.p) LVBA_LAUNCH_ID(true); else LVBA_LAUNCH_ID(false);
-#undef LVBA_LAUNCH_ID
+#define LVBA_LAUNCH_LA(PP) env_factor_la_kernel<PP, la_tile2(PP)><<<grid, LaCfg<PP, la_tile2(PP)>::kThreads, LaCfg<PP, la_tile2(PP)>::kSmem, s>>>(jobs, pm)
+    switch (id) {
+      case 0: LVBA_LAUNCH_LA(8); break;
+      case 1: LVBA_LAUNCH_LA(12); break;
+      case 2: LVBA_LAUNCH_LA(16); break;
+      case 3: LVBA_LAUNCH_LA(21); break;
+      case 4: LVBA_LAUNCH_LA(24); break;
+      default: LVBA_LAUNCH_LA(31);
+    }
 #undef LVBA_LAUNCH_LA
     ++*launches;
     return LVBA_OK;
@@ -536,62 +556,20 @@ struct EnvSolver {
     if (nrows > 0) env_dinv_apply_kernel<<<(6 * nrows + 127) / 128, 128, 0, s>>>(nrows, dinv_p, z_p, x_p);
   }
   void launch_backsolve(int grid, const BacksolveJob* bj, cudaStream_t s) { env_backsolve_warp_kernel<<<grid, 64, kBsSmem, s>>>(bj); }
-  void dump_timing(const Envelope& env, cudaStream_t s) {
-    if (!(dbg.p && dbg_dumped < dbg_max_dumps)) return;
-    cudaStreamSynchronize(s);
-    const int nsteps = tw ? tw_m : env.n;
-    std::vector<long long> h((size_t)env.n * 32);
-    cudaMemcpy(h.data(), dbg.p, h.size() * 8, cudaMemcpyDeviceToHost);
-    const int k0 = 64, k1 = nsteps - 64;
-    if (k1 <= k0) return;
-    fprintf(stderr, "[factor timing] n=%d max_col=%d twisted=%d : per role  s1-s0 | s2-s1 | s3-s2 | next s0-s3 | step   (cycles, avg over k=%d..%d)\n", env.n, env.max_col, (int)tw, k0, k1);
-    for (int role = 0; role < 8; ++role) {
-      double acc[5] = {0, 0, 0, 0, 0};
-      for (int k = k0; k < k1; ++k) {
-        const long long* a = &h[((size_t)k * 8 + role) * 4];
-        const long long* b = &h[((size_t)(k + 1) * 8 + role) * 4];
-        acc[0] += a[1] - a[0]; acc[1] += a[2] - a[1]; acc[2] += a[3] - a[2]; acc[3] += b[0] - a[3]; acc[4] += b[0] - a[0];
-      }
-      fprintf(stderr, "  role %d: %8.0f %8.0f %8.0f %8.0f %8.0f\n", role, acc[0] / (k1 - k0), acc[1] / (k1 - k0), acc[2] / (k1 - k0), acc[3] / (k1 - k0), acc[4] / (k1 - k0));
-    }
-    ++dbg_dumped;
-  }
-
-  // Block-diagonal system of independent groups (window BA): group g owns rows grp[g]..grp[g+1]-1; every group
-  // must fit the register window (<= 31 rows).  Call after prepare().
-  int prepare_batch(const Envelope& env, const std::vector<int>& grp, cudaStream_t s) {
-    wide = false;                 // windows are <= 31 poses: always the register-window kernel, one CTA per window
-    n_groups = (int)grp.size() - 1;
-    grp_ptr = grp;
-    std::vector<int> fr((size_t)env.n);
-    for (int g = 0; g < n_groups; ++g) {
-      if (grp[g + 1] - grp[g] > 31)
-        return fail(LVBA_ERR_UNSUPPORTED, "window %d has %d poses; the batched solve handles <= 31 per window", g, grp[g + 1] - grp[g]);
-      for (int r = grp[g]; r < grp[g + 1]; ++r) {
-        if (env.first[r] < grp[g]) return fail(LVBA_ERR_INVALID_ARG, "row %d couples to a pose outside its window", r);
-        fr[r] = env.first[r] - grp[g];
-      }
-    }
-    LVBA_TRY(first_rel.upload(fr, s));
-    LVBA_TRY(status.alloc((size_t)std::max(n_groups, 4)));
-    LVBA_CUDA(cudaStreamSynchronize(s));
-    batch = true; tw = false; nd_on = false; jobs_x = nullptr;
-    return LVBA_OK;
-  }
 
   int build_jobs(const Envelope& env, double* x, cudaStream_t s) {
     if (jobs_x == x && d_fjobs.p) return LVBA_OK;
     const EnvView v = env.view();
     std::vector<FactorJob> fj;
     std::vector<BacksolveJob> bj;
-    if (batch) {
+    if (path == kSolveBatch) {
       for (int g = 0; g < n_groups; ++g) {
         const int r0 = grp_ptr[g], ng = grp_ptr[g + 1] - r0;
         EnvView vg{ng, first_rel.p + r0, env.d_row_start.p + r0, env.d_last.p + r0, env.nblocks};
         fj.push_back(FactorJob{vg, L.p, dinv.p + 36 * (size_t)r0, z.p + 6 * (size_t)r0, ng, nullptr, nullptr, status.p + g});
         bj.push_back(BacksolveJob{vg, L.p, x + 6 * (size_t)r0, ng});
       }
-    } else if (tw) {
+    } else if (path == LVBA_SOLVE_TWISTED) {
       EnvView vt = v; vt.n = tw_send;                               // the top instance is a prefix of the matrix
       const EnvView vb = env_bot.view(), vs = env_sep.view();
       fj.push_back(FactorJob{vt, L.p, dinv.p, z.p, tw_m, wtop.p, ztopd.p, status.p});
@@ -619,8 +597,7 @@ struct EnvSolver {
     auto record = [&](int64_t* n_launch) -> int {
       NdCudaExec ex;
       ex.s = s;
-      ex.dense_map = nd.dense_sep ? nd.d_dense_map.p : nullptr;
-      ex.pipeline = nd.pipeline;
+      ex.dense_map = nd.d_dense_map.p;
       ex.factor_fn = [&](int max_col, int nj, const FactorJob* jobs) { return launch_factor(pid(max_col), nj, jobs, s, &ex.launches); };
       ex.back_fn = [&](int nj, const BacksolveJob* jobs) { launch_backsolve(nj, jobs, s); };
       cudaMemsetAsync(status.p, 0, status.n * sizeof(int), s);
@@ -634,8 +611,7 @@ struct EnvSolver {
       Comm& cm = comm();
       NdCudaExec ex;
       ex.s = s;
-      ex.dense_map = nd.dense_sep ? nd.d_dense_map.p : nullptr;
-      ex.pipeline = nd.pipeline;
+      ex.dense_map = nd.d_dense_map.p;
       ex.factor_fn = [&](int max_col, int nj, const FactorJob* jobs) { return launch_factor(pid(max_col), nj, jobs, s, &ex.launches); };
       ex.back_fn = [&](int nj, const BacksolveJob* jobs) { launch_backsolve(nj, jobs, s); };
       cudaMemsetAsync(status.p, 0, status.n * sizeof(int), s);
@@ -681,7 +657,7 @@ struct EnvSolver {
   // dadd (const is cast away for that), z must be valid everywhere, x comes back complete on every rank.  status[0] != 0 afterwards flags a
   // singular pivot (batched mode: status[g] per group).
   int solve(const Envelope& env, const double* H, const double* dadd, double* x, cudaStream_t s, int64_t* launches) {
-    if (nd_on && !batch) return solve_nd(env, H, dadd, x, s, launches);
+    if (path == LVBA_SOLVE_CHUNKED) return solve_nd(env, H, dadd, x, s, launches);
     const EnvView v = env.view();
     LVBA_CUDA(cudaMemcpyAsync(L.p, H, (size_t)env.nblocks * 36 * sizeof(double), cudaMemcpyDeviceToDevice, s));
     LVBA_CUDA(cudaMemsetAsync(status.p, 0, status.n * sizeof(int), s));
@@ -689,7 +665,7 @@ struct EnvSolver {
     env_add_diag_kernel<<<(n6 + 255) / 256, 256, 0, s>>>(v, dadd, L.p);
     ++*launches;
     const int mc = env.max_col;
-    if (wide) {
+    if (path == LVBA_SOLVE_ANY_WIDTH) {
       // ---------------- any width: every column step spread over the device (envelope_wide.h); 4 launches per block row
       const wide::View wv{env.n, env.d_first.p, env.d_row_start.p};                                       // z holds the right-hand side (written by the caller)
       int64_t n_launch = 0;
@@ -703,21 +679,19 @@ struct EnvSolver {
       LVBA_CUDA(cudaGetLastError());
       return LVBA_OK;
     }
-    const bool reg_path = batch || (mc <= 30 && env.n >= 3 && !force_generic);
-    if (reg_path) LVBA_TRY(build_jobs(env, x, s));
-    if (batch) {
+    if (path != LVBA_SOLVE_SHARED_WINDOW) LVBA_TRY(build_jobs(env, x, s));
+    if (path == kSolveBatch) {
       LVBA_TRY(launch_factor(pid(mc), n_groups, d_fjobs.p, s, launches));
       launch_apply(env.n, dinv.p, z.p, x, s);
       launch_backsolve(n_groups, d_bjobs.p, s);
       *launches += 2;
-    } else if (reg_path && tw) {
+    } else if (path == LVBA_SOLVE_TWISTED) {
       // ---------------- twisted: two half factorisations on two SMs, joined at the separator
       const int n = env.n, m = tw_m, bs = tw_bs;
       const EnvView vb = env_bot.view();
       env_reverse_gather_kernel<<<std::min(tw_nb, 2048), 128, 0, s>>>(v, vb, L.p, Lbot.p, z.p, zbot.p);
       ++*launches;
       LVBA_TRY(launch_factor(pid(std::max(mc, env_bot.max_col)), 2, d_fjobs.p, s, launches));
-      dump_timing(env, s);
       env_twist_combine_kernel<<<1, 1024, 0, s>>>(v, m, bs, L.p, z.p, wtop.p, wbot.p, ztopd.p, zbotd.p, Lsep.p, zsep.p);
       ++*launches;
       LVBA_TRY(launch_factor(pid(env_sep.max_col), 1, d_fjobs.p + 2, s, launches));
@@ -730,9 +704,8 @@ struct EnvSolver {
       env_twist_scatter_kernel<<<(tw_nbstop * 6 + 255) / 256, 256, 0, s>>>(n, tw_nbstop, xbot.p, x);
       env_status_or_kernel<<<1, 32, 0, s>>>(status.p, 3);
       *launches += 8;
-    } else if (reg_path) {
+    } else if (path == LVBA_SOLVE_ONE_CTA) {
       LVBA_TRY(launch_factor(pid(mc), 1, d_fjobs.p, s, launches));
-      dump_timing(env, s);
       launch_apply(env.n, dinv.p, z.p, x, s);
       launch_backsolve(1, d_bjobs.p, s);
       *launches += 2;

@@ -50,3 +50,11 @@ def make(first_raw, seed, indefinite=True, fill=0.85):
 
 def reference_solve(A, rhs):
     return spla.spsolve(A, rhs)
+
+
+def damped(br, bc, blocks, n, u):
+    """first[] and dadd = u diag(A) of a system as get_system() returns it (envelope blocks row by row, the diagonal block
+    last in each row): the damped system the LM step solves"""
+    first = np.full(n, n, np.int32)
+    np.minimum.at(first, br, bc)
+    return first, u * np.concatenate([np.diag(b) for b in blocks[br == bc]])

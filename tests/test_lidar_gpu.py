@@ -13,6 +13,7 @@ voxel and ~1e-9..1e-10 relative on the sum.  Stated tolerances:
 import numpy as np
 import pytest
 
+import solver_systems as ss
 from oracle import lidar_oracle as lo
 from oracle import synth
 
@@ -148,20 +149,27 @@ def test_config_B_single_iteration_cost_match(gpu_pkg):
     P.close()
 
 
-def test_twisted_and_single_ended_factorisation_agree(gpu_pkg, monkeypatch):
+def test_twisted_and_single_ended_factorisation_agree(gpu_pkg):
     """n >= 256 pose systems are factorised from both ends on two SMs (top half natural order, bottom half
-    reversed, joined at a separator).  Same solution as the single-ended and the generic kernels."""
+    reversed, joined at a separator).  Same solution as the single-ended and the shared-window kernels, and as the
+    LM step on the same system."""
     p = synth.make_config("B", visual=False)
-    dx = {}
-    for mode, env in (("twisted", {}), ("single", {"LVBA_NO_TWIST": "1"}), ("generic", {"LVBA_FORCE_GENERIC_SOLVER": "1"})):
-        for k in ("LVBA_NO_TWIST", "LVBA_FORCE_GENERIC_SOLVER"):
-            monkeypatch.delenv(k, raising=False)
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
-        P = gpu_pkg.LidarProblem(p["vox_ptr"], p["pose_idx"], p["clusters"], p["poses"])
-        P.build()
-        dx[mode] = P.solve(0.05)
-        P.close()
-    ref = np.abs(dx["generic"]).max()
-    assert np.abs(dx["twisted"] - dx["generic"]).max() <= 1e-8 * ref
-    assert np.abs(dx["single"] - dx["generic"]).max() <= 1e-8 * ref
+    W = 500
+    P = gpu_pkg.LidarProblem(p["vox_ptr"], p["pose_idx"], p["clusters"], p["poses"])
+    P.build()
+    g, br, bc, bl = P.get_system()
+    dx = P.solve(0.05)
+    P.close()
+    first, dadd = ss.damped(br, bc, bl, W, 0.05)
+    _, _, info = gpu_pkg.env_solve(first, bl, dadd, -g.ravel())
+    assert info["path"] == gpu_pkg.SOLVE_TWISTED, info
+    ref = np.abs(dx).max()
+    paths = (gpu_pkg.SOLVE_TWISTED, gpu_pkg.SOLVE_ONE_CTA, gpu_pkg.SOLVE_SHARED_WINDOW)
+    x = {}
+    for path in paths:
+        x[path], _, info = gpu_pkg.env_solve(first, bl, dadd, -g.ravel(), path=path)
+        assert info["path"] == path
+        assert np.abs(x[path] - dx).max() <= 1e-8 * ref, (path, np.abs(x[path] - dx).max())
+    for a in paths:
+        for b in paths:
+            assert np.abs(x[a] - x[b]).max() <= 1e-8 * ref, (a, b)

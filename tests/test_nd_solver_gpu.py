@@ -103,19 +103,18 @@ def test_singular_pivot_is_reported(pkg):
 
 
 def test_spike_beside_the_factorisation_gives_the_same_solution(pkg, monkeypatch):
-    """LVBA_ND_PIPELINE: the spike kernels either start beside the factorisation they read from (programmatic dependent launch +
-    progress counters) or after it; the arithmetic is the same up to the order of the SYRK's RED.ADDs, so the solutions agree to
-    rounding — also without the CUDA graph, and repeatedly (a consumer that ran ahead of its producer would read stale columns
-    only now and then, and be wrong by far more than rounding)."""
+    """The spike kernels start beside the factorisation they read from (programmatic dependent launch + progress counters);
+    the arithmetic is fixed up to the order of the SYRK's RED.ADDs, so repeated solves agree to rounding — also without the
+    CUDA graph (a consumer that ran ahead of its producer would read stale columns only now and then, and be wrong by far
+    more than rounding)."""
     first, blocks, dadd, rhs, A = ss.make(band(2000, 30), seed=77)
-    monkeypatch.setenv("LVBA_ND_PIPELINE", "0")
-    x_seq, _, info = pkg.env_solve(first, blocks, dadd, rhs, path=pkg.SOLVE_CHUNKED, chunks=16)
+    x0, _, info = pkg.env_solve(first, blocks, dadd, rhs, path=pkg.SOLVE_CHUNKED, chunks=16)
     assert info["chunks"] == 16
     xr = ss.reference_solve(A, rhs)
-    assert np.abs(x_seq - xr).max() <= TOL * np.abs(xr).max()
+    assert np.abs(x0 - xr).max() <= TOL * np.abs(xr).max()
     for graph in ("1", "0"):
-        monkeypatch.setenv("LVBA_ND_PIPELINE", "1")
         monkeypatch.setenv("LVBA_ND_GRAPH", graph)
         for rep in range(5):
             x_pipe, _, _ = pkg.env_solve(first, blocks, dadd, rhs, path=pkg.SOLVE_CHUNKED, chunks=16, reps=3)
-            assert np.abs(x_pipe - x_seq).max() <= 1e-11 * np.abs(xr).max(), (graph, rep, np.abs(x_pipe - x_seq).max())
+            assert np.abs(x_pipe - xr).max() <= TOL * np.abs(xr).max(), (graph, rep, np.abs(x_pipe - xr).max())
+            assert np.abs(x_pipe - x0).max() <= 1e-11 * np.abs(xr).max(), (graph, rep, np.abs(x_pipe - x0).max())

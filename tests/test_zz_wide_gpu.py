@@ -34,24 +34,33 @@ def _run(body, env=None, timeout=600):
 
 
 @pytest.mark.gpu
-def test_forced_wide_path_reproduces_the_banded_step(tmp_path):
-    body = """
-    p = synth.make_problem(60, 900, 400, seed=21)
-    P = pkg.LidarProblem(p["vox_ptr"], p["pose_idx"], p["clusters"], p["poses"]); P.build()
-    dx = P.solve(0.01); P.close()
-    np.save(%r, dx)
-    q, t, X, s = pkg.visual_lm(p["q"], p["t"], p["X"], p["plane_nd"], p["obs_ptr"], p["obs_cam"], p["obs_uv"], p["intr"], p["sigma_px"], p["sigma_plane"])
-    np.save(%r, np.array([s["cost_last"], s["iterations"]]))
-    """
-    a, b = str(tmp_path / "narrow_dx.npy"), str(tmp_path / "narrow_v.npy")
-    c, d = str(tmp_path / "wide_dx.npy"), str(tmp_path / "wide_v.npy")
-    _run(body % (a, b))
-    _run(body % (c, d), env={"LVBA_FORCE_WIDE_SOLVER": "1"})
+def test_forced_wide_path_reproduces_the_banded_step(gpu_pkg):
     import numpy as np
-    dn, dw = np.load(a), np.load(c)
-    assert np.abs(dn - dw).max() <= 1e-9 * np.abs(dn).max()
-    vn, vw = np.load(b), np.load(d)
-    assert vn[1] == vw[1] and abs(vn[0] - vw[0]) <= 1e-9 * vn[0]
+    import solver_systems as ss
+    from oracle import synth
+    pkg = gpu_pkg
+    p = synth.make_problem(60, 900, 400, seed=21)
+    # LiDAR: the any-width path on the pose system against the LM step (an in-SM path)
+    P = pkg.LidarProblem(p["vox_ptr"], p["pose_idx"], p["clusters"], p["poses"]); P.build()
+    g, br, bc, bl = P.get_system()
+    dx = P.solve(0.01); P.close()
+    first, dadd = ss.damped(br, bc, bl, P.W, 0.01)
+    xw, _, info = pkg.env_solve(first, bl, dadd, -g.ravel(), path=pkg.SOLVE_ANY_WIDTH)
+    assert info["path"] == pkg.SOLVE_ANY_WIDTH
+    assert np.abs(xw - dx).max() <= 1e-9 * np.abs(dx).max()
+    # visual: the reduced camera system at the initial state and after a few LM iterations, any-width against AUTO
+    V = pkg.VisualProblem(p["q"], p["t"], p["X"], p["plane_nd"], p["obs_ptr"], p["obs_cam"], p["obs_uv"], p["intr"], p["sigma_px"], p["sigma_plane"])
+    V.step(1e4)
+    systems = [V.get_system()]
+    V.iterate(3)
+    systems.append(V.get_system())
+    V.close()
+    for k, (cam, rhs, br, bc, bl) in enumerate(systems):
+        first, dadd = ss.damped(br, bc, bl, len(cam), 1e-4)
+        xa, _, ia = pkg.env_solve(first, bl, dadd, rhs.ravel())
+        xw, _, iw = pkg.env_solve(first, bl, dadd, rhs.ravel(), path=pkg.SOLVE_ANY_WIDTH)
+        assert ia["path"] != pkg.SOLVE_ANY_WIDTH and iw["path"] == pkg.SOLVE_ANY_WIDTH
+        assert np.abs(xw - xa).max() <= 1e-9 * np.abs(xa).max(), (k, np.abs(xw - xa).max() / np.abs(xa).max())
 
 
 @pytest.mark.gpu
