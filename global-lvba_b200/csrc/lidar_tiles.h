@@ -7,7 +7,8 @@
 //   * cut_ranges: consecutive voxels into tiles of <= max_slots slots and <= max_vox voxels, never across a window.
 //   * build_runs: per tile, the (slot i, slot j) pose pairs grouped by destination H block, and the slots grouped by pose
 //     (diagonal blocks and gradient rows).  Functors over items run by an execution policy: CudaExec (exec.cuh) in the
-//     library, the host policy of tests/emu in the CPU tests.
+//     library, the host policy of tests/emu in the CPU tests.  Its radix sort and run passes (sort_runs) also build the
+//     table of the reduced camera system build (visual_tiles.h).
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -81,9 +82,9 @@ struct PairCountF {
 };
 
 // one item per pose pair (i < j) of a voxel: key = (tile, lower-envelope block (pose_j, pose_i)), code = li | lj << 16 (slots
-// local to the tile)
+// local to the tile).  key / code are set by sort_runs.
 struct PairKeyF {
-  TableIn in; uint64_t* key; uint32_t* code;
+  TableIn in; uint64_t* key = nullptr; uint32_t* code = nullptr;
   LVBA_THD void operator()(int64_t p) const {
     const TableIn& q = in;
     int64_t t = 0, hi = q.n_tiles;                            // tile: the last one starting at or before p
@@ -106,7 +107,7 @@ struct PairKeyF {
 
 // one item per slot: key = (tile, pose), code = slot local to the tile
 struct SlotKeyF {
-  TableIn in; uint64_t* key; uint32_t* code;
+  TableIn in; uint64_t* key = nullptr; uint32_t* code = nullptr;
   LVBA_THD void operator()(int64_t s) const {
     const TableIn& q = in;
     int64_t t = 0, hi = q.n_tiles;
@@ -116,25 +117,28 @@ struct SlotKeyF {
   }
 };
 
-// items 0..n: flag[p] = 1 where a run of equal keys starts (flag[n] = 0)
+// The sorted keys are tile * tile_keys + destination, followed by the items that have no destination (key = end, the number of
+// tiles times tile_keys).  items 0..n: flag[p] = 1 where a run of equal keys starts (flag[n] = 0)
 struct RunFlagF {
-  const uint64_t* key; int64_t n; int64_t* flag;
-  LVBA_THD void operator()(int64_t p) const { flag[p] = (p < n && (p == 0 || key[p] != key[p - 1])) ? 1 : 0; }
+  const uint64_t* key; int64_t n; uint64_t end; int64_t* flag;
+  LVBA_THD void operator()(int64_t p) const { flag[p] = (p < n && key[p] < end && (p == 0 || key[p] != key[p - 1])) ? 1 : 0; }
 };
-// items 0..n: run_ptr[r] = first item of run r, run_ptr[R] = n
+// items 0..n: run_ptr[r] = first item of run r, run_ptr[R] = the first item without a destination (n when there is none)
 struct RunStartF {
-  const int64_t* flag; const int64_t* pos; int64_t n; int64_t* run_ptr;
+  const uint64_t* key; const int64_t* flag; const int64_t* pos; int64_t n; uint64_t end; int64_t* run_ptr;
   LVBA_THD void operator()(int64_t p) const {
-    if (p == n) run_ptr[pos[n]] = n;
+    if (p == n || key[p] >= end) { if (p == 0 || key[p - 1] < end) run_ptr[pos[p]] = p; }
     else if (flag[p]) run_ptr[pos[p]] = p;
   }
 };
-// items 0..n_tiles: tile_run[t] = first run of tile t (the items of a tile are contiguous: the tile is the key's major part)
+// items 0..n_tiles: tile_run[t] = first run of tile t, the run of the first sorted key >= t * tile_keys
 struct TileRunF {
-  TableIn in; const int64_t* pos; bool by_slot; int64_t* tile_run;
+  const uint64_t* key; int64_t n; uint64_t tile_keys; const int64_t* pos; int64_t* tile_run;
   LVBA_THD void operator()(int64_t t) const {
-    const int v = in.tile_vox[t];
-    tile_run[t] = pos[by_slot ? (int64_t)in.vox_ptr[v] : (int64_t)in.vox_pair[v]];
+    const uint64_t k = (uint64_t)t * tile_keys;
+    int64_t lo = 0, hi = n;
+    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (key[m] < k) lo = m + 1; else hi = m; }
+    tile_run[t] = pos[lo];
   }
 };
 
@@ -147,32 +151,41 @@ struct Runs {
   int64_t n_runs = 0;
 };
 
-// by_slot = false: the pose pairs of every voxel (n = vox_pair[V]) grouped by H block; true: the slots (n = vox_ptr[V])
-// grouped by pose.  Inside a run the items keep their enumeration order (stable sort).
-template <class Ex>
-int build_runs(Ex& ex, const TableIn& in, bool by_slot, int64_t n, Runs<Ex>& out) {
+// The n items of KeyF (a functor over items with members key and code: key = tile * tile_keys + destination < tile_keys, or
+// n_tiles * tile_keys for an item without a destination) grouped by destination.  Inside a run the items keep their enumeration
+// order (stable sort).
+template <class Ex, class KeyF>
+int sort_runs(Ex& ex, int64_t n, int64_t n_tiles, uint64_t tile_keys, KeyF kf, Runs<Ex>& out) {
 #define LVBA_TILES_TRY(call) do { int rc__ = (call); if (rc__ != 0) return rc__; } while (0)
   typename Ex::template Buf<uint64_t> key, key_s;
   typename Ex::template Buf<uint32_t> code;
   typename Ex::template Buf<int64_t> flag, pos;
   LVBA_TILES_TRY(key.alloc((size_t)n)); LVBA_TILES_TRY(key_s.alloc((size_t)n));
   LVBA_TILES_TRY(code.alloc((size_t)n)); LVBA_TILES_TRY(out.code.alloc((size_t)n));
-  if (by_slot) LVBA_TILES_TRY(ex.for_each(n, SlotKeyF{in, key.p, code.p}));
-  else LVBA_TILES_TRY(ex.for_each(n, PairKeyF{in, key.p, code.p}));
-  const uint64_t max_key = (uint64_t)(in.n_tiles > 0 ? in.n_tiles : 1) * (uint64_t)(by_slot ? in.W : in.nblocks);
+  kf.key = key.p; kf.code = code.p;
+  LVBA_TILES_TRY(ex.for_each(n, kf));
+  const uint64_t end = (uint64_t)n_tiles * tile_keys;
   int bits = 1;
-  while (bits < 64 && (max_key >> bits) != 0) ++bits;
+  while (bits < 64 && (end >> bits) != 0) ++bits;
   LVBA_TILES_TRY(ex.sort_pairs(key.p, key_s.p, code.p, out.code.p, n, bits));
   LVBA_TILES_TRY(flag.alloc((size_t)n + 1)); LVBA_TILES_TRY(pos.alloc((size_t)n + 1));
-  LVBA_TILES_TRY(ex.for_each(n + 1, RunFlagF{key_s.p, n, flag.p}));
+  LVBA_TILES_TRY(ex.for_each(n + 1, RunFlagF{key_s.p, n, end, flag.p}));
   LVBA_TILES_TRY(ex.exclusive_scan(flag.p, pos.p, n + 1));
   LVBA_TILES_TRY(ex.fetch(&out.n_runs, pos.p + n, 1));
   LVBA_TILES_TRY(out.run_ptr.alloc((size_t)out.n_runs + 1));
-  LVBA_TILES_TRY(ex.for_each(n + 1, RunStartF{flag.p, pos.p, n, out.run_ptr.p}));
-  LVBA_TILES_TRY(out.tile_run.alloc((size_t)in.n_tiles + 1));
-  LVBA_TILES_TRY(ex.for_each(in.n_tiles + 1, TileRunF{in, pos.p, by_slot, out.tile_run.p}));
+  LVBA_TILES_TRY(ex.for_each(n + 1, RunStartF{key_s.p, flag.p, pos.p, n, end, out.run_ptr.p}));
+  LVBA_TILES_TRY(out.tile_run.alloc((size_t)n_tiles + 1));
+  LVBA_TILES_TRY(ex.for_each(n_tiles + 1, TileRunF{key_s.p, n, tile_keys, pos.p, out.tile_run.p}));
   return ex.sync();                                          // the scratch buffers are released on return
 #undef LVBA_TILES_TRY
+}
+
+// by_slot = false: the pose pairs of every voxel (n = vox_pair[V]) grouped by H block; true: the slots (n = vox_ptr[V])
+// grouped by pose.
+template <class Ex>
+int build_runs(Ex& ex, const TableIn& in, bool by_slot, int64_t n, Runs<Ex>& out) {
+  if (by_slot) return sort_runs(ex, n, in.n_tiles, (uint64_t)in.W, SlotKeyF{in}, out);
+  return sort_runs(ex, n, in.n_tiles, (uint64_t)in.nblocks, PairKeyF{in}, out);
 }
 
 }  // namespace tiles

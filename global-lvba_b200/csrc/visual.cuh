@@ -9,32 +9,50 @@
 //   ceres-solver 2.1.0 (not vendored): Jacobi column scaling, LM diagonal, Schur complement,
 //   EigenQuaternionManifold on {w,x,y,z} memory (SURVEY.md Q9-Q11, Appendix A.2/A.3).
 //
-// Schedule: the observations of the landmarks that have a valid plane are stored CSR and cut into
-// batches of consecutive landmarks with <= kSlots observations; one CTA of kSlots threads per batch.
+// Schedule: the observations of the landmarks that have a valid plane are stored CSR, the landmarks in the order of the
+// lowest system row of their clique (visual_tiles.h).  The build and the column norms cut them into tiles of consecutive
+// landmarks with <= kVisTileSlots observations, one CTA of kVisTileSlots threads each; back-substitution and the cost cut the
+// same order into batches of <= kSlots observations, one CTA of kSlots threads each.
 //   phase 1  thread = observation: r (2), J_cam (2x6, tangent), J_X (2x3); J_X^T J_X, J_X^T r staged
 //   phase 2  thread = landmark   : C = sum J_X^T J_X + plane term + D_p^2, C^-1, g_p, w = C^-1 g_p
 //   phase 3  thread = observation: E = J_c^T J_X, Y = E C^-1, diagonal block J_c^T J_c - Y E^T,
 //                                  reduced rhs -(g_c - E w), column norms; factors [Y|E] to shared memory
-//   phase 4  warp = 8 camera pairs: S(hi,lo)[a][b] -= sum_m Y_hi[a][m] E_lo[b][m]  (3 FMA + RED.ADD.F64)
+//   phase 4  every distinct S block, diagonal block and camera row of the tile is summed on chip and written with one
+//            RED.ADD.F64 per element.  A destination table built once per structure lists the tile's camera-pair
+//            contributions grouped by S block and its observations grouped by row.  Off-diagonal blocks: four lanes per
+//            block sum S(hi,lo)[a][b] -= sum_m Y_hi[a][m] E_lo[b][m] over the block's pairs in registers.  Diagonal blocks,
+//            rhs, column norms and gradient: staged in shared memory and summed per row.
+//            Sorted landmarks share cameras: at config C a 256-slot tile holds 3.9 pair contributions per distinct block
+//            and 12 observations per row, and the element REDs per build fall from 79 M (one per pair and observation) to
+//            15 M.
 // The Jacobian is never materialised in HBM; back-substitution recomputes it.
 #pragma once
 #include "common.cuh"
 #include "envelope.cuh"
 #include "lidar.cuh"   // kSlots, kStageStride, reduce kernels
+#include "visual_tiles.h"
 
 namespace lvba {
 
+using tiles::kVisTileSlots;
+using tiles::kMaxTrkPerTile;
 constexpr int kMaxTrkPerBatch = 128;
 constexpr int kTrkParams = 16;     // Cinv(6) g_p(3) w(3) y_p(3) pad
 constexpr int kVFStride = 37;      // Y(18) E(18) + pad
 
 struct VisualView {
-  int n_batches;
+  int n_batches;             // back-substitution and cost: batches of <= kSlots observations
+  const int* batch_trk;      // [n_batches+1] landmark range per batch
+  int n_tiles;               // build and column norms: tiles of <= kVisTileSlots observations (visual_tiles.h)
+  const int* tile_trk;       // [n_tiles+1] landmark range per tile
+  const int64_t* tile_prun;  // [n_tiles+1] pair runs of every tile
+  const int64_t* prun_ptr;   // run r = pairs[prun_ptr[r] .. prun_ptr[r+1]): the camera-pair contributions of one S block
+  const unsigned* pairs;     // hi | lo << 16, observations local to the tile (contribution -Y_hi E_lo^T)
+  const int64_t* tile_drun;  // [n_tiles+1] row runs of every tile
+  const int64_t* drun_ptr;   // run r = dslot[drun_ptr[r] .. drun_ptr[r+1]): the observations of one system row
+  const unsigned* dslot;     // observations local to the tile
   const int* trk_ptr;        // [Tv+1] obs offsets (valid landmarks only, compact)
   const int* trk_id;         // [Tv]   original landmark index
-  const int* batch_trk;      // [n_batches+1]
-  const long long* batch_pair;   // [n_batches+1]
-  const unsigned* pairs;     // (hi | lo<<8 | local trk<<16)
   const int* obs_cam;        // [nnz] original camera index
   const int* obs_row;        // [nnz] reduced-system row of that camera, -1 when constant / unused
   const float2* obs_uv;      // [nnz]
@@ -169,14 +187,16 @@ struct VisualLM {
 // ------------------------------------------------------------------------------------------------
 // phase 1+2 shared by build and back-substitution.  Leaves per-landmark params in sT:
 //   [0..5] Cinv  [6..8] g_p  [9..11] w = Cinv g_p ; returns this thread's observation in `o` (scaled)
-template <bool kNeedJac>
-LVBA_DEV void visual_front(const VisualView& vv, const VisualState& st, const VisualLM& lm, int b,
+// The CTA (kThreads threads) takes the landmarks t0 .. t1 (<= kThreads observations, <= 256 landmarks).  With `env`, the
+// envelope row_start / first of the observation's row are loaded beside its camera state (rs, fr; untouched when row < 0).
+template <int kThreads, bool kNeedJac>
+LVBA_DEV void visual_front(const VisualView& vv, const VisualState& st, const VisualLM& lm, int t0, int t1,
                            double* stage, double* sT, ObsEval& o, int& row, int& ltrk, double* Xown,
-                           double& cost_part) {
+                           double& cost_part, const EnvView* env = nullptr, long long* rs = nullptr, int* fr = nullptr) {
   const int tid = threadIdx.x;
-  const int t0 = vv.batch_trk[b], t1 = vv.batch_trk[b + 1], nt = t1 - t0;
+  const int nt = t1 - t0;
   const int s0 = vv.trk_ptr[t0], ns = vv.trk_ptr[t1] - s0;
-  __shared__ unsigned char sTrkOf[kSlots];
+  __shared__ unsigned char sTrkOf[kThreads];
   if (tid < nt) {
     const int lo = vv.trk_ptr[t0 + tid] - s0, hi = vv.trk_ptr[t0 + tid + 1] - s0;
     for (int q = lo; q < hi; ++q) sTrkOf[q] = (unsigned char)tid;
@@ -189,6 +209,7 @@ LVBA_DEV void visual_front(const VisualView& vv, const VisualState& st, const Vi
     const int tr = vv.trk_id[t0 + ltrk];
     const int cam = vv.obs_cam[s0 + tid];
     row = vv.obs_row[s0 + tid];
+    if (env && row >= 0) { *rs = env->row_start[row]; *fr = env->first[row]; }
     Xown[0] = st.X[3 * (long long)tr]; Xown[1] = st.X[3 * (long long)tr + 1]; Xown[2] = st.X[3 * (long long)tr + 2];
     obs_eval<kNeedJac>(vv, st.q + 4 * (long long)cam, st.t + 3 * (long long)cam, Xown, vv.obs_uv[s0 + tid], o);
     cost_part = o.r[0] * o.r[0] + o.r[1] * o.r[1];
@@ -266,37 +287,44 @@ visual_cost_kernel(VisualView vv, VisualState st, double* __restrict__ batch_cos
   int row, ltrk;
   double Xown[3], cp;
   VisualLM lm{1.0, 0.0, 0.0, nullptr, nullptr};
-  visual_front<false>(vv, st, lm, blockIdx.x, nullptr, dummyT, o, row, ltrk, Xown, cp);
+  visual_front<kSlots, false>(vv, st, lm, vv.batch_trk[blockIdx.x], vv.batch_trk[blockIdx.x + 1], nullptr, dummyT, o, row, ltrk, Xown, cp);
   const double tot = block_sum<kSlots>(cp, red);
   if (threadIdx.x == 0) batch_cost[blockIdx.x] = 0.5 * tot;
 }
 
 // ------------------------------------------------------------------------------------------------
-// unscaled squared column norms (Jacobi scaling, computed once at iteration 0)
-__global__ void __launch_bounds__(kSlots)
+// unscaled squared column norms (Jacobi scaling, computed when the scale is reset).  One CTA per build tile: the camera
+// columns are summed per row of the tile (row runs of the destination table) before one RED per element.
+__global__ void __launch_bounds__(kVisTileSlots)
 visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_colsq, double* __restrict__ pt_colsq) {
+  constexpr int NS = kVisTileSlots, kC = 9;              // per observation: 3 point columns, 6 camera columns
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int t0 = vv.batch_trk[b], t1 = vv.batch_trk[b + 1], nt = t1 - t0;
+  const int t0 = vv.tile_trk[b], t1 = vv.tile_trk[b + 1], nt = t1 - t0;
   const int s0 = vv.trk_ptr[t0], ns = vv.trk_ptr[t1] - s0;
-  __shared__ double stage[kSlots * 4];
+  const int64_t d0 = vv.tile_drun[b];
+  const int nd = (int)(vv.tile_drun[b + 1] - d0);
+  const int64_t q0 = vv.drun_ptr[d0];
+  const int nq = (int)(vv.drun_ptr[d0 + nd] - q0);
+  __shared__ double stage[NS * kC];
+  __shared__ unsigned short sDSlot[NS], sDRun[NS + 1];
   if (tid < ns) {
-    const int lt_lo = 0; (void)lt_lo;
     // locate landmark by scanning is avoided: recompute from trk_ptr with a small search
     int lo = 0, hi = nt;
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (vv.trk_ptr[t0 + mid] - s0 <= tid) lo = mid; else hi = mid; }
     const int tr = vv.trk_id[t0 + lo];
     const int cam = vv.obs_cam[s0 + tid];
-    const int row = vv.obs_row[s0 + tid];
     const double X[3] = {st.X[3 * (long long)tr], st.X[3 * (long long)tr + 1], st.X[3 * (long long)tr + 2]};
     ObsEval o;
     obs_eval<true>(vv, st.q + 4 * (long long)cam, st.t + 3 * (long long)cam, X, vv.obs_uv[s0 + tid], o);
-    if (row >= 0)
+    double* sg = stage + tid * kC;
+    sg[0] = o.JX[0] * o.JX[0] + o.JX[3] * o.JX[3];
+    sg[1] = o.JX[1] * o.JX[1] + o.JX[4] * o.JX[4];
+    sg[2] = o.JX[2] * o.JX[2] + o.JX[5] * o.JX[5];
 #pragma unroll
-      for (int a = 0; a < 6; ++a) atomicAdd(cam_colsq + 6 * (long long)row + a, o.Jc[a] * o.Jc[a] + o.Jc[6 + a] * o.Jc[6 + a]);
-    stage[tid * 4 + 0] = o.JX[0] * o.JX[0] + o.JX[3] * o.JX[3];
-    stage[tid * 4 + 1] = o.JX[1] * o.JX[1] + o.JX[4] * o.JX[4];
-    stage[tid * 4 + 2] = o.JX[2] * o.JX[2] + o.JX[5] * o.JX[5];
+    for (int a = 0; a < 6; ++a) sg[3 + a] = o.Jc[a] * o.Jc[a] + o.Jc[6 + a] * o.Jc[6 + a];
   }
+  if (tid < nq) sDSlot[tid] = (unsigned short)vv.dslot[q0 + tid];
+  for (int r = tid; r <= nd; r += NS) sDRun[r] = (unsigned short)(vv.drun_ptr[d0 + r] - q0);
   __syncthreads();
   if (tid < nt) {
     const int lo = vv.trk_ptr[t0 + tid] - s0, hi = vv.trk_ptr[t0 + tid + 1] - s0;
@@ -305,9 +333,16 @@ visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_co
     double rp, J[3];
     plane_eval(vv, vv.plane + 4 * (long long)(t0 + tid), X, rp, J);
     double a0 = J[0] * J[0], a1 = J[1] * J[1], a2 = J[2] * J[2];
-    for (int s = lo; s < hi; ++s) { a0 += stage[s * 4]; a1 += stage[s * 4 + 1]; a2 += stage[s * 4 + 2]; }
+    for (int s = lo; s < hi; ++s) { a0 += stage[s * kC]; a1 += stage[s * kC + 1]; a2 += stage[s * kC + 2]; }
     double* o = pt_colsq + 3 * (long long)(t0 + tid);
     o[0] = a0; o[1] = a1; o[2] = a2;
+  }
+  for (int e = tid; e < nd * 6; e += NS) {
+    const int r = e / 6, a = e - r * 6;
+    const int qa = sDRun[r], qb = sDRun[r + 1];
+    double v = 0.0;
+    for (int q = qa; q < qb; ++q) v += stage[sDSlot[q] * kC + 3 + a];
+    atomicAdd(cam_colsq + 6 * (long long)vv.obs_row[s0 + sDSlot[qa]] + a, v);
   }
 }
 
@@ -318,29 +353,48 @@ __global__ void visual_scale_kernel(long long n, const double* __restrict__ cols
 }
 
 // ------------------------------------------------------------------------------------------------
-// linearise + Schur-eliminate: S (envelope, lower), rhs, camera column norms, camera gradient
-__global__ void __launch_bounds__(kSlots)
+// linearise + Schur-eliminate: S (envelope, lower), rhs, camera column norms, camera gradient.  One CTA per tile.
+__global__ void __launch_bounds__(kVisTileSlots, 1)
 visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, double* __restrict__ S,
                     double* __restrict__ rhs, double* __restrict__ cam_colsq, double* __restrict__ cam_grad,
                     double* __restrict__ batch_cost, double* __restrict__ batch_gmax) {
+  constexpr int NS = kVisTileSlots;
   extern __shared__ double sm[];
-  double* stage = sm;                                    // [kSlots][kStageStride]
-  double* sF = stage + kSlots * kStageStride;            // [kSlots][kVFStride]   Y | E
-  double* sG = sF + kSlots * kVFStride;                  // [kSlots][18]  rhs | colsq | grad
-  double* sT = sG + kSlots * 18;                         // [kMaxTrkPerBatch][kTrkParams]
-  double* red = sT + kMaxTrkPerBatch * kTrkParams;       // [32]
-  long long* sDiag = reinterpret_cast<long long*>(red + 32);     // [kSlots]
-  long long* sRowRS = sDiag + kSlots;                            // [kSlots] envelope row_start of the camera row
-  int* sRow = reinterpret_cast<int*>(sRowRS + kSlots);           // [kSlots]
-  int* sRowFirst = sRow + kSlots;                                // [kSlots]
+  double* stage = sm;                                    // [NS][kStageStride]
+  double* sF = stage + NS * kStageStride;                // [NS][kVFStride]   Y | E
+  double* sG = sF + NS * kVFStride;                      // [NS][18]  rhs | colsq | grad
+  double* sT = sG + NS * 18;                             // [kMaxTrkPerTile][kTrkParams]
+  double* red = sT + kMaxTrkPerTile * kTrkParams;        // [32]
+  long long* sDiag = reinterpret_cast<long long*>(red + 32);     // [NS]
+  long long* sRowRS = sDiag + NS;                                // [NS] envelope row_start of the camera row
+  int* sRow = reinterpret_cast<int*>(sRowRS + NS);               // [NS]
+  int* sRowFirst = sRow + NS;                                    // [NS]
+  unsigned short* sDSlot = reinterpret_cast<unsigned short*>(sRowFirst + NS);   // [NS] the tile's observations grouped by row
+  unsigned short* sDRun = sDSlot + NS;                           // [NS + 1] row run r = sDSlot[sDRun[r] .. sDRun[r + 1])
 
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int t0 = vv.batch_trk[b], t1 = vv.batch_trk[b + 1], nt = t1 - t0;
-  const int s0 = vv.trk_ptr[t0], ns = vv.trk_ptr[t1] - s0;
+  const int t0 = vv.tile_trk[b], t1 = vv.tile_trk[b + 1], nt = t1 - t0;
+  const int ns = vv.trk_ptr[t1] - vv.trk_ptr[t0];
+  // With one CTA per SM no other CTA hides a dependent global load, so every load that does not depend on phases 1-3 is issued
+  // here, into registers, where it overlaps the loads of phase 1: the tile's row runs and the first pair run of every lane of
+  // phase 4b.  The envelope rows of the observations come with the camera state in visual_front.
+  const int64_t d0 = vv.tile_drun[b];
+  const int nd = (int)(vv.tile_drun[b + 1] - d0);
+  const int64_t q0 = vv.drun_ptr[d0];
+  const bool has_dslot = tid < vv.drun_ptr[d0 + nd] - q0;
+  const unsigned dslot = has_dslot ? vv.dslot[q0 + tid] : 0u;
+  const int64_t drun = tid <= nd ? vv.drun_ptr[d0 + tid] : 0;
+  const int64_t r0 = vv.tile_prun[b], nr = vv.tile_prun[b + 1] - r0;
+  const int pq = lane >> 2, k = lane & 3;
+  int64_t qa = 0, qb = 0;                                // pair run of this lane in the current round of phase 4b
+  unsigned code = 0;
+  if ((int64_t)warp * 8 + pq < nr) { qa = vv.prun_ptr[r0 + warp * 8 + pq]; qb = vv.prun_ptr[r0 + warp * 8 + pq + 1]; code = vv.pairs[qa]; }
   ObsEval o;
   int row, ltrk;
+  long long rs = 0;
+  int fr = 0;
   double Xown[3], cp;
-  visual_front<true>(vv, st, lm, b, stage, sT, o, row, ltrk, Xown, cp);
+  visual_front<NS, true>(vv, st, lm, t0, t1, stage, sT, o, row, ltrk, Xown, cp, &env, &rs, &fr);
   // gradient max-norm (unscaled) of the point blocks
   double gm = 0.0;
   if (tid < nt) {
@@ -349,7 +403,7 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
     gm = fmax(fabs(p[6] / sp[0]), fmax(fabs(p[7] / sp[1]), fabs(p[8] / sp[2])));
   }
   {
-    const double tot = block_sum<kSlots>(cp, red);
+    const double tot = block_sum<NS>(cp, red);
     if (tid == 0) batch_cost[b] = 0.5 * tot;
     // max via the same scratch
 #pragma unroll
@@ -358,7 +412,7 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
     __syncthreads();
     if (tid == 0) {
       double m = 0.0;
-      for (int w = 0; w < kSlots / 32; ++w) m = fmax(m, red[w]);
+      for (int w = 0; w < NS / 32; ++w) m = fmax(m, red[w]);
       batch_gmax[b] = m;
     }
     __syncthreads();
@@ -395,52 +449,52 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
       }
 #pragma unroll
       for (int q = 0; q < 18; ++q) { sf[q] = Y[q]; sf[18 + q] = E[q]; }
-      const long long rs = env.row_start[row];
-      const int fr = env.first[row];
       sRowRS[tid] = rs; sRowFirst[tid] = fr;
       sDiag[tid] = (rs + (row - fr)) * 36;
-    } else {
-      sDiag[tid] = -1;
     }
   }
+  if (has_dslot) sDSlot[tid] = (unsigned short)dslot;
+  if (tid <= nd) sDRun[tid] = (unsigned short)(drun - q0);
+  if (tid == 0 && nd == NS) sDRun[NS] = (unsigned short)(vv.drun_ptr[d0 + NS] - q0);
   __syncthreads();
-  // ---- phase 4a: flush diagonal blocks, rhs, column norms, gradient
-  for (int e = tid; e < ns * 36; e += kSlots) {
-    const int sl = e / 36, el = e - sl * 36;
-    if (sDiag[sl] >= 0) atomicAdd(S + sDiag[sl] + el, stage[sl * kStageStride + el]);
+  // ---- phase 4a: diagonal blocks, rhs, column norms and gradient, summed per row of the tile (nd runs) and written with one
+  //      RED per element
+  for (int e = tid; e < nd * 36; e += NS) {
+    const int r = e / 36, el = e - r * 36;
+    const int qa = sDRun[r], qb = sDRun[r + 1];
+    double v = 0.0;
+    for (int q = qa; q < qb; ++q) v += stage[sDSlot[q] * kStageStride + el];
+    atomicAdd(S + sDiag[sDSlot[qa]] + el, v);
   }
-  for (int e = tid; e < ns * 18; e += kSlots) {
-    const int sl = e / 18, el = e - sl * 18;
-    const int r = sRow[sl];
-    if (r >= 0) {
-      const int which = el / 6, a = el - which * 6;
-      double* dst = (which == 0) ? rhs : (which == 1) ? cam_colsq : cam_grad;
-      atomicAdd(dst + 6 * (long long)r + a, sG[e]);
-    }
+  for (int e = tid; e < nd * 18; e += NS) {
+    const int r = e / 18, el = e - r * 18;
+    const int qa = sDRun[r], qb = sDRun[r + 1];
+    double v = 0.0;
+    for (int q = qa; q < qb; ++q) v += sG[sDSlot[q] * 18 + el];
+    const int which = el / 6, a = el - which * 6;
+    double* dst = (which == 0) ? rhs : (which == 1) ? cam_colsq : cam_grad;
+    atomicAdd(dst + 6 * (long long)sRow[sDSlot[qa]] + a, v);
   }
-  // ---- phase 4b: camera pairs.  Lane (pq, k) = (lane >> 2, lane & 3) owns the elements 4 m + k, m = 0..8, of pair pq (the
-  //      mapping of lidar_build_kernel's phase 4b): one aligned 32-byte sector per pair and instruction, factors read once.
-  const long long p0 = vv.batch_pair[b], np = vv.batch_pair[b + 1] - p0;
-  const int pq = lane >> 2, k = lane & 3;
+  // ---- phase 4b: off-diagonal blocks.  The tile's camera-pair contributions come grouped by destination block (runs); every
+  //      warp takes 8 runs at a time, sums each block in registers over the pairs of its run and writes it with 9 REDs per lane.
+  //      Lane (pq, k) = (lane >> 2, lane & 3) owns the elements 4 m + k, m = 0..8, of run pq (the mapping of
+  //      lidar_build_kernel's phase 4b): one aligned 32-byte sector per run and RED instruction.  The next round's run bounds are
+  //      loaded at the start of a round, its first code after the round's sums.
   const bool upper = k >= 2;
   const int col0 = k, col1 = upper ? k - 2 : 4 + k, col2 = 2 + k;
-  unsigned code_next = 0;
-  {
-    const long long c0 = (long long)warp * 8;
-    if (c0 + pq < np) code_next = vv.pairs[p0 + c0 + pq];
-  }
-  for (long long c = (long long)warp * 8; c < np; c += (kSlots / 32) * 8) {
-    const bool live = c + pq < np;
-    const unsigned code = code_next;
-    {
-      const long long cn = c + (kSlots / 32) * 8;
-      code_next = (cn + pq < np) ? vv.pairs[p0 + cn + pq] : 0u;
-    }
-    if (live) {
-      const int hi = code & 0xff, lo = (code >> 8) & 0xff;
-      double* dst = S + (sRowRS[hi] + (sRow[lo] - sRowFirst[hi])) * 36 + k;
-      const double* y = sF + hi * kVFStride;               // Y_hi, row a at 3 a
-      const double* ee = sF + lo * kVFStride + 18;         // E_lo, row bq at 3 bq
+  for (int64_t c = (int64_t)warp * 8; c < nr; c += (NS / 32) * 8) {
+    const int64_t cn = c + (NS / 32) * 8;
+    int64_t qa_next = 0, qb_next = 0;
+    if (cn + pq < nr) { qa_next = vv.prun_ptr[r0 + cn + pq]; qb_next = vv.prun_ptr[r0 + cn + pq + 1]; }
+    if (c + pq < nr) {
+    double* dst = S + (sRowRS[code & 0xffff] + (sRow[code >> 16] - sRowFirst[code & 0xffff])) * 36 + k;
+    double acc[9];
+#pragma unroll
+    for (int m = 0; m < 9; ++m) acc[m] = 0.0;
+    for (int64_t q = qa; q < qb; ++q) {
+      const unsigned code_next = q + 1 < qb ? vv.pairs[q + 1] : 0u;
+      const double* y = sF + (code & 0xffff) * kVFStride;       // Y_hi, row a at 3 a
+      const double* ee = sF + (code >> 16) * kVFStride + 18;    // E_lo, row bq at 3 bq
       double ce[3][3], ry[6][3];
 #pragma unroll
       for (int t = 0; t < 3; ++t) { ce[0][t] = ee[3 * col0 + t]; ce[1][t] = ee[3 * col1 + t]; ce[2][t] = ee[3 * col2 + t]; }
@@ -451,21 +505,28 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
 #pragma unroll
       for (int m = 0; m < 9; ++m) {
         const int j2 = 2 * (m / 3), ph = m % 3;
-        double r0, r1, r2;
-        if (ph == 0) { r0 = ry[j2][0]; r1 = ry[j2][1]; r2 = ry[j2][2]; }
-        else if (ph == 2) { r0 = ry[j2 + 1][0]; r1 = ry[j2 + 1][1]; r2 = ry[j2 + 1][2]; }
-        else { r0 = upper ? ry[j2 + 1][0] : ry[j2][0]; r1 = upper ? ry[j2 + 1][1] : ry[j2][1]; r2 = upper ? ry[j2 + 1][2] : ry[j2][2]; }
-        const double val = -(r0 * ce[ph][0] + r1 * ce[ph][1] + r2 * ce[ph][2]);
-        atomicAdd(dst + 4 * m, val);
+        double r0_, r1_, r2_;
+        if (ph == 0) { r0_ = ry[j2][0]; r1_ = ry[j2][1]; r2_ = ry[j2][2]; }
+        else if (ph == 2) { r0_ = ry[j2 + 1][0]; r1_ = ry[j2 + 1][1]; r2_ = ry[j2 + 1][2]; }
+        else { r0_ = upper ? ry[j2 + 1][0] : ry[j2][0]; r1_ = upper ? ry[j2 + 1][1] : ry[j2][1]; r2_ = upper ? ry[j2 + 1][2] : ry[j2][2]; }
+        acc[m] -= r0_ * ce[ph][0] + r1_ * ce[ph][1] + r2_ * ce[ph][2];
       }
+      code = code_next;
     }
+#pragma unroll
+    for (int m = 0; m < 9; ++m) atomicAdd(dst + 4 * m, acc[m]);
+    }
+    qa = qa_next; qb = qb_next;
+    code = cn + pq < nr ? vv.pairs[qa] : 0u;
   }
 }
 
 constexpr size_t visual_build_smem_bytes() {
-  return sizeof(double) * (kSlots * kStageStride + kSlots * kVFStride + kSlots * 18 + kMaxTrkPerBatch * kTrkParams + 32)
-       + sizeof(long long) * 2 * kSlots + sizeof(int) * 2 * kSlots + 64;
+  return sizeof(double) * (kVisTileSlots * (kStageStride + kVFStride + 18) + kMaxTrkPerTile * kTrkParams + 32)
+       + sizeof(long long) * 2 * kVisTileSlots + sizeof(int) * 2 * kVisTileSlots + sizeof(unsigned short) * (2 * kVisTileSlots + 1) + 64;
 }
+// the static sTrkOf of visual_front comes on top
+static_assert(visual_build_smem_bytes() + kVisTileSlots <= 227 * 1024, "visual_build_kernel: shared memory above the 227 kB an H100 CTA may hold");
 
 // ------------------------------------------------------------------------------------------------
 // back-substitution y_p = -C^-1 (g_p + sum E^T y_c), model cost change, candidate landmarks
@@ -483,7 +544,7 @@ visual_backsub_kernel(VisualView vv, VisualState st, VisualLM lm, const double* 
   ObsEval o;
   int row, ltrk;
   double Xown[3], cp;
-  visual_front<true>(vv, st, lm, b, stage, sT, o, row, ltrk, Xown, cp);
+  visual_front<kSlots, true>(vv, st, lm, t0, t1, stage, sT, o, row, ltrk, Xown, cp);
   double yc[6] = {0, 0, 0, 0, 0, 0};
   if (tid < ns) {
     if (row >= 0)

@@ -5,21 +5,20 @@
 #include <cmath>
 #include <memory>
 
+#include "exec.cuh"
 #include "runtime.cuh"   // (pulls comm.cuh in)
-#include "runtime.cuh"
 #include "visual.cuh"
 
 struct lvba_visual_problem {
   int M = 0;
   long long T = 0, Tv = 0, nnz = 0, n_pairs = 0;
-  int n_rows = 0, n_batches = 0, device = 0, fixed_cam = 0;
+  int n_rows = 0, n_batches = 0, n_tiles = 0, device = 0, fixed_cam = 0;
   std::vector<int> cam_of_row;
   cudaStream_t stream = nullptr;
   double intr[8];
   double sigma_px = 1, sigma_pl = 1;
-  lvba::DevBuf<int> trk_ptr, trk_id, batch_trk, obs_cam, obs_row, d_cam_of_row;
-  lvba::DevBuf<long long> batch_pair;
-  lvba::DevBuf<unsigned> pairs;
+  lvba::DevBuf<int> trk_ptr, trk_id, batch_trk, tile_trk, obs_cam, obs_row, d_cam_of_row;
+  lvba::tiles::Runs<lvba::CudaExec> prun, drun;   // the build's destination table: pair contributions by S block, observations by row
   lvba::DevBuf<float2> obs_uv;
   lvba::DevBuf<double> plane;
   lvba::DevBuf<double> q, t, X, qc, tc, Xc;         // state and candidate
@@ -40,8 +39,10 @@ struct lvba_visual_problem {
 
   lvba::VisualView view() const {
     lvba::VisualView v;
-    v.n_batches = n_batches; v.trk_ptr = trk_ptr.p; v.trk_id = trk_id.p; v.batch_trk = batch_trk.p;
-    v.batch_pair = batch_pair.p; v.pairs = pairs.p; v.obs_cam = obs_cam.p; v.obs_row = obs_row.p;
+    v.n_batches = n_batches; v.batch_trk = batch_trk.p; v.n_tiles = n_tiles; v.tile_trk = tile_trk.p;
+    v.tile_prun = prun.tile_run.p; v.prun_ptr = prun.run_ptr.p; v.pairs = prun.code.p;
+    v.tile_drun = drun.tile_run.p; v.drun_ptr = drun.run_ptr.p; v.dslot = drun.code.p;
+    v.trk_ptr = trk_ptr.p; v.trk_id = trk_id.p; v.obs_cam = obs_cam.p; v.obs_row = obs_row.p;
     v.obs_uv = obs_uv.p; v.plane = plane.p;
     for (int i = 0; i < 8; ++i) v.intr[i] = intr[i];
     v.inv_sigma_px = 1.0 / sigma_px;
@@ -58,9 +59,9 @@ struct lvba_visual_problem {
 
 namespace lvba {
 
-// ---- set-up kernels: the per-observation arrays and the pair table are derived on the device from the caller's arrays
-// (uploaded as they are: one DMA each from the caller's — ideally pinned — memory) instead of being gathered on the host
-// and pushed through pageable staging copies (config C: 16 MB of observations + 18 MB of pair words).
+// ---- set-up kernel: the per-observation arrays are derived on the device from the caller's arrays (uploaded as they are: one
+// DMA each from the caller's — ideally pinned — memory) instead of being gathered on the host and pushed through pageable
+// staging copies (config C: 16 MB of observations).
 // One thread per local landmark k (source landmark trk_id[k]): its observations, camera rows and plane.
 __global__ void visual_gather_kernel(long long Tv, const int* __restrict__ trk_id, const int* __restrict__ trk_ptr,
                                      const long long* __restrict__ obs_ptr, const int* __restrict__ raw_cam,
@@ -77,70 +78,6 @@ __global__ void visual_gather_kernel(long long Tv, const int* __restrict__ trk_i
     const int c = raw_cam[q];
     l_cam[w] = c; l_row[w] = row_of_cam[c]; l_uv[w] = raw_uv[q];
   }
-}
-
-// The camera-pair words of one batch in the order visual_build_kernel walks them (landmarks ascending, x < y inside a
-// landmark; hi = the larger reduced row; a camera observed twice contributes both orderings).  Thread = landmark of the batch;
-// count == true writes the number of words of the batch to batch_pair[b + 1], otherwise the words go to pairs + batch_pair[b].
-template <bool kCount>
-__global__ void __launch_bounds__(kSlots)
-visual_pairs_kernel(const int* __restrict__ trk_ptr, const int* __restrict__ batch_trk, const int* __restrict__ obs_row,
-                    long long* __restrict__ batch_pair, unsigned* __restrict__ pairs) {
-  __shared__ long long off[kMaxTrkPerBatch + 1];
-  const int b = blockIdx.x, lt = threadIdx.x;
-  const int k0 = batch_trk[b], nt = batch_trk[b + 1] - k0, sbase = trk_ptr[k0];
-  int lo = 0, hi = 0;
-  long long cnt = 0;
-  if (lt < nt) {
-    lo = trk_ptr[k0 + lt] - sbase; hi = trk_ptr[k0 + lt + 1] - sbase;
-    for (int x = lo; x < hi; ++x) {
-      const int rx = obs_row[sbase + x];
-      if (rx < 0) continue;
-      for (int y = x + 1; y < hi; ++y) {
-        const int ry = obs_row[sbase + y];
-        if (ry < 0) continue;
-        cnt += (rx == ry) ? 2 : 1;
-      }
-    }
-    off[lt + 1] = cnt;
-  }
-  if (lt == 0) off[0] = 0;
-  __syncthreads();
-  if (lt == 0) for (int i = 0; i < nt; ++i) off[i + 1] += off[i];
-  __syncthreads();
-  if (kCount) {
-    if (lt == 0) batch_pair[b + 1] = off[nt];
-    return;
-  }
-  if (lt >= nt) return;
-  unsigned* dst = pairs + batch_pair[b] + off[lt];
-  const unsigned tl = (unsigned)lt << 16;
-  for (int x = lo; x < hi; ++x) {
-    const int rx = obs_row[sbase + x];
-    if (rx < 0) continue;
-    for (int y = x + 1; y < hi; ++y) {
-      const int ry = obs_row[sbase + y];
-      if (ry < 0) continue;
-      if (rx > ry) *dst++ = (unsigned)x | ((unsigned)y << 8) | tl;
-      else if (ry > rx) *dst++ = (unsigned)y | ((unsigned)x << 8) | tl;
-      else { *dst++ = (unsigned)x | ((unsigned)y << 8) | tl; *dst++ = (unsigned)y | ((unsigned)x << 8) | tl; }
-    }
-  }
-}
-
-// in-place inclusive scan of batch_pair[1..n] by one block (n_batches is a few ten thousand)
-__global__ void visual_pair_scan_kernel(int n, long long* __restrict__ batch_pair) {
-  __shared__ long long part[1024];
-  const int tid = threadIdx.x, per = (n + 1023) / 1024;
-  const int i0 = 1 + tid * per, i1 = min(n + 1, i0 + per);
-  long long s = 0;
-  for (int i = i0; i < i1; ++i) s += batch_pair[i];
-  part[tid] = s;
-  __syncthreads();
-  if (tid == 0) { long long run = 0; for (int w = 0; w < 1024; ++w) { const long long v = part[w]; part[w] = run; run += v; } batch_pair[0] = 0; }
-  __syncthreads();
-  long long run = part[tid];
-  for (int i = i0; i < i1; ++i) { run += batch_pair[i]; batch_pair[i] = run; }
 }
 
 inline bool plane_valid(const double* p) {   // has_valid_plane, src/lvba_system.cpp:1598
@@ -260,13 +197,20 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   lap("envelope + solver prepare");
   // ---- shard (SURVEY.md §8e): landmark -> owner of its lowest camera index
   Comm& cm = comm();
-  std::vector<int64_t> mine;
-  if (!cm.active()) mine.swap(valid);                          // one rank: every valid landmark
-  else
-    for (int64_t k = 0; k < Tv_all; ++k)
-      if ((P->solver.dist() ? P->solver.dist_owner(min_sys_row[k]) : shard_owner(min_row[k], M, cm.n_ranks)) == cm.rank)
-        mine.push_back(valid[k]);
-  const int64_t Tv = (int64_t)mine.size();
+  std::vector<int64_t> own;                                    // indices into valid
+  for (int64_t k = 0; k < Tv_all; ++k)
+    if (!cm.active() || (P->solver.dist() ? P->solver.dist_owner(min_sys_row[k]) : shard_owner(min_row[k], M, cm.n_ranks)) == cm.rank)
+      own.push_back(k);
+  const int64_t Tv = (int64_t)own.size();
+  // the landmarks in the order of the lowest system row of their clique: the landmarks of a build tile then share cameras,
+  // whose S blocks and rows the tile sums on chip (visual_tiles.h)
+  std::vector<int64_t> mine((size_t)Tv);
+  {
+    std::vector<int> key((size_t)Tv);
+    for (int64_t j = 0; j < Tv; ++j) key[j] = min_sys_row[own[j]];
+    const std::vector<int64_t> order = tiles::order_by_key(std::max(P->n_rows, 1), key.data(), Tv);
+    for (int64_t j = 0; j < Tv; ++j) mine[j] = valid[own[order[j]]];
+  }
   P->Tv = Tv;
   std::vector<int> trk_ptr(Tv + 1, 0), trk_id(Tv);
   for (int64_t k = 0; k < Tv; ++k) {
@@ -276,24 +220,17 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   const long long nnz = trk_ptr[Tv];
   P->nnz = nnz;
   lap("landmark list");
-  // ---- batches
-  std::vector<int> batch_trk{0};
-  {
-    int ns = 0, nt = 0;
-    for (int64_t k = 0; k < Tv; ++k) {
-      const int L = trk_ptr[k + 1] - trk_ptr[k];
-      if (nt > 0 && (ns + L > kSlots || nt + 1 > kMaxTrkPerBatch)) { batch_trk.push_back((int)k); ns = 0; nt = 0; }
-      ns += L; ++nt;
-    }
-    if (Tv > 0) batch_trk.push_back((int)Tv);
-  }
+  // ---- back-substitution / cost batches (<= kSlots observations) and build tiles (<= kVisTileSlots observations)
+  const std::vector<int> batch_trk = tiles::cut_ranges(Tv, trk_ptr.data(), nullptr, kSlots, kMaxTrkPerBatch);
+  const std::vector<int> tile_trk = tiles::cut_ranges(Tv, trk_ptr.data(), nullptr, kVisTileSlots, kMaxTrkPerTile);
   P->n_batches = (int)batch_trk.size() - 1;
-  lap("batches");
+  P->n_tiles = (int)tile_trk.size() - 1;
+  lap("batches + tiles");
 
-  // ---- upload the caller's arrays as they are; gather the per-observation arrays and build the pair table on the device
+  // ---- upload the caller's arrays as they are; gather the per-observation arrays and build the destination table on the device
   LVBA_TRY(P->trk_ptr.upload(trk_ptr, s, &P->h2d));
-  LVBA_TRY(P->batch_pair.alloc((size_t)P->n_batches + 1));
-  LVBA_TRY(P->batch_pair.zero(s));
+  LVBA_TRY(P->batch_trk.upload(batch_trk, s, &P->h2d));
+  LVBA_TRY(P->tile_trk.upload(tile_trk, s, &P->h2d));
   if (Tv > 0) {
     const int64_t nnz_all = obs_ptr[T];
     DevBuf<long long> d_obs_ptr;
@@ -309,26 +246,31 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
     LVBA_TRY(P->trk_id.upload(trk_id, s, &P->h2d));
     LVBA_TRY(P->obs_cam.alloc((size_t)nnz)); LVBA_TRY(P->obs_row.alloc((size_t)nnz)); LVBA_TRY(P->obs_uv.alloc((size_t)nnz));
     LVBA_TRY(P->plane.alloc((size_t)Tv * 4));
-    LVBA_TRY(P->batch_trk.upload(batch_trk, s, &P->h2d));
     visual_gather_kernel<<<(unsigned)((Tv + 127) / 128), 128, 0, s>>>(Tv, P->trk_id.p, P->trk_ptr.p, d_obs_ptr.p, d_raw_cam.p, d_raw_uv.p,
                                                                      d_raw_plane.p, d_row_of_cam.p, P->obs_cam.p, P->obs_row.p, P->obs_uv.p, P->plane.p);
-    visual_pairs_kernel<true><<<P->n_batches, kSlots, 0, s>>>(P->trk_ptr.p, P->batch_trk.p, P->obs_row.p, P->batch_pair.p, nullptr);
-    visual_pair_scan_kernel<<<1, 1024, 0, s>>>(P->n_batches, P->batch_pair.p);
-    long long np = 0;
-    LVBA_CUDA(cudaMemcpyAsync(&np, P->batch_pair.p + P->n_batches, sizeof(long long), cudaMemcpyDeviceToHost, s));
-    LVBA_CUDA(cudaStreamSynchronize(s));          // the temporaries above may now go back to the pool
-    P->n_pairs = np;
-    if (np > 0) {
-      LVBA_TRY(P->pairs.alloc((size_t)np));
-      visual_pairs_kernel<false><<<P->n_batches, kSlots, 0, s>>>(P->trk_ptr.p, P->batch_trk.p, P->obs_row.p, P->batch_pair.p, P->pairs.p);
-    }
     LVBA_CUDA(cudaGetLastError());
-    P->launches += 4;
+    ++P->launches;
+    CudaExec ex;
+    ex.stream = s;
+    DevBuf<long long> d_pair_cnt, d_trk_pair;                  // ordered observation pairs before every local landmark
+    LVBA_TRY(d_pair_cnt.alloc((size_t)Tv + 1));
+    LVBA_TRY(d_trk_pair.alloc((size_t)Tv + 1));
+    LVBA_TRY(ex.for_each(Tv + 1, tiles::VisPairCountF{P->trk_ptr.p, Tv, d_pair_cnt.p}));
+    LVBA_TRY(ex.exclusive_scan(d_pair_cnt.p, d_trk_pair.p, Tv + 1));
+    long long n_ordered = 0;
+    for (int64_t k = 0; k < Tv; ++k) n_ordered += (long long)(trk_ptr[k + 1] - trk_ptr[k]) * (trk_ptr[k + 1] - trk_ptr[k] - 1);
+    const tiles::VisTableIn tin{P->n_tiles, P->n_rows, P->env.nblocks, P->tile_trk.p, P->trk_ptr.p, P->obs_row.p, d_trk_pair.p,
+                                P->env.d_first.p, P->env.d_row_start.p};
+    LVBA_TRY(tiles::sort_runs(ex, n_ordered, P->n_tiles, (uint64_t)P->env.nblocks, tiles::VisPairKeyF{tin}, P->prun));
+    LVBA_TRY(tiles::sort_runs(ex, nnz, P->n_tiles, (uint64_t)P->n_rows, tiles::ObsKeyF{tin}, P->drun));
+    int64_t np = 0;
+    LVBA_TRY(ex.fetch(&np, P->prun.run_ptr.p + P->prun.n_runs, 1));
+    P->n_pairs = np;
+    P->launches += ex.launches;
   } else {
-    LVBA_TRY(P->batch_trk.upload(batch_trk, s, &P->h2d));
     P->n_pairs = 0;
   }
-  lap("device gather + pair table");
+  lap("device gather + destination table");
   if (P->n_rows > 0) LVBA_TRY(P->d_cam_of_row.upload(P->cam_of_row, s, &P->h2d));
   LVBA_TRY(P->q.upload(q, (size_t)M * 4, s, &P->h2d));
   LVBA_TRY(P->t.upload(t, (size_t)M * 3, s, &P->h2d));
@@ -348,7 +290,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   LVBA_TRY(P->cam_colsq.alloc(n6)); LVBA_TRY(P->cam_grad.alloc(n6)); LVBA_TRY(P->s_cam.alloc(n6));
   LVBA_TRY(P->s_pt.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
   LVBA_TRY(P->pt_colsq.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
-  const size_t nb = (size_t)std::max(P->n_batches, 1);
+  const size_t nb = (size_t)std::max(std::max(P->n_batches, P->n_tiles), 1);
   LVBA_TRY(P->batch_cost.alloc(nb)); LVBA_TRY(P->batch_gmax.alloc(nb)); LVBA_TRY(P->batch_out.alloc(nb * 4));
   LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
   LVBA_TRY(P->scal.alloc(16)); LVBA_TRY(P->scal.zero(s));
@@ -367,8 +309,8 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
 inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
   cudaStream_t s = P->stream;
   LVBA_TRY(P->cam_colsq.zero(s));
-  if (P->n_batches > 0) {
-    visual_colnorm_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
+  if (P->n_tiles > 0) {
+    visual_colnorm_kernel<<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
     ++P->launches;
   }
   Comm& cm = comm();
@@ -395,13 +337,13 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
   P->timers.begin(PH_BUILD);
   LVBA_TRY(P->S.zero(s)); LVBA_TRY(P->rhs.zero(s)); LVBA_TRY(P->cam_colsq.zero(s)); LVBA_TRY(P->cam_grad.zero(s));
   LVBA_CUDA(cudaMemsetAsync(P->scal.p + 1, 0, sizeof(double), s));
-  if (P->n_batches > 0) {
-    visual_build_kernel<<<P->n_batches, kSlots, visual_build_smem_bytes(), s>>>(
+  if (P->n_tiles > 0) {
+    visual_build_kernel<<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
         P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
     ++P->launches;
   }
-  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, P->n_batches, P->scal.p + 0);
-  reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, P->n_batches, P->scal.p + 1);
+  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, P->n_tiles, P->scal.p + 0);
+  reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, P->n_tiles, P->scal.p + 1);
   P->launches += 2;
   if (cm.active()) {
     // row-owned reduced camera system (SURVEY.md 8(e)): see lidar_build_dev
