@@ -34,6 +34,7 @@ EXPORTS = [
     "lvba_visual_lm", "lvba_visual_create", "lvba_visual_destroy", "lvba_visual_set_state",
     "lvba_visual_get_state", "lvba_visual_cost", "lvba_visual_step", "lvba_visual_structure",
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
+    "lvba_visual_big_counts",
     "lvba_voxel_default_opts", "lvba_voxel_map_create", "lvba_voxel_map_create_windows", "lvba_voxel_map_windows",
     "lvba_voxel_map_lidar_lm_batch", "lvba_voxel_map_summary", "lvba_voxel_map_export",
     "lvba_voxel_map_lookup", "lvba_voxel_map_lidar_create", "lvba_voxel_map_lidar_lm", "lvba_voxel_map_destroy",
@@ -411,6 +412,12 @@ class VisualProblem:
         a, b, c, d = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int64()
         _chk(self._lib.lvba_visual_counts(self._h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return dict(nnz_valid=a.value, n_valid_tracks=b.value, n_blocks_env=c.value, n_pairs=d.value)
+
+    def big_counts(self):
+        """Landmarks with more than 128 observations, which take their own device passes: dict(n_big, n_big_obs, n_big_pairs)."""
+        a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
+        _chk(self._lib.lvba_visual_big_counts(self._h, C.byref(a), C.byref(b), C.byref(c)))
+        return dict(n_big=a.value, n_big_obs=b.value, n_big_pairs=c.value)
 
 
 # ------------------------------------------------------------------ B3: adaptive voxel map

@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <math.h>
 
+#include "vec3.h"
+
 #define LVBA_DEV __device__ __forceinline__
 
 namespace lvba {
@@ -38,18 +40,7 @@ LVBA_DEV void mat3t_vec(const double* A, const double* x, double* y) {   // y = 
 #pragma unroll
   for (int i = 0; i < 3; ++i) y[i] = A[i] * x[0] + A[3 + i] * x[1] + A[6 + i] * x[2];
 }
-LVBA_DEV void cross3(const double* a, const double* b, double* c) {
-  c[0] = a[1] * b[2] - a[2] * b[1];
-  c[1] = a[2] * b[0] - a[0] * b[2];
-  c[2] = a[0] * b[1] - a[1] * b[0];
-}
-LVBA_DEV double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
-// hat(v): reference include/BALM/tools.hpp:105-112
-LVBA_DEV void hat3(const double* v, double* H) {
-  H[0] = 0.0;   H[1] = -v[2]; H[2] = v[1];
-  H[3] = v[2];  H[4] = 0.0;   H[5] = -v[0];
-  H[6] = -v[1]; H[7] = v[0];  H[8] = 0.0;
-}
+// cross3, dot3, hat3: vec3.h
 // A * hat(w) without forming hat:  (A hat(w))_{:,0} = A_{:,1} w2 - A_{:,2} w1, ...
 LVBA_DEV void mat3_mul_hat(const double* A, const double* w, double* C) {
 #pragma unroll

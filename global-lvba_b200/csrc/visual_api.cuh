@@ -8,6 +8,7 @@
 #include "exec.cuh"
 #include "runtime.cuh"   // (pulls comm.cuh in)
 #include "visual.cuh"
+#include "visual_big.h"
 
 struct lvba_visual_problem {
   int M = 0;
@@ -27,6 +28,11 @@ struct lvba_visual_problem {
   lvba::DevBuf<double> batch_cost, batch_gmax, batch_out, cam_out, scal, cam_step, pt_step;
   lvba::Envelope env;
   lvba::EnvSolver solver;
+  // landmarks with more than kSlots observations: local landmarks [Tv_small, Tv), outside the tiles and batches, through the
+  // passes of visual_big.h
+  long long Tv_small = 0, n_big = 0, n_big_obs = 0, n_big_pairs = 0;
+  lvba::DevBuf<int64_t> big_pair_ptr;
+  lvba::DevBuf<double> big_obs, big_params;
   lvba::PhaseTimers timers;
   double* h_scal = nullptr;
   int64_t launches = 0, h2d = 0, d2h = 0;
@@ -49,6 +55,7 @@ struct lvba_visual_problem {
     v.inv_sigma_pl = 1.0 / std::max(1e-9, sigma_pl);        // utils.hpp:131
     return v;
   }
+  lvba::vbig::View big_view() const { return lvba::vbig::View{(int64_t)n_big, (int64_t)Tv_small, big_pair_ptr.p, env.d_first.p, env.d_row_start.p}; }
   lvba::VisualState state() const { return lvba::VisualState{q.p, t.p, X.p}; }
   lvba::VisualState cand() const { return lvba::VisualState{qc.p, tc.p, Xc.p}; }
   ~lvba_visual_problem() {
@@ -131,22 +138,14 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   std::vector<char> cam_used(M, 0);
   {
     std::vector<char> is_valid((size_t)T, 0), used_w((size_t)kMaxSetupThreads * (size_t)M, 0);
-    int64_t too_long[kMaxSetupThreads];
-    for (int w = 0; w < kMaxSetupThreads; ++w) too_long[w] = -1;
     parallel_chunks(T, 1 << 13, [&](int64_t i0, int64_t i1, int w) {
       char* used = used_w.data() + (size_t)w * (size_t)M;
       for (int64_t i = i0; i < i1; ++i) {
         if (!plane_valid(plane_nd + 4 * i)) continue;
-        if (obs_ptr[i + 1] - obs_ptr[i] > kSlots) { if (too_long[w] < 0) too_long[w] = i; continue; }
         is_valid[(size_t)i] = 1;
         for (int64_t q_ = obs_ptr[i]; q_ < obs_ptr[i + 1]; ++q_) used[obs_cam[q_]] = 1;
       }
     });
-    for (int w = 0; w < kMaxSetupThreads; ++w)
-      if (too_long[w] >= 0) {
-        const int64_t i = too_long[w];
-        return fail(LVBA_ERR_UNSUPPORTED, "landmark %lld has %lld observations; this build handles <= %d", (long long)i, (long long)(obs_ptr[i + 1] - obs_ptr[i]), kSlots);
-      }
     for (int w = 0; w < kMaxSetupThreads; ++w)
       for (int c = 0; c < M; ++c) cam_used[c] |= used_w[(size_t)w * (size_t)M + c];
     for (int64_t i = 0; i < T; ++i) if (is_valid[(size_t)i]) valid.push_back(i);
@@ -203,15 +202,22 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
       own.push_back(k);
   const int64_t Tv = (int64_t)own.size();
   // the landmarks in the order of the lowest system row of their clique: the landmarks of a build tile then share cameras,
-  // whose S blocks and rows the tile sums on chip (visual_tiles.h)
+  // whose S blocks and rows the tile sums on chip (visual_tiles.h).  Landmarks with more than kSlots observations go after all
+  // small ones, in the same order: they take the passes of visual_big.h.
   std::vector<int64_t> mine((size_t)Tv);
+  int64_t Tv_small = 0;
   {
     std::vector<int> key((size_t)Tv);
     for (int64_t j = 0; j < Tv; ++j) key[j] = min_sys_row[own[j]];
     const std::vector<int64_t> order = tiles::order_by_key(std::max(P->n_rows, 1), key.data(), Tv);
-    for (int64_t j = 0; j < Tv; ++j) mine[j] = valid[own[order[j]]];
+    auto is_big = [&](int64_t i) { return obs_ptr[i + 1] - obs_ptr[i] > kSlots; };
+    for (int64_t j = 0; j < Tv; ++j) if (!is_big(valid[own[order[j]]])) mine[Tv_small++] = valid[own[order[j]]];
+    int64_t w = Tv_small;
+    for (int64_t j = 0; j < Tv; ++j) if (is_big(valid[own[order[j]]])) mine[w++] = valid[own[order[j]]];
   }
   P->Tv = Tv;
+  P->Tv_small = Tv_small;
+  P->n_big = Tv - Tv_small;
   std::vector<int> trk_ptr(Tv + 1, 0), trk_id(Tv);
   for (int64_t k = 0; k < Tv; ++k) {
     trk_id[k] = (int)mine[k];
@@ -221,8 +227,8 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   P->nnz = nnz;
   lap("landmark list");
   // ---- back-substitution / cost batches (<= kSlots observations) and build tiles (<= kVisTileSlots observations)
-  const std::vector<int> batch_trk = tiles::cut_ranges(Tv, trk_ptr.data(), nullptr, kSlots, kMaxTrkPerBatch);
-  const std::vector<int> tile_trk = tiles::cut_ranges(Tv, trk_ptr.data(), nullptr, kVisTileSlots, kMaxTrkPerTile);
+  const std::vector<int> batch_trk = tiles::cut_ranges(Tv_small, trk_ptr.data(), nullptr, kSlots, kMaxTrkPerBatch);
+  const std::vector<int> tile_trk = tiles::cut_ranges(Tv_small, trk_ptr.data(), nullptr, kVisTileSlots, kMaxTrkPerTile);
   P->n_batches = (int)batch_trk.size() - 1;
   P->n_tiles = (int)tile_trk.size() - 1;
   lap("batches + tiles");
@@ -250,23 +256,53 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
                                                                      d_raw_plane.p, d_row_of_cam.p, P->obs_cam.p, P->obs_row.p, P->obs_uv.p, P->plane.p);
     LVBA_CUDA(cudaGetLastError());
     ++P->launches;
-    CudaExec ex;
-    ex.stream = s;
-    DevBuf<long long> d_pair_cnt, d_trk_pair;                  // ordered observation pairs before every local landmark
-    LVBA_TRY(d_pair_cnt.alloc((size_t)Tv + 1));
-    LVBA_TRY(d_trk_pair.alloc((size_t)Tv + 1));
-    LVBA_TRY(ex.for_each(Tv + 1, tiles::VisPairCountF{P->trk_ptr.p, Tv, d_pair_cnt.p}));
-    LVBA_TRY(ex.exclusive_scan(d_pair_cnt.p, d_trk_pair.p, Tv + 1));
-    long long n_ordered = 0;
-    for (int64_t k = 0; k < Tv; ++k) n_ordered += (long long)(trk_ptr[k + 1] - trk_ptr[k]) * (trk_ptr[k + 1] - trk_ptr[k] - 1);
-    const tiles::VisTableIn tin{P->n_tiles, P->n_rows, P->env.nblocks, P->tile_trk.p, P->trk_ptr.p, P->obs_row.p, d_trk_pair.p,
-                                P->env.d_first.p, P->env.d_row_start.p};
-    LVBA_TRY(tiles::sort_runs(ex, n_ordered, P->n_tiles, (uint64_t)P->env.nblocks, tiles::VisPairKeyF{tin}, P->prun));
-    LVBA_TRY(tiles::sort_runs(ex, nnz, P->n_tiles, (uint64_t)P->n_rows, tiles::ObsKeyF{tin}, P->drun));
-    int64_t np = 0;
-    LVBA_TRY(ex.fetch(&np, P->prun.run_ptr.p + P->prun.n_runs, 1));
-    P->n_pairs = np;
-    P->launches += ex.launches;
+    if (Tv_small > 0) {                                        // the destination table covers the small landmarks only
+      CudaExec ex;
+      ex.stream = s;
+      DevBuf<long long> d_pair_cnt, d_trk_pair;                // ordered observation pairs before every local landmark
+      LVBA_TRY(d_pair_cnt.alloc((size_t)Tv_small + 1));
+      LVBA_TRY(d_trk_pair.alloc((size_t)Tv_small + 1));
+      LVBA_TRY(ex.for_each(Tv_small + 1, tiles::VisPairCountF{P->trk_ptr.p, Tv_small, d_pair_cnt.p}));
+      LVBA_TRY(ex.exclusive_scan(d_pair_cnt.p, d_trk_pair.p, Tv_small + 1));
+      long long n_ordered = 0;
+      for (int64_t k = 0; k < Tv_small; ++k) n_ordered += (long long)(trk_ptr[k + 1] - trk_ptr[k]) * (trk_ptr[k + 1] - trk_ptr[k] - 1);
+      const tiles::VisTableIn tin{P->n_tiles, P->n_rows, P->env.nblocks, P->tile_trk.p, P->trk_ptr.p, P->obs_row.p, d_trk_pair.p,
+                                  P->env.d_first.p, P->env.d_row_start.p};
+      LVBA_TRY(tiles::sort_runs(ex, n_ordered, P->n_tiles, (uint64_t)P->env.nblocks, tiles::VisPairKeyF{tin}, P->prun));
+      LVBA_TRY(tiles::sort_runs(ex, (int64_t)trk_ptr[Tv_small], P->n_tiles, (uint64_t)P->n_rows, tiles::ObsKeyF{tin}, P->drun));
+      int64_t np = 0;
+      LVBA_TRY(ex.fetch(&np, P->prun.run_ptr.p + P->prun.n_runs, 1));
+      P->n_pairs = np;
+      P->launches += ex.launches;
+    }
+    if (P->n_big > 0) {
+      // pair items of the big landmarks (K (K - 1) each) and their camera-pair contributions: an unordered pair of observations
+      // of two distinct rows once, of one row in both orders, i.e. C(n, 2) + sum_row C(n_row, 2) over the n observations of
+      // non-constant cameras
+      std::vector<int64_t> bpp((size_t)P->n_big + 1, 0);
+      std::vector<int> rows;
+      for (int64_t b = 0; b < P->n_big; ++b) {
+        const int64_t i = mine[Tv_small + b], K = obs_ptr[i + 1] - obs_ptr[i];
+        bpp[b + 1] = bpp[b] + K * (K - 1);
+        rows.clear();
+        for (int64_t q_ = obs_ptr[i]; q_ < obs_ptr[i + 1]; ++q_) if (row_of_cam[obs_cam[q_]] >= 0) rows.push_back(row_of_cam[obs_cam[q_]]);
+        std::sort(rows.begin(), rows.end());
+        const long long n = (long long)rows.size();
+        long long contrib = n * (n - 1) / 2;
+        for (size_t a = 0; a < rows.size();) {
+          size_t e = a;
+          while (e < rows.size() && rows[e] == rows[a]) ++e;
+          contrib += (long long)(e - a) * (long long)(e - a - 1) / 2;
+          a = e;
+        }
+        P->n_pairs += contrib;
+      }
+      P->n_big_obs = nnz - trk_ptr[Tv_small];
+      P->n_big_pairs = bpp.back();
+      LVBA_TRY(P->big_pair_ptr.upload(bpp, s, &P->h2d));
+      LVBA_TRY(P->big_obs.alloc((size_t)P->n_big_obs * vbig::kObs));
+      LVBA_TRY(P->big_params.alloc((size_t)P->n_big * kTrkParams));
+    }
   } else {
     P->n_pairs = 0;
   }
@@ -290,7 +326,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   LVBA_TRY(P->cam_colsq.alloc(n6)); LVBA_TRY(P->cam_grad.alloc(n6)); LVBA_TRY(P->s_cam.alloc(n6));
   LVBA_TRY(P->s_pt.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
   LVBA_TRY(P->pt_colsq.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
-  const size_t nb = (size_t)std::max(std::max(P->n_batches, P->n_tiles), 1);
+  const size_t nb = (size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1);   // partial slots, big landmarks last
   LVBA_TRY(P->batch_cost.alloc(nb)); LVBA_TRY(P->batch_gmax.alloc(nb)); LVBA_TRY(P->batch_out.alloc(nb * 4));
   LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
   LVBA_TRY(P->scal.alloc(16)); LVBA_TRY(P->scal.zero(s));
@@ -305,6 +341,15 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   return LVBA_OK;
 }
 
+// one pass of visual_big.h over `items` items (grid-stride, 128 threads per CTA)
+template <class F>
+inline void visual_big_launch(lvba_visual_problem* P, int64_t items, const F& f) {
+  if (items <= 0) return;
+  const int grid = (int)std::min<int64_t>((items + 127) / 128, kNumSMs * 16);
+  env_wide_pass_kernel<<<grid, 128, 0, P->stream>>>(items, f);
+  ++P->launches;
+}
+
 // Jacobi scaling vectors from the Jacobian at the current state (Ceres: once, at iteration 0)
 inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
   cudaStream_t s = P->stream;
@@ -312,6 +357,10 @@ inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
   if (P->n_tiles > 0) {
     visual_colnorm_kernel<<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
     ++P->launches;
+  }
+  if (P->n_big > 0) {
+    visual_big_launch(P, P->n_big_obs, vbig::ColObsF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p});
+    visual_big_launch(P, P->n_big, vbig::ColTrackF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->pt_colsq.p});
   }
   Comm& cm = comm();
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->cam_colsq.p, (size_t)P->n_rows * 6, s));
@@ -342,8 +391,17 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
         P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
     ++P->launches;
   }
-  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, P->n_tiles, P->scal.p + 0);
-  reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, P->n_tiles, P->scal.p + 1);
+  if (P->n_big > 0) {        // cost and gradient max of landmark b in the partial slots n_tiles + b
+    const VisualView vv = P->view();
+    const vbig::View bv = P->big_view();
+    visual_big_launch(P, P->n_big_obs, vbig::ObsF{vv, bv, P->state(), lm, P->big_obs.p});
+    visual_big_launch(P, P->n_big, vbig::TrackF{vv, bv, P->state(), lm, P->big_obs.p, P->big_params.p, P->batch_cost.p + P->n_tiles,
+                                                P->batch_gmax.p + P->n_tiles});
+    visual_big_launch(P, P->n_big_obs, vbig::SlotsF{vv, bv, P->big_params.p, P->big_obs.p, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p});
+    visual_big_launch(P, P->n_big_pairs, vbig::PairsF{vv, bv, P->big_obs.p, P->S.p});
+  }
+  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_tiles + P->n_big), P->scal.p + 0);
+  reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, (int)(P->n_tiles + P->n_big), P->scal.p + 1);
   P->launches += 2;
   if (cm.active()) {
     // row-owned reduced camera system (SURVEY.md 8(e)): see lidar_build_dev
@@ -371,7 +429,10 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
         P->view(), P->state(), lm, P->y.p, P->Xc.p, want_steps ? P->pt_step.p : nullptr, P->batch_out.p);
     ++P->launches;
   }
-  reduce_cols_kernel<<<1, 256, 0, s>>>(P->batch_out.p, P->n_batches, 4, 3, P->scal.p + 2);
+  if (P->n_big > 0)
+    visual_big_launch(P, P->n_big, vbig::BacksubF{P->view(), P->big_view(), P->state(), lm, P->big_obs.p, P->big_params.p, P->y.p, P->Xc.p,
+                                                  want_steps ? P->pt_step.p : nullptr, P->batch_out.p + 4 * (int64_t)P->n_batches});
+  reduce_cols_kernel<<<1, 256, 0, s>>>(P->batch_out.p, (int)(P->n_batches + P->n_big), 4, 3, P->scal.p + 2);
   ++P->launches;
   const int ncb = (P->n_rows + 127) / 128;
   if (ncb > 0) {
@@ -387,7 +448,8 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
     visual_cost_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->cand(), P->batch_cost.p);
     ++P->launches;
   }
-  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, P->n_batches, P->scal.p + 8);
+  if (P->n_big > 0) visual_big_launch(P, P->n_big, vbig::CostF{P->view(), P->big_view(), P->cand(), P->batch_cost.p + P->n_batches});
+  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_batches + P->n_big), P->scal.p + 8);
   ++P->launches;
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 8, 1, s));
   P->timers.end();
@@ -529,7 +591,8 @@ int lvba_visual_cost(lvba_visual_problem* p, double* cost) LVBA_ABI_BEGIN {
   LVBA_CUDA(cudaSetDevice(p->device));
   cudaStream_t s = p->stream;
   if (p->n_batches > 0) { lvba::visual_cost_kernel<<<p->n_batches, lvba::kSlots, 0, s>>>(p->view(), p->state(), p->batch_cost.p); ++p->launches; }
-  lvba::reduce_partials_kernel<<<1, 256, 0, s>>>(p->batch_cost.p, p->n_batches, p->scal.p + 8);
+  if (p->n_big > 0) lvba::visual_big_launch(p, p->n_big, lvba::vbig::CostF{p->view(), p->big_view(), p->state(), p->batch_cost.p + p->n_batches});
+  lvba::reduce_partials_kernel<<<1, 256, 0, s>>>(p->batch_cost.p, (int)(p->n_batches + p->n_big), p->scal.p + 8);
   ++p->launches;
   if (lvba::comm().active()) LVBA_TRY(lvba::comm().allreduce_sum(p->scal.p + 8, 1, s));
   LVBA_CUDA(cudaMemcpyAsync(p->h_scal, p->scal.p + 8, sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -610,6 +673,14 @@ int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_va
   if (n_pairs) *n_pairs = p->n_pairs;
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_counts")
+
+int lvba_visual_big_counts(lvba_visual_problem* p, int64_t* n_big, int64_t* n_big_obs, int64_t* n_big_pairs) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  if (n_big) *n_big = p->n_big;
+  if (n_big_obs) *n_big_obs = p->n_big_obs;
+  if (n_big_pairs) *n_big_pairs = p->n_big_pairs;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_big_counts")
 
 int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const double* plane_nd, const int64_t* obs_ptr,
                    const int32_t* obs_cam, const float* obs_uv, const double intr[8], double sigma_px, double sigma_plane,

@@ -179,7 +179,8 @@ int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env
  *   t           [M*3] in/out   ts[k]
  *   X           [T*3] in/out   Xs[pi]  (:1521-1525); landmarks without a valid plane are left untouched
  *   plane_nd    [T*4] (n, d); n == 0 marks "no valid plane" => landmark and its observations are skipped (:1598-1603)
- *   obs_ptr     [T+1] CSR; obs_cam [nnz] camera of each inlier observation; obs_uv [nnz*2] float pixel (:1624-1625)
+ *   obs_ptr     [T+1] CSR; obs_cam [nnz] camera of each inlier observation; obs_uv [nnz*2] float pixel (:1624-1625).
+ *               A landmark may have any number of observations, and may see one camera more than once.
  *   fixed_cam   camera held constant (0 in the reference, :1582-1583); -1 = none
  * ====================================================================================== */
 int lvba_visual_lm(int32_t M, int64_t T, double* q_wxyz, double* t, double* X,
@@ -213,6 +214,9 @@ int lvba_visual_reset_state(lvba_visual_problem* p);
 int lvba_visual_iterate(lvba_visual_problem* p, int32_t n_iter, lvba_summary* summary);
 int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_valid_tracks,
                        int64_t* n_blocks_env, int64_t* n_pairs);
+/* Landmarks with more than 128 observations (this rank's, with a valid plane) do not fit the build tiles and take their own
+ * device passes: their number, their observations and their ordered observation pairs (sum of K (K - 1)). */
+int lvba_visual_big_counts(lvba_visual_problem* p, int64_t* n_big, int64_t* n_big_obs, int64_t* n_big_pairs);
 
 /* ======================================================================================
  * B3  adaptive voxel map (set-up stage) — replaces the cut_voxel / recut / tras_opt sequence in front of every
