@@ -27,7 +27,7 @@ struct FactorJob {
   double* zdump;   // [bs*6]
   int* status;     // set to 1 when a pivot block is singular / non-finite
   // Optional progress counter for a consumer that runs BESIDE this factorisation (the spike kernel, nd_kernels.cuh): the number of
-  // leading columns of L that are final in global memory, published with release semantics every few pivots and once more — as
+  // leading columns of L that are final in global memory, published with release semantics every few pivots (values below n_stop) and once more — as
   // the very last global write of the CTA — with the value n_stop.  nullptr: nothing is published.
   int* progress = nullptr;
 };

@@ -598,7 +598,8 @@ env_factor_la_kernel(const FactorJob* __restrict__ jobs, const unsigned* __restr
         __syncwarp();
         if (lane < 6) sZ[c * 6 + lane] = (k + P < n) ? sZin[((k + P) & 7) * 6 + lane] : 0.0;   // row k+P takes slot c
         // columns 0..k of L were complete in global memory before the block barrier this warp passed at the top of the step
-        if (J.progress && lane == 0 && (k & 3) == 3) progress_publish(J.progress, k + 1);
+        // (never the final value n_stop: that one comes after the last barrier, when the dumps and the status are out too)
+        if (J.progress && lane == 0 && (k & 3) == 3 && k + 1 < n_stop) progress_publish(J.progress, k + 1);
       } else {
         // ---- column items: T_{i,k+1} = A_{i,k+1} - L_{i,k} T_{k+1,k}^T for rows i = k+2 .. k+P, then L = T D_{k+1}^-1
         stream_row(k + 1);                                          // row k+1+P -> sEnter[nxt]

@@ -42,10 +42,12 @@ constexpr int kSpikeZStride = 26;                // doubles per block row of a w
 constexpr int kSpikeBS = 38;                     // doubles per staged block of L
 constexpr int kSpikeBufs = 3;                    // rows of L in flight (cp.async, two rows ahead)
 constexpr size_t kSpikeSmem = sizeof(double) * (kSpikeBufs * 32 * kSpikeBS + kSpikeWarps * 33 * kSpikeZStride);
+constexpr int kSpikePublish = 4;                 // rows of Z between two publications of SpikeJob::zprog
 static_assert(kSpikeC == 4, "the reduce-scatter below is written for 24 values per lane");
 
 __global__ void __launch_bounds__(kSpikeThreads)
 nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
+  pdl_launch_dependents();                                     // the SYRK that follows this spike's rows (nd_syrk_kernel)
   extern __shared__ __align__(16) double smem_spike[];
   double* sRow = smem_spike;                                   // [kSpikeBufs][32][kSpikeBS] blocks of rows k, k+1, k+2
   const nd::SpikeJob J = jobs[blockIdx.y];
@@ -162,6 +164,9 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
     }
     // lane l now holds the outputs 12 (l >> 4 & 1) + 6 (l >> 3 & 1) + 3 (l >> 2 & 1) + {0,1,2} = 3 (l >> 2) + {0,1,2}
     __syncwarp();                                              // every lane has read the window entries it needs of row k-32
+    // rows 0..k-1 of Z (stored by all four warps before this row's block barrier) -> the SYRK, once per chunk of its rows: here,
+    // where the publishing lane's own stores of row k-1 have long landed, the release costs the row chain little
+    if (J.zprog && tid == 32 && k > 0 && k % kSpikePublish == 0) progress_publish(J.zprog + blockIdx.x, k);
     if (owner) {
 #pragma unroll
       for (int q = 0; q < 3; ++q) {
@@ -173,55 +178,93 @@ nd_spike_kernel(const nd::SpikeJob* __restrict__ jobs) {
     __syncwarp();
     f0 = f1; f1 = f2; f2 = f3; rs2 = rs3; f3 = f4; rs3 = rs4;
   }
+  if (J.zprog) {
+    // the final value waits for the factorisation's last write as well: once every counter of a node reads e.n, spike and
+    // factorisation are both done with it (the SYRK's last CTAs wait for exactly that)
+    wait_row(n);
+    __syncthreads();
+    if (tid == 0) progress_publish(J.zprog + blockIdx.x, n);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // SYRK: U -= sum_k Z_k^T K_k Z_k, u -= sum_k Z_k^T K_k w_k over the pivot rows of a node (SyrkSeg, nd_passes.h): the
 // product (KS x R)(R x KS), R = 6 rows, of Z^T with Y = K Z.  grid = (tiles of 64 x 64 scalars of the lower triangle,
-// groups of kSyrkSplit block rows, segments); a CTA walks its rows in chunks of 4 block rows: Z for the tile's row and
-// column side is brought to shared memory by cp.async one chunk ahead, Y = K Z is formed there, each thread accumulates a
+// groups of kSyrkSplit block rows, segments); a CTA walks its rows in chunks of 4 block rows: Z for the tile's row side is
+// brought to shared memory by cp.async one chunk ahead, for the column side (one buffer: 55 kB of shared memory in all, so that
+// a SYRK CTA fits on an SM beside three spike CTAs) as soon as Y = K Z of the previous chunk is formed; each thread accumulates a
 // 8 x 8 register tile (64 threads per 64 x 64 tile: 16 operand doubles from shared memory per 64 FMAs — a 4 x 4 tile loads 8 per 16
 // and is bound by the 128 B/clk shared-memory return path, at half the FP64 rate).  A thread's rows / columns are four PAIRS 16 apart
 // (2 t + 16 m + {0,1}), so that the LDS.128 of a warp cover 128 contiguous bytes.  Partial sums of the row groups meet in U by
-// RED.ADD.F64.
+// RED.ADD.F64.  grid = (tiles, segments, groups of kSyrkSplit block rows): the first rows of every segment are placed first.
+//
+// Beside the spike (SyrkSeg::zprog): a chunk of rows [kc, kc + 4) needs rows < kc + 4 of Z from the spike CTAs that own the
+// tile's two column ranges, and of K and w from the factorisation; nine threads poll those counters before the chunk is staged
+// (cp.async.cg reads L2, never a stale L1 line), the block barrier hands the acquired view to the others.  Nothing starves:
+// the factorisation, the spike and the SYRK are launched in this order on one stream, the spike and the SYRK with
+// programmatic stream serialisation, and both the factorisation and the spike execute griddepcontrol.launch_dependents first
+// thing — so no CTA of the spike is placed before every CTA of the factorisation runs, and no CTA of the SYRK before every CTA
+// of the spike runs.  A consumer only ever waits for producers that are already running and wait for nobody downstream.  This
+// holds for eager launches (the multi-GPU solve) and for the programmatic edges a stream capture turns them into.
 constexpr int kSyrkTile = 64;            // scalar columns per tile side
 constexpr int kSyrkThreads = 64;         // 8 x 8 threads, 8 x 8 outputs each
 constexpr int kSyrkChunk = 4;            // block rows per shared-memory chunk (24 scalar rows)
-constexpr int kSyrkSplit = 8;            // block rows per CTA: two chunks, both in flight from the start
+constexpr int kSyrkSplit = 8;            // block rows per CTA: two chunks
 constexpr int kSyrkLd = kSyrkTile + 4;   // leading dimension of the shared tiles
 constexpr int kSyrkTileDoubles = kSyrkChunk * 6 * kSyrkLd;
-constexpr size_t kSyrkSmem = sizeof(double) * (5 * kSyrkTileDoubles + 2 * kSyrkChunk * 36 + 2 * kSyrkChunk * 6 + kSyrkChunk * 6);
+constexpr size_t kSyrkSmem = sizeof(double) * (4 * kSyrkTileDoubles + 2 * kSyrkChunk * 36 + 2 * kSyrkChunk * 6 + kSyrkChunk * 6);
+constexpr int kSyrkTileGroups = kSyrkTile / kSpikeCols;      // spike CTAs per tile side
+static_assert(kSyrkTile % kSpikeCols == 0 && kSyrkChunk % kSpikePublish == 0 && kSyrkSplit % kSyrkChunk == 0,
+              "a chunk of the SYRK must end where the spike publishes");
+static_assert(2 * kSyrkTileGroups + 1 <= kSyrkThreads, "one polling thread per counter");
 
 __global__ void __launch_bounds__(kSyrkThreads)
 nd_syrk_kernel(const nd::SyrkSeg* __restrict__ segs, int split) {
   constexpr int TS = kSyrkTile, RC = kSyrkChunk * 6, LD = kSyrkLd;
   extern __shared__ __align__(16) double smem_syrk[];
   double* sA = smem_syrk;                             // [2][RC][LD] Z[r][tile row side]
-  double* sB = sA + 2 * kSyrkTileDoubles;             // [2][RC][LD] Z[r][tile column side]
-  double* sY = sB + 2 * kSyrkTileDoubles;             // [RC][LD]    (K Z)[r][tile column side]
+  double* sB = sA + 2 * kSyrkTileDoubles;             // [RC][LD]    Z[r][tile column side]
+  double* sY = sB + kSyrkTileDoubles;                 // [RC][LD]    (K Z)[r][tile column side]
   double* sK = sY + kSyrkTileDoubles;                 // [2][chunk][36]
   double* sW = sK + 2 * kSyrkChunk * 36;              // [2][RC] w
   double* sKw = sW + 2 * RC;                          // [RC]
-  const nd::SyrkSeg G = segs[blockIdx.z];
+  const nd::SyrkSeg G = segs[blockIdx.y];
   int ti = 0, tj = 0;                                 // tile (ti, tj), tj <= ti, from the linear index
   { int t = blockIdx.x; while ((ti + 1) * (ti + 2) / 2 <= t) ++ti; tj = t - ti * (ti + 1) / 2; }
   if (ti * TS >= G.KS) return;
-  const int k0 = blockIdx.y * split;
+  const int k0 = blockIdx.z * split;
   if (k0 >= G.rows) return;
   const int k1 = min(G.rows, k0 + split);
   const int tid = threadIdx.x, tx = tid & 7, ty = tid >> 3;
   const int KS = G.KS;
+  // threads 0 .. 2 kSyrkTileGroups - 1: the spike counters of the row and the column tile; the next one: the factorisation's
+  const int* poll = nullptr;
+  if (G.zprog) {
+    if (tid < 2 * kSyrkTileGroups) {
+      const int g = (tid < kSyrkTileGroups ? ti : tj) * kSyrkTileGroups + tid % kSyrkTileGroups;
+      if (g * kSpikeCols < KS) poll = G.zprog + g;
+    } else if (tid == 2 * kSyrkTileGroups) {
+      poll = G.fprog;
+    }
+  }
+  // rows < r of Z, K and w final: Z once the spike counters read r, K and w once the factorisation's reads r + 1 (its counter
+  // covers D^-1 and z one row behind L) or its final value.  The caller's block barrier follows.
+  auto need = [&](int r) { return poll == G.fprog ? min(r + 1, G.rows) : r; };
+  auto wait_rows = [&](int r) {
+    if (poll) { const int v = need(r); while (progress_read(poll) < v) __nanosleep(64); }
+  };
+  auto rows_ready = [&](int r) { return !poll || progress_read(poll) >= need(r); };
+  auto wait_spike_done = [&]() {                      // spike (and with it the factorisation) finished with this node
+    if (poll && tid < 2 * kSyrkTileGroups) while (progress_read(poll) < G.zdone) __nanosleep(64);
+  };
   // chunk kc -> buffer par: 16-byte pieces (KS is even, the tiles start at even columns); rows / columns beyond the data are zero-filled
-  auto prefetch = [&](int kc, int par) {
+  auto prefetch = [&](int kc, int par) {              // row side, K, w
     const int nr = min(kSyrkChunk, k1 - kc) * 6;
     double* dA = sA + par * kSyrkTileDoubles;
-    double* dB = sB + par * kSyrkTileDoubles;
     for (int o = tid; o < RC * (TS / 2); o += kSyrkThreads) {
       const int r = o / (TS / 2), a2 = (o - r * (TS / 2)) * 2;
-      const double* zr = G.Z + ((long long)kc * 6 + (r < nr ? r : 0)) * KS;
-      const bool va = r < nr && ti * TS + a2 < KS, vb = r < nr && tj * TS + a2 < KS;
-      cp_async16_zfill(dA + r * LD + a2, va ? zr + ti * TS + a2 : G.Z, va);
-      cp_async16_zfill(dB + r * LD + a2, vb ? zr + tj * TS + a2 : G.Z, vb);
+      const bool va = r < nr && ti * TS + a2 < KS;
+      cp_async16_zfill(dA + r * LD + a2, va ? G.Z + ((long long)kc * 6 + r) * KS + ti * TS + a2 : G.Z, va);
     }
     for (int o = tid; o < kSyrkChunk * 18; o += kSyrkThreads) {
       const int bk = o / 18;
@@ -234,24 +277,40 @@ nd_syrk_kernel(const nd::SyrkSeg* __restrict__ segs, int split) {
       cp_async16_zfill(sW + par * RC + 2 * o, v ? G.w + (long long)kc * 6 + 2 * o : G.w, v);
     }
   };
+  auto prefetch_col = [&](int kc) {                   // column side
+    const int nr = min(kSyrkChunk, k1 - kc) * 6;
+    for (int o = tid; o < RC * (TS / 2); o += kSyrkThreads) {
+      const int r = o / (TS / 2), a2 = (o - r * (TS / 2)) * 2;
+      const bool vb = r < nr && tj * TS + a2 < KS;
+      cp_async16_zfill(sB + r * LD + a2, vb ? G.Z + ((long long)kc * 6 + r) * KS + tj * TS + a2 : G.Z, vb);
+    }
+  };
   double acc[8][8];
 #pragma unroll
   for (int i = 0; i < 8; ++i)
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[i][j] = 0.0;
   double racc = 0.0;
+  wait_rows(min(k0 + kSyrkChunk, k1));
+  __syncthreads();
   prefetch(k0, 0);
+  prefetch_col(k0);
   asm volatile("cp.async.commit_group;" ::: "memory");
   int par = 0;
   for (int kc = k0; kc < k1; kc += kSyrkChunk, par ^= 1) {
-    if (kc + kSyrkChunk < k1) prefetch(kc + kSyrkChunk, par ^ 1);        // its buffer was consumed before the last barrier of the previous chunk
+    const int nr = min(kSyrkChunk, k1 - kc) * 6, next_r = min(kc + 2 * kSyrkChunk, k1);
+    const bool more = kc + kSyrkChunk < k1;                              // (uniform over the CTA)
+    // the next chunk comes in while this one is computed if its rows are final already; otherwise this chunk is computed
+    // first and the next one waited for afterwards (chasing the spike, the chunk at hand is not held up by the next)
+    const bool early = more && __syncthreads_and(rows_ready(next_r));
+    if (early) prefetch(kc + kSyrkChunk, par ^ 1);                       // its buffer was consumed before the last barrier of the previous chunk
     asm volatile("cp.async.commit_group;" ::: "memory");
-    asm volatile("cp.async.wait_group 1;" ::: "memory");
+    asm volatile("cp.async.wait_group 1;" ::: "memory");               // everything but the row side of chunk kc+1
     __syncthreads();                                                     // chunk kc landed
     const double* cA = sA + par * kSyrkTileDoubles;
-    const double* cB = sB + par * kSyrkTileDoubles;
+    const double* cB = sB;
     const double* cK = sK + par * kSyrkChunk * 36;
-    for (int o = tid; o < RC * TS; o += kSyrkThreads) {                  // Y = K Z on the column side
+    for (int o = tid; o < nr * TS; o += kSyrkThreads) {                  // Y = K Z on the column side (rows beyond nr: zero)
       const int r = o / TS, b = o - r * TS, bk = r / 6, x = r - bk * 6;
       const double* Kx = cK + bk * 36 + x * 6;
       double s = 0.0;
@@ -259,16 +318,18 @@ nd_syrk_kernel(const nd::SyrkSeg* __restrict__ segs, int split) {
       for (int q = 0; q < 6; ++q) s += Kx[q] * cB[(bk * 6 + q) * LD + b];
       sY[r * LD + b] = s;
     }
-    if (tj == 0 && tid < RC) {                                           // (K w)[r]
+    if (tj == 0 && tid < nr) {                                           // (K w)[r]
       const int bk = tid / 6, x = tid - bk * 6;
       double s = 0.0;
 #pragma unroll
       for (int q = 0; q < 6; ++q) s += cK[bk * 36 + x * 6 + q] * sW[par * RC + bk * 6 + q];
       sKw[tid] = s;
     }
-    __syncthreads();
+    __syncthreads();                                                     // sB consumed: the column side of the next chunk may come in
+    if (early) prefetch_col(kc + kSyrkChunk);
+    asm volatile("cp.async.commit_group;" ::: "memory");
 #pragma unroll 2
-    for (int r = 0; r < RC; ++r) {
+    for (int r = 0; r < nr; ++r) {
       double av[8], bv[8];
 #pragma unroll
       for (int m = 0; m < 4; ++m) {
@@ -283,11 +344,18 @@ nd_syrk_kernel(const nd::SyrkSeg* __restrict__ segs, int split) {
     }
     if (tj == 0 && tid < TS) {
       double s = 0.0;
-      for (int r = 0; r < RC; ++r) s += cA[r * LD + tid] * sKw[r];
+      for (int r = 0; r < nr; ++r) s += cA[r * LD + tid] * sKw[r];
       racc += s;
     }
+    if (more && !early) wait_rows(next_r);
     __syncthreads();                                                     // sY, sKw and this chunk's buffers are free again
+    if (more && !early) {
+      prefetch(kc + kSyrkChunk, par ^ 1);
+      prefetch_col(kc + kSyrkChunk);
+      asm volatile("cp.async.commit_group;" ::: "memory");
+    }
   }
+  if (k1 == G.rows) wait_spike_done();               // the last rows: this grid ends after the spike and the factorisation
 #pragma unroll
   for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -436,11 +504,17 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
       }
       __syncthreads();                                             // (s) L_s, T_s published; column s+2 handed over by the pair threads
       // the two idle warps of this group: D_s^-1 to global memory (the inverting warp left it in sK[par]; it writes that buffer again
-      // two pivots from now), and word to a spike kernel running beside this CTA that columns 0..s of L are in global memory
+      // two pivots from now) with the final z_s (no pivot after s-1 touches row s), and word to the spike and the SYRK running beside
+      // this CTA that columns 0..s of L — and with them D^-1 and z of rows 0..s-1, stored one barrier ago — are in global memory
+      // (the warp that publishes has no stores of its own in flight: the release does not wait for them)
       if (idle) {
-        if (ct - kDenseColThreads < 18)
-          reinterpret_cast<double2*>(J.dinv + (long long)s * 36)[ct - kDenseColThreads] = reinterpret_cast<const double2*>(sK + par * 36)[ct - kDenseColThreads];
-        if (J.progress && ct == kDenseColThreads + 32 && (s & 3) == 3) progress_publish(J.progress, s + 1);
+        const int l = ct - kDenseColThreads;
+        if (l < 18)
+          reinterpret_cast<double2*>(J.dinv + (long long)s * 36)[l] = reinterpret_cast<const double2*>(sK + par * 36)[l];
+        else if (l < 24)
+          J.z[s * 6 + l - 18] = sZ[s * 6 + l - 18];
+        // (never the final value n: that one comes after the last barrier, when D^-1 and z of the last row are out too)
+        if (J.progress && l == 32 && (s & 3) == 3 && s + 1 < n) progress_publish(J.progress, s + 1);
       }
     }
   } else if (tid >= kDenseInvWarp) {
@@ -508,12 +582,8 @@ nd_dense_factor_kernel(const FactorJob* __restrict__ jobs, const unsigned short*
       __syncthreads();                                             // (s)
     }
   }
-  __syncthreads();
-  for (int o = tid; o < n * 6; o += kDenseThreads) J.z[o] = sZ[o];
-  if (J.progress) {                                                // the last global write of the CTA
-    __syncthreads();
-    if (tid == 0) progress_publish(J.progress, n);
-  }
+  __syncthreads();                                                 // (z went out row by row, with D^-1)
+  if (J.progress && tid == 0) progress_publish(J.progress, n);     // the last global write of the CTA
 }
 
 // thread -> block map of nd_dense_factor_kernel: blocks of the 30 x 30 lower triangle grouped by 8 x 4 patches

@@ -47,6 +47,10 @@ struct SpikeJob {
   double* Z;
   int KS;
   const int* progress = nullptr;   // FactorJob::progress of the factorisation that produces L, when the two run side by side
+  // per group of right-hand sides (one spike CTA): the number of leading block rows of Z that are final in global memory,
+  // published with release semantics every few rows and, once the factorisation has finished too, with the value e.n; for
+  // the SYRK that runs beside the spike.  nullptr: nothing is published.
+  int* zprog = nullptr;
 };
 // U -= sum_k Z_k^T K_k Z_k  and  u -= sum_k Z_k^T K_k w_k  over the pivot rows of one node (K_k = D_k^-1).
 // U: dense lower block triangle over KS/6 block rows, block (i,j), j <= i, at (i(i+1)/2 + j)*36 (leading part of the node's U).
@@ -58,6 +62,13 @@ struct SyrkSeg {
   int KS;
   double* U;
   double* u;
+  // running beside the spike that produces Z and the factorisation that produces K and w: the SYRK stages rows below r once
+  // the zprog counters (SpikeJob::zprog) of its two column tiles have reached r and fprog (FactorJob::progress, which covers
+  // D^-1 and z one row behind L) r + 1 or its final value; the CTAs of the last rows also wait for zdone (the spike's final
+  // value), so that the SYRK finishes after both.  nullptr: no waiting.
+  const int* fprog = nullptr;
+  const int* zprog = nullptr;
+  int zdone = 0;
 };
 
 // everything the passes touch
@@ -76,7 +87,9 @@ struct Tables {
   double* U; double* u; double* Z; double* E; double* T; double* W; double* w;     // pools (offsets in NodeDev); u == U (one pool)
   // multi-GPU only: writable views of H / dadd (the rows of the other ranks' rank separators arrive through the exchange region)
   double* Hw; double* daddw;
-  int* prog = nullptr;            // [nodes] progress counters (FactorJob::progress), or null: factorisation and spike run one after the other
+  int* prog = nullptr;            // [nodes] progress counters (FactorJob::progress), then [nodes][zstride] those of the spike CTAs
+                                  // (SpikeJob::zprog), or null: factorisation, spike and SYRK run one after the other
+  int zstride = 0;                // spike counters per node (groups of right-hand sides of the widest node)
 };
 
 LVBA_NHD void tri_dec(long long t, int& a, int& b) {
@@ -381,8 +394,11 @@ inline void build_level_jobs(const Plan& P, const Tables& t, const int* first_re
                                    (t.prog && v.ks > 0) ? t.prog + id : nullptr});
       J.back.push_back(BacksolveJob{e, Lp, t.x + 6 * (long long)v.r0, v.npiv});
       if (v.ks > 0) {
-        J.spike.push_back(SpikeJob{e, Lp, v.npiv, t.E + v.offE, v.kind == 0 ? v.nE : v.npiv, t.Z + v.offZ, v.ks, t.prog ? t.prog + id : nullptr});
-        J.syrk.push_back(SyrkSeg{t.Z + v.offZ, t.dinv + 36 * (long long)v.r0, zp, v.npiv, v.ks, t.U + v.offU, t.u + v.offu});
+        int* zprog = t.prog ? t.prog + (long long)P.nodes.size() + (long long)id * t.zstride : nullptr;
+        J.spike.push_back(SpikeJob{e, Lp, v.npiv, t.E + v.offE, v.kind == 0 ? v.nE : v.npiv, t.Z + v.offZ, v.ks, t.prog ? t.prog + id : nullptr,
+                                   zprog});
+        J.syrk.push_back(SyrkSeg{t.Z + v.offZ, t.dinv + 36 * (long long)v.r0, zp, v.npiv, v.ks, t.U + v.offU, t.u + v.offu,
+                                 t.prog ? t.prog + id : nullptr, zprog, e.n});
         J.max_ks = std::max(J.max_ks, v.ks);
       }
       J.max_rows = std::max(J.max_rows, v.npiv);
@@ -418,7 +434,7 @@ template <class Exec>
 inline void run_up_local(Exec& ex, const Plan& P, const Tables& t, const LevelDev* lv, int n_levels, long long nblocks,
                          long long leaf_e, long long leaf_fin, const RegionDev* reg) {
   ex.copy(t.L, t.H, nblocks * 36);
-  if (t.prog) ex.pass((long long)P.nodes.size(), ZeroProgF{t.prog});
+  if (t.prog) ex.pass((long long)P.nodes.size() * (1 + t.zstride), ZeroProgF{t.prog});
   ex.pass((long long)6 * t.n, AddDiagF{t});
   ex.zero(t.U, P.sizeU);
   // ---- leaves

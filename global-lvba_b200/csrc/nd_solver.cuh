@@ -26,9 +26,10 @@ struct NdDevice {
   int n_ranks = 1, my_rank = 0;
   DevBuf<double> xchg;                     // multi-GPU: rows received from the left neighbour (exchange_rows)
   DevBuf<unsigned short> d_dense_map;      // thread -> block of nd_dense_factor_kernel
-  // the spike kernels start while the factorisation they read from is still running and follow its progress counters
-  // (programmatic dependent launch)
-  DevBuf<int> d_prog;                      // [nodes]
+  // the spike kernels start while the factorisation they read from is still running and follow its progress counters, and
+  // the SYRK starts while the spike is running and follows the counters of the spike CTAs (programmatic dependent launch)
+  DevBuf<int> d_prog;                      // [nodes] factorisations, then [nodes][zstride] spike CTAs (nd::Tables::prog)
+  int zstride = 0;
   // numeric pools
   DevBuf<double> zs, U, u, Z, E, T, W, w;
   // job tables (rebuilt when the caller's pointers change)
@@ -55,11 +56,16 @@ struct NdDevice {
   // number of chunks for a system of n block rows with columns of at most max_col blocks: the chain is
   // (interior) + (tree depth) x (separator width) pivot columns; more chunks shorten the first term and lengthen the second
   static int default_chunks(int n, int max_col) {
-    // a leaf costs a fixed time per row (factor + spike + substitutions), a tree level a time linear in the separator width
-    // w; the twisted pair a (smaller) time per row of the whole system.  Interiors of about three band widths balance the
-    // two terms; below ~800 rows the two-CTA twisted solve wins (tools/solver_bench.py measures the crossover).
+    // a leaf costs a fixed time per row (factor + spike + substitutions), a tree level a time that grows with the separator
+    // width w; the twisted pair a (smaller) time per row of the whole system.  More chunks also mean more leaf factorisations
+    // and spikes at once, which crowd the SMs, so the best p grows more slowly than n: the largest power of two up to
+    // 16 sqrt(n) / w.  tools/solver_bench.py on an H100 80GB HBM3 at a 400 W power limit, with the SYRK beside the spike
+    // (ms per solve, p = 16 / 24 / 32 / 64): 2000x30 0.852 / 0.866 / 0.901 / 1.144 -> 16; 2000x20 0.595 / 0.588 / 0.573 / 0.701
+    // -> 32; 5000x30 1.477 / 1.306 / 1.316 / 1.559 -> 32; 5000x20 1.033 / 0.895 / 0.816 / 0.937 -> 32.  (The former rule,
+    // n / (3 w + 30), took 16 at 2000x20 and would take 64 from ~4600 rows at w = 20.)  Below ~800 rows the two-CTA twisted
+    // solve wins.
     if (n < 768) return 0;
-    const long long want = (long long)n / (3LL * max_col + 30);
+    const double want = 16.0 * sqrt((double)n) / max_col;
     int best = 0;
     for (int p = 4; p <= 256 && p <= want; p *= 2) best = p;
     return best;
@@ -121,7 +127,9 @@ struct NdDevice {
       }
       LVBA_TRY(xchg.alloc((size_t)std::max<long long>(mx, 1)));
     }
-    LVBA_TRY(d_prog.alloc(plan.nodes.size()));
+    zstride = 0;
+    for (const nd::Node& v : plan.nodes) zstride = std::max(zstride, (v.ks + kSpikeCols - 1) / kSpikeCols);
+    LVBA_TRY(d_prog.alloc(plan.nodes.size() * (size_t)(1 + zstride)));
     LVBA_CUDA(cudaFuncSetAttribute(nd_spike_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSpikeSmem));
     LVBA_CUDA(cudaFuncSetAttribute(nd_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
     LVBA_CUDA(cudaFuncSetAttribute(nd_dense_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kDenseSmem));
@@ -143,7 +151,7 @@ struct NdDevice {
     tab.U = U.p; tab.u = U.p; tab.Z = Z.p; tab.E = E.p; tab.T = T.p; tab.W = W.p; tab.w = w.p;
     tab.Hw = n_ranks > 1 ? const_cast<double*>(H) : nullptr;       // multi-GPU: the other ranks' rank-separator rows are written into
     tab.daddw = n_ranks > 1 ? const_cast<double*>(dadd) : nullptr; // the caller's H / dadd (documented at EnvSolver::solve)
-    tab.prog = d_prog.p;
+    tab.prog = d_prog.p; tab.zstride = zstride;
     std::vector<nd::LevelJobs> jobs;
     nd::DenseViewArrays dv{d_zeros.p, d_tri.p, d_last_by_w.p};
     nd::build_level_jobs(plan, tab, d_first_rel.p, d_rs_adj.p, d_last_rel.p, genv.nblocks, dv, status + 1, jobs, my_rank);
@@ -214,8 +222,19 @@ struct NdCudaExec {
   }
   void syrk(const nd::SyrkSeg* segs, int n, int max_ks, int max_rows) {
     if (n <= 0 || max_ks <= 0) return;
+    // the kernel launched just before this one is the spike whose Z these segments read: start as soon as all of ITS CTAs run
+    // (nd_syrk_kernel says why nothing can starve).  Row groups are the slowest grid dimension, so that the CTAs of the first
+    // rows of every segment are placed first.
     const int nt1 = (max_ks + kSyrkTile - 1) / kSyrkTile, nt = nt1 * (nt1 + 1) / 2;
-    nd_syrk_kernel<<<dim3(nt, (max_rows + kSyrkSplit - 1) / kSyrkSplit, n), kSyrkThreads, kSyrkSmem, s>>>(segs, kSyrkSplit);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(nt, n, (max_rows + kSyrkSplit - 1) / kSyrkSplit); cfg.blockDim = dim3(kSyrkThreads); cfg.dynamicSmemBytes = kSyrkSmem;
+    cfg.stream = s;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, nd_syrk_kernel, segs, kSyrkSplit);
+    if (e != cudaSuccess) rc = fail(LVBA_ERR_CUDA, "cudaLaunchKernelEx(nd_syrk_kernel): %s", cudaGetErrorString(e));
     ++launches;
   }
   void correct_apply(const nd::Tables& t, const int* ids, int n_ids, int stride) {
