@@ -57,7 +57,7 @@ class LvbaError(RuntimeError):
 
 class LidarOpts(C.Structure):
     _fields_ = [("u0", C.c_double), ("v0", C.c_double), ("max_iter", C.c_int32), ("rel_tol", C.c_double),
-                ("device", C.c_int32), ("verbose", C.c_int32)]
+                ("device", C.c_int32), ("verbose", C.c_int32), ("deterministic", C.c_int32)]
 
 
 class VisualOpts(C.Structure):
@@ -65,7 +65,8 @@ class VisualOpts(C.Structure):
                 ("min_radius", C.c_double), ("min_lm_diagonal", C.c_double), ("max_lm_diagonal", C.c_double),
                 ("min_relative_decrease", C.c_double), ("function_tolerance", C.c_double),
                 ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double),
-                ("jacobi_scaling", C.c_int32), ("device", C.c_int32), ("verbose", C.c_int32)]
+                ("jacobi_scaling", C.c_int32), ("device", C.c_int32), ("verbose", C.c_int32),
+                ("deterministic", C.c_int32)]
 
 
 class Summary(C.Structure):

@@ -169,7 +169,11 @@ lidar_residual_kernel(LidarView lv, const double* __restrict__ poses, double* __
 }
 
 // ------------------------------------------------------------------------------------------------
-// Hessian + gradient + residual build: one CTA of kTileSlots threads per tile
+// Hessian + gradient + residual build: one CTA of kTileSlots threads per tile.
+// kDet = false: every run's sum goes into H and g by RED.  kDet = true (deterministic mode): H and g are the records of
+// tiles::FixedSum (lidar_tiles.h) and every run's sum is stored into its own: the pair runs' blocks at H[r], the pose runs'
+// diagonal blocks at H[n_pair_runs + r] and their gradient rows at g[r]; tiles::GatherF adds them up in a fixed order.
+template <bool kDet>
 __global__ void __launch_bounds__(kTileSlots, 512 / kTileSlots)
 lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, double* __restrict__ H,
                    double* __restrict__ g, double* __restrict__ batch_res) {
@@ -336,7 +340,8 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
       const int qa = sDRun[r], qb = sDRun[r + 1];
       double v = 0.0;
       for (int q = qa; q < qb; ++q) v += stage[sDSlot[q] * kLStage + el];
-      atomicAdd(H + sDiag[sDSlot[qa]] + 18 * half + el, v);
+      if constexpr (kDet) H[(lv.tile_prun[lv.n_tiles] + d0 + r) * 36 + 18 * half + el] = v;
+      else atomicAdd(H + sDiag[sDSlot[qa]] + 18 * half + el, v);
     }
   }
   for (int e = tid; e < nd * 6; e += S) {
@@ -344,7 +349,8 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
     const int qa = sDRun[r], qb = sDRun[r + 1];
     double v = 0.0;
     for (int q = qa; q < qb; ++q) v += sG[sDSlot[q] * 6 + el];
-    atomicAdd(g + 6 * (long long)sPose[sDSlot[qa]] + el, v);
+    if constexpr (kDet) g[(d0 + r) * 6 + el] = v;
+    else atomicAdd(g + 6 * (long long)sPose[sDSlot[qa]] + el, v);
   }
 
   // ---- phase 4b: off-diagonal blocks.  The tile's pose pairs come grouped by destination block (runs); every warp takes 8
@@ -366,7 +372,9 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
     const int64_t qa = lv.prun_ptr[r0 + c + pq], qb = lv.prun_ptr[r0 + c + pq + 1];
     unsigned code = lv.pairs[qa];
     // lower-triangle block: row = larger pose (slot lj, ascending order inside a voxel), col = slot li
-    double* dst = H + (sRowRS[code >> 16] + (sPose[code & 0xffff] - sRowFirst[code >> 16])) * 36 + k;
+    double* dst;
+    if constexpr (kDet) dst = H + (r0 + c + pq) * 36 + k;
+    else dst = H + (sRowRS[code >> 16] + (sPose[code & 0xffff] - sRowFirst[code >> 16])) * 36 + k;
     double acc[9];
 #pragma unroll
     for (int m = 0; m < 9; ++m) acc[m] = 0.0;
@@ -393,7 +401,10 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
       code = code_next;
     }
 #pragma unroll
-    for (int m = 0; m < 9; ++m) atomicAdd(dst + 4 * m, acc[m]);
+    for (int m = 0; m < 9; ++m) {
+      if constexpr (kDet) dst[4 * m] = acc[m];
+      else atomicAdd(dst + 4 * m, acc[m]);
+    }
   }
 }
 

@@ -129,6 +129,10 @@ struct lvba_lidar_problem {
   lvba::DevBuf<int64_t> big_vox_ptr, big_pair_ptr;
   lvba::DevBuf<int32_t> big_pose;
   lvba::DevBuf<double> big_cl, big_params, big_feat;
+  // ---- deterministic mode (lvba_lidar_opts::deterministic): the records of every contribution to H and g and the order in
+  // which they are summed, set up when a reset first asks for the mode (lidar_det_setup)
+  bool det = false, det_ready = false;
+  lvba::tiles::FixedSum<lvba::CudaExec> det_H, det_g;
   lvba::big::View big_view() const {
     return lvba::big::View{(int64_t)n_big, big_vox_ptr.p, big_pose.p, big_cl.p, big_pair_ptr.p, env.d_first.p, env.d_row_start.p};
   }
@@ -433,7 +437,7 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   LVBA_TRY(P->batch_res.alloc((size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1)));
   LVBA_TRY(P->scal.alloc(8));
   LVBA_TRY(P->scal.zero(s));
-  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
   LVBA_CUDA(cudaStreamSynchronize(s));
   aos.release();                                               // the caller's records were consumed by the kernels above
   lap("index upload+allocs");
@@ -443,9 +447,58 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   return LVBA_OK;
 }
 
+// Deterministic mode: the records of the build and their destinations.  Records of H: the tiles' pair runs, the tiles' pose
+// runs, the big voxels' slots, the big voxels' pairs; records of g: the tiles' pose runs, the big voxels' slots.  Each set in
+// its enumeration order, so that every destination's records come in ascending (tile, run) order, then in item order.
+inline int lidar_det_setup(lvba_lidar_problem* P) {
+  if (P->det_ready) return LVBA_OK;
+  const int64_t npr = P->prun.n_runs, ndr = P->drun.n_runs;
+  const int64_t nH = npr + ndr + P->n_big_slots + P->n_big_pairs, ng = ndr + P->n_big_slots;
+  if (nH >= (int64_t)1 << 32) return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode: %lld contributions to H (at most 2^32)", (long long)nH);
+  CudaExec ex;
+  ex.stream = P->stream;
+  LVBA_TRY(tiles::fixed_sum_alloc(P->det_H, nH, 36));
+  LVBA_TRY(tiles::fixed_sum_alloc(P->det_g, ng, 6));
+  if (P->n_tiles > 0) {
+    const tiles::TableIn tin{P->n_tiles, P->W, P->env.nblocks, P->tile_vox.p, P->vox_ptr.p, P->pidx.p, nullptr,
+                             P->env.d_first.p, P->env.d_row_start.p};
+    LVBA_TRY(ex.for_each(npr, tiles::PairRunDstF{tin, P->prun.tile_run.p, P->prun.run_ptr.p, P->prun.code.p, P->det_H.dst.p}));
+    LVBA_TRY(ex.for_each(ndr, tiles::SlotRunDstF{tin, P->drun.tile_run.p, P->drun.run_ptr.p, P->drun.code.p, P->det_H.dst.p + npr,
+                                                 P->det_g.dst.p}));
+  }
+  if (P->n_big > 0) {
+    const big::View bv = P->big_view();
+    LVBA_TRY(ex.for_each(P->n_big_slots, big::SlotDstF{bv, P->det_H.dst.p + npr + ndr, P->det_g.dst.p + ndr}));
+    LVBA_TRY(ex.for_each(P->n_big_pairs, big::PairDstF{bv, P->det_H.dst.p + npr + ndr + P->n_big_slots}));
+  }
+  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_H, P->env.nblocks));
+  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_g, P->W));
+  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
+  P->launches += ex.launches;
+  P->det_ready = true;
+  return LVBA_OK;
+}
+
+// the LM mode of the handle (lvba_lidar_reset_lm and the one-shot calls)
+inline int lidar_set_mode(lvba_lidar_problem* P, const lvba_lidar_opts& o) {
+  if (o.deterministic && comm().active())
+    return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode runs on one GPU: the multi-GPU sums of NCCL have no fixed order");
+  if (o.deterministic) {
+    LVBA_CUDA(cudaSetDevice(P->device));
+    const int rc = lidar_det_setup(P);
+    if (rc != LVBA_OK) {                                      // nothing half set up stays on the handle
+      tiles::fixed_sum_release(P->det_H); tiles::fixed_sum_release(P->det_g);
+      return rc;
+    }
+  }
+  P->det = o.deterministic != 0;
+  P->solver.set_deterministic(P->det);
+  return LVBA_OK;
+}
+
 // voxels seen from more than kSlots poses (lidar_big.h): lambda_0 of voxel b -> batch_res[n_before + b] (after the partials of
 // the tiles or batches); with the Hessian, their gradient / diagonal-block / pair-block contributions are added to g and H by
-// atomics
+// atomics, or in deterministic mode stored into their records
 inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool residual_only, int n_before) {
   cudaStream_t s = P->stream;
   const big::View bv = P->big_view();
@@ -455,9 +508,39 @@ inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool r
     ++P->launches;
   };
   launch((int64_t)P->n_big, big::ParamsF{bv, d_poses, P->big_params.p, P->batch_res.p + n_before});
-  if (!residual_only) {
+  if (!residual_only && P->det) {
+    const int64_t h0 = P->prun.n_runs + P->drun.n_runs, g0 = P->drun.n_runs;
+    launch((int64_t)P->n_big_slots, big::SlotsDetF{bv, d_poses, P->big_params.p, P->big_feat.p, P->det_H.rec.p + 36 * h0, P->det_g.rec.p + 6 * g0});
+    launch((int64_t)P->n_big_pairs, big::PairsDetF{bv, P->big_params.p, P->big_feat.p, P->det_H.rec.p + 36 * (h0 + P->n_big_slots)});
+  } else if (!residual_only) {
     launch((int64_t)P->n_big_slots, big::SlotsF{bv, d_poses, P->big_params.p, P->big_feat.p, P->H.p, P->g.p});
     launch((int64_t)P->n_big_pairs, big::PairsF{bv, P->big_params.p, P->big_feat.p, P->H.p});
+  }
+  LVBA_CUDA(cudaGetLastError());
+  return LVBA_OK;
+}
+
+// H and g at the poses in `d_poses`; the partial residual sums of the tiles and big voxels in batch_res
+inline int lidar_build_hg(lvba_lidar_problem* P, const double* d_poses) {
+  cudaStream_t s = P->stream;
+  LVBA_TRY(P->H.zero(s));
+  LVBA_TRY(P->g.zero(s));
+  if (P->n_tiles > 0) {
+    if (P->det)
+      lidar_build_kernel<true><<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->det_H.rec.p,
+                                                                                         P->det_g.rec.p, P->batch_res.p);
+    else
+      lidar_build_kernel<false><<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->H.p, P->g.p,
+                                                                                          P->batch_res.p);
+    ++P->launches;
+  }
+  if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/false, P->n_tiles));
+  if (P->det) {
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(ex.for_each(P->det_H.by_dst.n_runs * 36, tiles::gather_of(P->det_H, P->H.p)));
+    LVBA_TRY(ex.for_each(P->det_g.by_dst.n_runs * 6, tiles::gather_of(P->det_g, P->g.p)));
+    P->launches += ex.launches;
   }
   LVBA_CUDA(cudaGetLastError());
   return LVBA_OK;
@@ -466,13 +549,7 @@ inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool r
 // H, g, sum(lambda0) at the poses in `d_poses`; result scalar lands in scal[slot]
 inline int lidar_build_dev(lvba_lidar_problem* P, const double* d_poses, int slot) {
   cudaStream_t s = P->stream;
-  LVBA_TRY(P->H.zero(s));
-  LVBA_TRY(P->g.zero(s));
-  if (P->n_tiles > 0) {
-    lidar_build_kernel<<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->H.p, P->g.p, P->batch_res.p);
-    ++P->launches;
-  }
-  if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/false, P->n_tiles));
+  LVBA_TRY(lidar_build_hg(P, d_poses));
   reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_res.p, (int)(P->n_tiles + P->n_big), P->scal.p + slot);
   ++P->launches;
   LVBA_CUDA(cudaGetLastError());
@@ -630,12 +707,7 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
     P->h2d += (int64_t)G * 8;
     // ---- H, g, sum(lambda0) per window
     P->timers.begin(PH_BUILD);
-    LVBA_TRY(P->H.zero(s));
-    LVBA_TRY(P->g.zero(s));
-    if (P->n_tiles > 0) {
-      lidar_build_kernel<<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), ev, P->poses.p, P->H.p, P->g.p, P->batch_res.p);
-      ++P->launches;
-    }
+    LVBA_TRY(lidar_build_hg(P, P->poses.p));
     lidar_group_sum_kernel<<<G, 128, 0, s>>>(P->batch_res.p, P->d_grp_tile.p, P->d_grp_scal.p, 0);
     ++P->launches;
     P->timers.end();
@@ -728,7 +800,7 @@ extern "C" {
 
 void lvba_lidar_default_opts(lvba_lidar_opts* o) {
   if (!o) return;
-  o->u0 = 0.01; o->v0 = 2.0; o->max_iter = 10; o->rel_tol = 1e-6; o->device = -1; o->verbose = 0;
+  o->u0 = 0.01; o->v0 = 2.0; o->max_iter = 10; o->rel_tol = 1e-6; o->device = -1; o->verbose = 0; o->deterministic = 0;
 }
 
 int lvba_lidar_create(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
@@ -819,7 +891,10 @@ int lvba_lidar_get_system(lvba_lidar_problem* p, double* g, double* blocks) LVBA
 
 int lvba_lidar_reset_lm(lvba_lidar_problem* p, const lvba_lidar_opts* opts) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
-  if (opts) p->opts = *opts; else lvba_lidar_default_opts(&p->opts);
+  lvba_lidar_opts o;
+  if (opts) o = *opts; else lvba_lidar_default_opts(&o);
+  LVBA_TRY(lvba::lidar_set_mode(p, o));
+  p->opts = o;
   p->u = p->opts.u0; p->v = p->opts.v0; p->is_calc_hess = true; p->have_first = false; p->converged = false;
   p->iters = p->accepted = p->builds = 0; p->termination = LVBA_TERM_MAX_ITER; p->residual1 = 0.0;
   return LVBA_OK;
@@ -905,8 +980,11 @@ int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, co
   p->opts = o;
   lvba_summary tot;
   memset(&tot, 0, sizeof tot);
-  try { rc = lvba::lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
-  catch (...) { rc = lvba::fail(LVBA_ERR_NOMEM, "host allocation failed in lvba_lidar_lm_batch"); }
+  rc = lvba::lidar_set_mode(p, o);
+  if (rc == LVBA_OK) {
+    try { rc = lvba::lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
+    catch (...) { rc = lvba::fail(LVBA_ERR_NOMEM, "host allocation failed in lvba_lidar_lm_batch"); }
+  }
   if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);     // written back only on success; skipped windows are unchanged on the device
   if (rc == LVBA_OK && total) {
     *total = tot;

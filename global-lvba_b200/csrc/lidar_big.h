@@ -123,7 +123,10 @@ struct ParamsF {               // one item per big voxel
   }
 };
 
-struct SlotsF {                // one item per slot of the big voxels
+// kDet = false: the contributions go into H and g by atomics; true (deterministic mode): H = the slots' records [n_slots][36]
+// and g = [n_slots][6], one record per slot, summed per destination by tiles::GatherF (lidar_tiles.h) in slot order.
+template <bool kDet>
+struct SlotsPass {             // one item per slot of the big voxels
   View bv; const double* poses; const double* params; double* feat; double* H; double* g;
   LVBA_BHD void operator()(int64_t s) const {
     int64_t lo = 0, hi = bv.n_vox;                                                // voxel of the slot
@@ -187,23 +190,37 @@ struct SlotsF {                // one item per slot of the big voxels
         Hd[6 * (3 + j) + i] += hrt;
         Hd[6 * (3 + i) + 3 + j] += c1 * (n - n * n / NN) * uk[i] * uk[j];
       }
-    double* Hb = H + (bv.row_start[pose] + (pose - bv.first[pose])) * 36;
-    for (int i = 0; i < 36; ++i) atomic_add_f64(Hb + i, Hd[i]);
-    for (int j = 0; j < 6; ++j) atomic_add_f64(g + 6 * (int64_t)pose + j, jjt[j]);
+    if constexpr (kDet) {
+      for (int i = 0; i < 36; ++i) H[36 * s + i] = Hd[i];
+      for (int j = 0; j < 6; ++j) g[6 * s + j] = jjt[j];
+    } else {
+      double* Hb = H + (bv.row_start[pose] + (pose - bv.first[pose])) * 36;
+      for (int i = 0; i < 36; ++i) atomic_add_f64(Hb + i, Hd[i]);
+      for (int j = 0; j < 6; ++j) atomic_add_f64(g + 6 * (int64_t)pose + j, jjt[j]);
+    }
   }
 };
 
-struct PairsF {                // one item per slot pair (i < j) of the big voxels
+// slot pair p (i < j) of the big voxels: its voxel lo and its two slots si < sj
+LVBA_BHD void pair_slots(const View& bv, int64_t p, int64_t& lo, int64_t& si, int64_t& sj) {
+  lo = 0;
+  int64_t hi = bv.n_vox;
+  while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if (bv.pair_ptr[mid] <= p) lo = mid; else hi = mid; }
+  const int64_t t = p - bv.pair_ptr[lo];                          // strict lower-triangular index: j > i, t = j (j - 1) / 2 + i
+  int64_t j = (int64_t)((sqrt(8.0 * (double)t + 1.0) + 1.0) * 0.5);
+  while (j * (j - 1) / 2 > t) --j;
+  while ((j + 1) * j / 2 <= t) ++j;
+  const int64_t i = t - j * (j - 1) / 2;
+  si = bv.vox_ptr[lo] + i; sj = bv.vox_ptr[lo] + j;
+}
+
+// kDet = false: the block goes into H by atomics; true: H = the pairs' records [n_pairs][36] (see SlotsF)
+template <bool kDet>
+struct PairsPass {             // one item per slot pair (i < j) of the big voxels
   View bv; const double* params; const double* feat; double* H;
   LVBA_BHD void operator()(int64_t p) const {
-    int64_t lo = 0, hi = bv.n_vox;
-    while (hi - lo > 1) { const int64_t mid = (lo + hi) >> 1; if (bv.pair_ptr[mid] <= p) lo = mid; else hi = mid; }
-    const int64_t t = p - bv.pair_ptr[lo];                        // strict lower-triangular index: j > i, t = j (j - 1) / 2 + i
-    int64_t j = (int64_t)((sqrt(8.0 * (double)t + 1.0) + 1.0) * 0.5);
-    while (j * (j - 1) / 2 > t) --j;
-    while ((j + 1) * j / 2 <= t) ++j;
-    const int64_t i = t - j * (j - 1) / 2;
-    const int64_t si = bv.vox_ptr[lo] + i, sj = bv.vox_ptr[lo] + j;
+    int64_t lo, si, sj;
+    pair_slots(bv, p, lo, si, sj);
     const double* q = params + kParams * lo;
     const double* uk = q; const double* um = q + 3;
     const double NN = q[15];
@@ -222,10 +239,40 @@ struct PairsF {                // one item per slot pair (i < j) of the big voxe
         Hb[6 * (3 + r) + c] += k * ni * uk[r] * fj[18 + c];
         Hb[6 * (3 + r) + 3 + c] += k * ni * nj * uk[r] * uk[c];
       }
-    const int pi = bv.pose_idx[si], pj = bv.pose_idx[sj];             // ascending inside a voxel: pi < pj
-    double* B = H + (bv.row_start[pj] + (pi - bv.first[pj])) * 36;    // lower block (pj, pi) = Hb^T   (:171-173)
-    for (int r = 0; r < 6; ++r)
-      for (int c = 0; c < 6; ++c) atomic_add_f64(B + 6 * c + r, Hb[6 * r + c]);
+    if constexpr (kDet) {
+      for (int r = 0; r < 6; ++r)
+        for (int c = 0; c < 6; ++c) H[36 * p + 6 * c + r] = Hb[6 * r + c];
+    } else {
+      const int pi = bv.pose_idx[si], pj = bv.pose_idx[sj];           // ascending inside a voxel: pi < pj
+      double* B = H + (bv.row_start[pj] + (pi - bv.first[pj])) * 36;  // lower block (pj, pi) = Hb^T   (:171-173)
+      for (int r = 0; r < 6; ++r)
+        for (int c = 0; c < 6; ++c) atomic_add_f64(B + 6 * c + r, Hb[6 * r + c]);
+    }
+  }
+};
+
+using SlotsF = SlotsPass<false>;
+using PairsF = PairsPass<false>;
+using SlotsDetF = SlotsPass<true>;
+using PairsDetF = PairsPass<true>;
+
+// Destinations of the deterministic records of SlotsDetF (the slot's diagonal H block and gradient row) and PairsDetF
+// (the lower H block of the pair), in the units of tiles::FixedSum
+struct SlotDstF {
+  View bv; int64_t* dst_H; int64_t* dst_g;
+  LVBA_BHD void operator()(int64_t s) const {
+    const int pose = bv.pose_idx[s];
+    dst_H[s] = bv.row_start[pose] + (pose - bv.first[pose]);
+    dst_g[s] = pose;
+  }
+};
+struct PairDstF {
+  View bv; int64_t* dst_H;
+  LVBA_BHD void operator()(int64_t p) const {
+    int64_t lo, si, sj;
+    pair_slots(bv, p, lo, si, sj);
+    const int pi = bv.pose_idx[si], pj = bv.pose_idx[sj];
+    dst_H[p] = bv.row_start[pj] + (pi - bv.first[pj]);
   }
 };
 

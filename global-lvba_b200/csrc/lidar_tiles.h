@@ -13,6 +13,7 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <vector>
 
 #if defined(__CUDACC__)
@@ -187,6 +188,99 @@ int build_runs(Ex& ex, const TableIn& in, bool by_slot, int64_t n, Runs<Ex>& out
   if (by_slot) return sort_runs(ex, n, in.n_tiles, (uint64_t)in.W, SlotKeyF{in}, out);
   return sort_runs(ex, n, in.n_tiles, (uint64_t)in.nblocks, PairKeyF{in}, out);
 }
+
+// ---- fixed-order sums (deterministic mode).  Where the default build adds a run's sum into its destination by RED, the
+// deterministic build stores it into a record of its own: the records of the tiles' runs in (tile, run) order, then those of
+// the items of lidar_big.h in item order.  FixedSum lists per destination its records in ascending order (a stable sort of the
+// records by destination), and GatherF adds them up in that order, so that every run gives the same bits.
+template <class Ex>
+struct FixedSum {
+  typename Ex::template Buf<double> rec;     // [n_rec][width] one record per contribution
+  typename Ex::template Buf<int64_t> dst;    // [n_rec] destination of every record, in units of width elements
+  Runs<Ex> by_dst;                           // run r = the records of one destination, ascending
+  int64_t n_rec = 0;
+  int width = 0;
+  int64_t bytes() const {
+    return n_rec * (int64_t)(width * sizeof(double) + sizeof(int64_t) + sizeof(uint32_t)) + (by_dst.n_runs + 3) * (int64_t)sizeof(int64_t);
+  }
+};
+
+template <class Ex>
+int fixed_sum_alloc(FixedSum<Ex>& f, int64_t n_rec, int width) {
+  f.n_rec = n_rec; f.width = width;
+  const int rc = f.rec.alloc((size_t)std::max<int64_t>(n_rec, 1) * (size_t)width);
+  return rc != 0 ? rc : f.dst.alloc((size_t)std::max<int64_t>(n_rec, 1));
+}
+
+// the memory of f (device policy: a set-up that failed part-way leaves nothing on its handle)
+template <class Ex>
+void fixed_sum_release(FixedSum<Ex>& f) {
+  f.rec.release(); f.dst.release(); f.by_dst.code.release(); f.by_dst.run_ptr.release(); f.by_dst.tile_run.release();
+  f.by_dst.n_runs = 0; f.n_rec = 0;
+}
+
+// items 0..n_rec: key = destination, code = record.  A record whose destination is n_dest has none (fixed_sum_index leaves it
+// out of the runs).
+struct RecKeyF {
+  const int64_t* dst; uint64_t* key = nullptr; uint32_t* code = nullptr;
+  LVBA_THD void operator()(int64_t p) const { key[p] = (uint64_t)dst[p]; code[p] = (uint32_t)p; }
+};
+
+// after f.dst is filled: the records grouped by destination (< n_dest); the records keep their order inside a group
+template <class Ex>
+int fixed_sum_index(Ex& ex, FixedSum<Ex>& f, int64_t n_dest) {
+  return sort_runs(ex, f.n_rec, 1, (uint64_t)n_dest, RecKeyF{f.dst.p}, f.by_dst);
+}
+
+// items 0..n_runs * n_el: element el0 + e of destination run r = the sum of its records in ascending order, written to
+// out[destination * n_el + e].  Records are `width` doubles apart.  Destinations without a record are not written.
+struct GatherF {
+  const int64_t* run_ptr; const uint32_t* code; const int64_t* dst; const double* rec; int width, el0, n_el; double* out;
+  LVBA_THD void operator()(int64_t i) const {
+    const int64_t r = i / n_el;
+    const int e = (int)(i - r * n_el);
+    const int64_t qa = run_ptr[r], qb = run_ptr[r + 1];
+    double v = 0.0;
+    for (int64_t q = qa; q < qb; ++q) v += rec[(int64_t)code[q] * width + el0 + e];
+    out[dst[code[qa]] * n_el + e] = v;
+  }
+};
+// the whole record of f's own records
+template <class Ex>
+GatherF gather_of(const FixedSum<Ex>& f, double* out) {
+  return GatherF{f.by_dst.run_ptr.p, f.by_dst.code.p, f.dst.p, f.rec.p, f.width, 0, f.width, out};
+}
+// elements el0 .. el0 + n_el of other records `rec` (width doubles each) with the destinations and order of f
+template <class Ex>
+GatherF gather_part(const FixedSum<Ex>& f, const double* rec, int width, int el0, int n_el, double* out) {
+  return GatherF{f.by_dst.run_ptr.p, f.by_dst.code.p, f.dst.p, rec, width, el0, n_el, out};
+}
+
+// Destinations of the records of the LiDAR build (lidar_build_kernel<true>): one item per pair run (the lower H block of its
+// pose pair), one per pose run (the diagonal H block and the gradient row of its pose).  tile_run / run_ptr / code: a Runs.
+LVBA_THD int64_t tile_of_run(const int64_t* tile_run, int64_t n_tiles, int64_t r) {
+  int64_t t = 0, hi = n_tiles;                                 // the last tile whose runs start at or before r
+  while (hi - t > 1) { const int64_t m = (t + hi) >> 1; if (tile_run[m] <= r) t = m; else hi = m; }
+  return t;
+}
+struct PairRunDstF {
+  TableIn in; const int64_t* tile_run; const int64_t* run_ptr; const uint32_t* code; int64_t* dst_H;
+  LVBA_THD void operator()(int64_t r) const {
+    const int s0 = in.vox_ptr[in.tile_vox[tile_of_run(tile_run, in.n_tiles, r)]];
+    const uint32_t c = code[run_ptr[r]];
+    const int pi = in.pidx[s0 + (int)(c & 0xffff)], pj = in.pidx[s0 + (int)(c >> 16)];
+    dst_H[r] = in.row_start[pj] + (pi - in.first[pj]);
+  }
+};
+struct SlotRunDstF {
+  TableIn in; const int64_t* tile_run; const int64_t* run_ptr; const uint32_t* code; int64_t* dst_H; int64_t* dst_g;
+  LVBA_THD void operator()(int64_t r) const {
+    const int s0 = in.vox_ptr[in.tile_vox[tile_of_run(tile_run, in.n_tiles, r)]];
+    const int pose = in.pidx[s0 + (int)code[run_ptr[r]]];
+    dst_H[r] = in.row_start[pose] + (pose - in.first[pose]);
+    dst_g[r] = pose;
+  }
+};
 
 }  // namespace tiles
 }  // namespace lvba

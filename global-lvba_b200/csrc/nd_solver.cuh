@@ -189,6 +189,7 @@ struct NdCudaExec {
   const unsigned short* dense_map = nullptr;                       // thread -> block of nd_dense_factor_kernel (NdDevice::d_dense_map)
   int64_t launches = 0;
   int rc = LVBA_OK;
+  bool det = false;                                                // deterministic mode: the SYRK without split-K (EnvSolver::det)
   template <class F> void pass(long long n, const F& f) {
     if (n <= 0) return;
     const int grid = (int)std::min<long long>((n + 255) / 256, kNumSMs * 8);
@@ -225,15 +226,17 @@ struct NdCudaExec {
     // the kernel launched just before this one is the spike whose Z these segments read: start as soon as all of ITS CTAs run
     // (nd_syrk_kernel says why nothing can starve).  Row groups are the slowest grid dimension, so that the CTAs of the first
     // rows of every segment are placed first.
+    // Deterministic mode: one row group of all max_rows rows, so that no two CTAs add into one element.
     const int nt1 = (max_ks + kSyrkTile - 1) / kSyrkTile, nt = nt1 * (nt1 + 1) / 2;
+    const int split = det ? std::max(max_rows, 1) : kSyrkSplit;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(nt, n, (max_rows + kSyrkSplit - 1) / kSyrkSplit); cfg.blockDim = dim3(kSyrkThreads); cfg.dynamicSmemBytes = kSyrkSmem;
+    cfg.gridDim = dim3(nt, n, (max_rows + split - 1) / split); cfg.blockDim = dim3(kSyrkThreads); cfg.dynamicSmemBytes = kSyrkSmem;
     cfg.stream = s;
     cudaLaunchAttribute at[1];
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at; cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, nd_syrk_kernel, segs, kSyrkSplit);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, nd_syrk_kernel, segs, split);
     if (e != cudaSuccess) rc = fail(LVBA_ERR_CUDA, "cudaLaunchKernelEx(nd_syrk_kernel): %s", cudaGetErrorString(e));
     ++launches;
   }

@@ -389,6 +389,13 @@ struct EnvSolver {
   // ---- substructured solve (nd_solver.cuh): p chunk interiors + a tree of separators, one CTA per node; chosen for
   //      systems long enough that  interior + depth x separator  pivot columns beat the two halves of the twisted solve
   NdDevice nd;
+  // deterministic mode: the separator SYRK runs without split-K (one CTA per tile covers all rows of its node, so every element
+  // of U and u gets exactly one add); the graph of the other mode is dropped and the solve captured again
+  bool det = false;
+  void set_deterministic(bool d) {
+    if (d != det) nd.drop_graph();
+    det = d;
+  }
   // multi-GPU, row-owned system: rank r owns the rows dist_begin() .. dist_end()-1 of H / S (its chunks, inner separators and
   // its right rank separator); voxels / tracks are assigned to the owner of their lowest row, so a rank's contributions reach
   // at most max_col rows into the next rank's range: exchange_rows() ships exactly those rows
@@ -597,6 +604,7 @@ struct EnvSolver {
     auto record = [&](int64_t* n_launch) -> int {
       NdCudaExec ex;
       ex.s = s;
+      ex.det = det;
       ex.dense_map = nd.d_dense_map.p;
       ex.factor_fn = [&](int max_col, int nj, const FactorJob* jobs) { return launch_factor(pid(max_col), nj, jobs, s, &ex.launches); };
       ex.back_fn = [&](int nj, const BacksolveJob* jobs) { launch_backsolve(nj, jobs, s); };

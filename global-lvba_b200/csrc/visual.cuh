@@ -150,7 +150,10 @@ visual_cost_kernel(VisualView vv, VisualState st, double* __restrict__ batch_cos
 
 // ------------------------------------------------------------------------------------------------
 // unscaled squared column norms (Jacobi scaling, computed when the scale is reset).  One CTA per build tile: the camera
-// columns are summed per row of the tile (row runs of the destination table) before one RED per element.
+// columns are summed per row of the tile (row runs of the destination table) before one RED per element.  kDet = true
+// (deterministic mode): cam_colsq holds records of 6 doubles, and row run r of the tiles stores its sum into record r with a
+// plain store (summed per row by tiles::GatherF in record order).
+template <bool kDet>
 __global__ void __launch_bounds__(kVisTileSlots)
 visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_colsq, double* __restrict__ pt_colsq) {
   constexpr int NS = kVisTileSlots, kC = 9;              // per observation: 3 point columns, 6 camera columns
@@ -198,7 +201,8 @@ visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_co
     const int qa = sDRun[r], qb = sDRun[r + 1];
     double v = 0.0;
     for (int q = qa; q < qb; ++q) v += stage[sDSlot[q] * kC + 3 + a];
-    atomicAdd(cam_colsq + 6 * (long long)vv.obs_row[s0 + sDSlot[qa]] + a, v);
+    if constexpr (kDet) cam_colsq[(d0 + r) * 6 + a] = v;
+    else atomicAdd(cam_colsq + 6 * (long long)vv.obs_row[s0 + sDSlot[qa]] + a, v);
   }
 }
 
@@ -210,6 +214,11 @@ __global__ void visual_scale_kernel(long long n, const double* __restrict__ cols
 
 // ------------------------------------------------------------------------------------------------
 // linearise + Schur-eliminate: S (envelope, lower), rhs, camera column norms, camera gradient.  One CTA per tile.
+// kDet = false: every run's sum goes into S, rhs, cam_colsq and cam_grad by RED.  kDet = true (deterministic mode): S and rhs
+// are the records of tiles::FixedSum and every run stores its sum into its own record: the pair runs' blocks at S[r], the row
+// runs' diagonal blocks at S[n_pair_runs + r] and their rhs | column-norm | gradient rows at rhs[18 r]; cam_colsq and cam_grad
+// are not used.  tiles::GatherF adds the records up in a fixed order.
+template <bool kDet>
 __global__ void __launch_bounds__(kVisTileSlots, 1)
 visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, double* __restrict__ S,
                     double* __restrict__ rhs, double* __restrict__ cam_colsq, double* __restrict__ cam_grad,
@@ -320,16 +329,21 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
     const int qa = sDRun[r], qb = sDRun[r + 1];
     double v = 0.0;
     for (int q = qa; q < qb; ++q) v += stage[sDSlot[q] * kStageStride + el];
-    atomicAdd(S + sDiag[sDSlot[qa]] + el, v);
+    if constexpr (kDet) S[(vv.tile_prun[vv.n_tiles] + d0 + r) * 36 + el] = v;
+    else atomicAdd(S + sDiag[sDSlot[qa]] + el, v);
   }
   for (int e = tid; e < nd * 18; e += NS) {
     const int r = e / 18, el = e - r * 18;
     const int qa = sDRun[r], qb = sDRun[r + 1];
     double v = 0.0;
     for (int q = qa; q < qb; ++q) v += sG[sDSlot[q] * 18 + el];
-    const int which = el / 6, a = el - which * 6;
-    double* dst = (which == 0) ? rhs : (which == 1) ? cam_colsq : cam_grad;
-    atomicAdd(dst + 6 * (long long)sRow[sDSlot[qa]] + a, v);
+    if constexpr (kDet) {
+      rhs[(d0 + r) * 18 + el] = v;
+    } else {
+      const int which = el / 6, a = el - which * 6;
+      double* dst = (which == 0) ? rhs : (which == 1) ? cam_colsq : cam_grad;
+      atomicAdd(dst + 6 * (long long)sRow[sDSlot[qa]] + a, v);
+    }
   }
   // ---- phase 4b: off-diagonal blocks.  The tile's camera-pair contributions come grouped by destination block (runs); every
   //      warp takes 8 runs at a time, sums each block in registers over the pairs of its run and writes it with 9 REDs per lane.
@@ -343,7 +357,9 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
     int64_t qa_next = 0, qb_next = 0;
     if (cn + pq < nr) { qa_next = vv.prun_ptr[r0 + cn + pq]; qb_next = vv.prun_ptr[r0 + cn + pq + 1]; }
     if (c + pq < nr) {
-    double* dst = S + (sRowRS[code & 0xffff] + (sRow[code >> 16] - sRowFirst[code & 0xffff])) * 36 + k;
+    double* dst;
+    if constexpr (kDet) dst = S + (r0 + c + pq) * 36 + k;
+    else dst = S + (sRowRS[code & 0xffff] + (sRow[code >> 16] - sRowFirst[code & 0xffff])) * 36 + k;
     double acc[9];
 #pragma unroll
     for (int m = 0; m < 9; ++m) acc[m] = 0.0;
@@ -370,7 +386,10 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
       code = code_next;
     }
 #pragma unroll
-    for (int m = 0; m < 9; ++m) atomicAdd(dst + 4 * m, acc[m]);
+    for (int m = 0; m < 9; ++m) {
+      if constexpr (kDet) dst[4 * m] = acc[m];
+      else atomicAdd(dst + 4 * m, acc[m]);
+    }
     }
     qa = qa_next; qb = qb_next;
     code = cn + pq < nr ? vv.pairs[qa] : 0u;

@@ -33,6 +33,12 @@ struct lvba_visual_problem {
   long long Tv_small = 0, n_big = 0, n_big_obs = 0, n_big_pairs = 0;
   lvba::DevBuf<int64_t> big_pair_ptr;
   lvba::DevBuf<double> big_obs, big_params;
+  // ---- deterministic mode (lvba_visual_opts::deterministic): the records of every contribution to S and to the camera rows
+  // (rhs | column norms | gradient, and the column norms of the scale pass, which share the rows' records and order), set up
+  // when a reset first asks for the mode (visual_det_setup)
+  bool det = false, det_ready = false;
+  lvba::tiles::FixedSum<lvba::CudaExec> det_S, det_G;
+  lvba::DevBuf<double> det_C;                       // [det_G.n_rec][6] records of the column-norm pass
   lvba::PhaseTimers timers;
   double* h_scal = nullptr;
   int64_t launches = 0, h2d = 0, d2h = 0;
@@ -331,7 +337,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
   LVBA_TRY(P->scal.alloc(16)); LVBA_TRY(P->scal.zero(s));
   LVBA_TRY(P->cam_step.alloc((size_t)M * 6)); LVBA_TRY(P->pt_step.alloc((size_t)std::max<int64_t>(T, 1) * 3));
-  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
   LVBA_CUDA(cudaFuncSetAttribute(visual_backsub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_backsub_smem_bytes()));
   LVBA_CUDA(cudaStreamSynchronize(s));
   lap("uploads + allocations");
@@ -350,17 +356,80 @@ inline void visual_big_launch(lvba_visual_problem* P, int64_t items, const F& f)
   ++P->launches;
 }
 
+// Deterministic mode: the records of the build and their destinations.  Records of S: the tiles' pair runs, the tiles' row runs,
+// the big landmarks' observations, the big landmarks' ordered pairs; records of the camera rows: the tiles' row runs, the big
+// landmarks' observations.  Each set in its enumeration order, so that every destination's records come in ascending (tile, run)
+// order, then in item order.  Observations of constant cameras and pairs outside the lower envelope get a record without a
+// destination.
+inline int visual_det_setup(lvba_visual_problem* P) {
+  if (P->det_ready) return LVBA_OK;
+  const int64_t npr = P->prun.n_runs, ndr = P->drun.n_runs;
+  const int64_t nS = npr + ndr + P->n_big_obs + P->n_big_pairs, nG = ndr + P->n_big_obs;
+  if (nS >= (int64_t)1 << 32) return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode: %lld contributions to S (at most 2^32)", (long long)nS);
+  CudaExec ex;
+  ex.stream = P->stream;
+  LVBA_TRY(tiles::fixed_sum_alloc(P->det_S, nS, 36));
+  LVBA_TRY(tiles::fixed_sum_alloc(P->det_G, nG, 18));
+  LVBA_TRY(P->det_C.alloc((size_t)std::max<int64_t>(nG, 1) * 6));
+  if (P->n_tiles > 0) {
+    const tiles::VisTableIn tin{P->n_tiles, P->n_rows, P->env.nblocks, P->tile_trk.p, P->trk_ptr.p, P->obs_row.p, nullptr,
+                                P->env.d_first.p, P->env.d_row_start.p};
+    LVBA_TRY(ex.for_each(npr, tiles::VisPairRunDstF{tin, P->prun.tile_run.p, P->prun.run_ptr.p, P->prun.code.p, P->det_S.dst.p}));
+    LVBA_TRY(ex.for_each(ndr, tiles::ObsRunDstF{tin, P->drun.tile_run.p, P->drun.run_ptr.p, P->drun.code.p, P->det_S.dst.p + npr,
+                                                P->det_G.dst.p}));
+  }
+  if (P->n_big > 0) {
+    const VisualView vv = P->view();
+    const vbig::View bv = P->big_view();
+    LVBA_TRY(ex.for_each(P->n_big_obs, vbig::ObsDstF{vv, bv, P->env.nblocks, P->n_rows, P->det_S.dst.p + npr + ndr, P->det_G.dst.p + ndr}));
+    LVBA_TRY(ex.for_each(P->n_big_pairs, vbig::PairDstF{vv, bv, P->env.nblocks, P->det_S.dst.p + npr + ndr + P->n_big_obs}));
+  }
+  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_S, P->env.nblocks));
+  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_G, P->n_rows));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
+  P->launches += ex.launches;
+  P->det_ready = true;
+  return LVBA_OK;
+}
+
+// the LM mode of the handle (lvba_visual_reset_lm and the one-shot call)
+inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
+  if (o.deterministic && comm().active())
+    return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode runs on one GPU: the multi-GPU sums of NCCL have no fixed order");
+  if (o.deterministic) {
+    LVBA_CUDA(cudaSetDevice(P->device));
+    const int rc = visual_det_setup(P);
+    if (rc != LVBA_OK) {                                      // nothing half set up stays on the handle
+      tiles::fixed_sum_release(P->det_S); tiles::fixed_sum_release(P->det_G); P->det_C.release();
+      return rc;
+    }
+  }
+  P->det = o.deterministic != 0;
+  P->solver.set_deterministic(P->det);
+  return LVBA_OK;
+}
+
 // Jacobi scaling vectors from the Jacobian at the current state (Ceres: once, at iteration 0)
 inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
   cudaStream_t s = P->stream;
   LVBA_TRY(P->cam_colsq.zero(s));
   if (P->n_tiles > 0) {
-    visual_colnorm_kernel<<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
+    if (P->det) visual_colnorm_kernel<true><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->det_C.p, P->pt_colsq.p);
+    else visual_colnorm_kernel<false><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
     ++P->launches;
   }
   if (P->n_big > 0) {
-    visual_big_launch(P, P->n_big_obs, vbig::ColObsF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p});
+    if (P->det)
+      visual_big_launch(P, P->n_big_obs, vbig::ColObsDetF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->det_C.p + 6 * P->drun.n_runs});
+    else
+      visual_big_launch(P, P->n_big_obs, vbig::ColObsF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p});
     visual_big_launch(P, P->n_big, vbig::ColTrackF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->pt_colsq.p});
+  }
+  if (P->det) {
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(ex.for_each(P->det_G.by_dst.n_runs * 6, tiles::gather_part(P->det_G, P->det_C.p, 6, 0, 6, P->cam_colsq.p)));
+    P->launches += ex.launches;
   }
   Comm& cm = comm();
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->cam_colsq.p, (size_t)P->n_rows * 6, s));
@@ -387,8 +456,12 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
   LVBA_TRY(P->S.zero(s)); LVBA_TRY(P->rhs.zero(s)); LVBA_TRY(P->cam_colsq.zero(s)); LVBA_TRY(P->cam_grad.zero(s));
   LVBA_CUDA(cudaMemsetAsync(P->scal.p + 1, 0, sizeof(double), s));
   if (P->n_tiles > 0) {
-    visual_build_kernel<<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
-        P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
+    if (P->det)
+      visual_build_kernel<true><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
+          P->view(), ev, P->state(), lm, P->det_S.rec.p, P->det_G.rec.p, nullptr, nullptr, P->batch_cost.p, P->batch_gmax.p);
+    else
+      visual_build_kernel<false><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
+          P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
     ++P->launches;
   }
   if (P->n_big > 0) {        // cost and gradient max of landmark b in the partial slots n_tiles + b
@@ -397,8 +470,25 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
     visual_big_launch(P, P->n_big_obs, vbig::ObsF{vv, bv, P->state(), lm, P->big_obs.p});
     visual_big_launch(P, P->n_big, vbig::TrackF{vv, bv, P->state(), lm, P->big_obs.p, P->big_params.p, P->batch_cost.p + P->n_tiles,
                                                 P->batch_gmax.p + P->n_tiles});
-    visual_big_launch(P, P->n_big_obs, vbig::SlotsF{vv, bv, P->big_params.p, P->big_obs.p, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p});
-    visual_big_launch(P, P->n_big_pairs, vbig::PairsF{vv, bv, P->big_obs.p, P->S.p});
+    if (P->det) {
+      const int64_t s0 = P->prun.n_runs + P->drun.n_runs, g0 = P->drun.n_runs;
+      visual_big_launch(P, P->n_big_obs, vbig::SlotsDetF{vv, bv, P->big_params.p, P->big_obs.p, P->det_S.rec.p + 36 * s0,
+                                                         P->det_G.rec.p + 18 * g0, nullptr, nullptr});
+      visual_big_launch(P, P->n_big_pairs, vbig::PairsDetF{vv, bv, P->big_obs.p, P->det_S.rec.p + 36 * (s0 + P->n_big_obs)});
+    } else {
+      visual_big_launch(P, P->n_big_obs, vbig::SlotsF{vv, bv, P->big_params.p, P->big_obs.p, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p});
+      visual_big_launch(P, P->n_big_pairs, vbig::PairsF{vv, bv, P->big_obs.p, P->S.p});
+    }
+  }
+  if (P->det) {
+    CudaExec ex;
+    ex.stream = s;
+    const int64_t nr = P->det_G.by_dst.n_runs;
+    LVBA_TRY(ex.for_each(P->det_S.by_dst.n_runs * 36, tiles::gather_of(P->det_S, P->S.p)));
+    LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 0, 6, P->rhs.p)));
+    LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 6, 6, P->cam_colsq.p)));
+    LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 12, 6, P->cam_grad.p)));
+    P->launches += ex.launches;
   }
   reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_tiles + P->n_big), P->scal.p + 0);
   reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, (int)(P->n_tiles + P->n_big), P->scal.p + 1);
@@ -532,7 +622,7 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
   o->max_iter = 50; o->initial_radius = 1e4; o->max_radius = 1e16; o->min_radius = 1e-32;
   o->min_lm_diagonal = 1e-6; o->max_lm_diagonal = 1e32; o->min_relative_decrease = 1e-3;
   o->function_tolerance = 1e-6; o->gradient_tolerance = 1e-10; o->parameter_tolerance = 1e-8;
-  o->jacobi_scaling = 1; o->device = -1; o->verbose = 0;
+  o->jacobi_scaling = 1; o->device = -1; o->verbose = 0; o->deterministic = 0;
 }
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
@@ -642,7 +732,10 @@ int lvba_visual_get_system(lvba_visual_problem* p, double* rhs, double* blocks) 
 
 int lvba_visual_reset_lm(lvba_visual_problem* p, const lvba_visual_opts* opts) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
-  if (opts) p->opts = *opts; else lvba_visual_default_opts(&p->opts);
+  lvba_visual_opts o;
+  if (opts) o = *opts; else lvba_visual_default_opts(&o);
+  LVBA_TRY(lvba::visual_set_mode(p, o));
+  p->opts = o;
   p->radius = p->opts.initial_radius; p->nu = 2.0; p->have_scale = false; p->have_first = false; p->converged = false;
   p->iters = p->accepted = p->builds = p->invalid = 0; p->termination = LVBA_TERM_MAX_ITER;
   return LVBA_OK;

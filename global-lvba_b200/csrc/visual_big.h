@@ -120,7 +120,11 @@ struct TrackF {                // one item per big landmark; cost[b] = 1/2 sum r
   }
 };
 
-struct SlotsF {                // one item per observation of the big landmarks
+// kDet = false: the camera-side sums go into S, rhs, cam_colsq and cam_grad by atomics.  true (deterministic mode): S = the
+// observations' records [n_obs][36] and rhs = [n_obs][18] (rhs | column norms | gradient), one record per observation, summed per
+// destination by tiles::GatherF (lidar_tiles.h) in observation order; cam_colsq and cam_grad are not used.
+template <bool kDet>
+struct SlotsPass {             // one item per observation of the big landmarks
   VisualView vv; View bv; const double* params; double* obs; double* S; double* rhs; double* cam_colsq; double* cam_grad;
   LVBA_BHD void operator()(int64_t i) const {
     const int64_t s = vv.trk_ptr[bv.t0] + i;
@@ -136,40 +140,63 @@ struct SlotsF {                // one item per observation of the big landmarks
       for (int m = 0; m < 3; ++m) E[3 * a + m] = Jc[a] * JX[m] + Jc[6 + a] * JX[3 + m];
     for (int a = 0; a < 6; ++a)
       for (int m = 0; m < 3; ++m) Y[3 * a + m] = E[3 * a] * Ci[m] + E[3 * a + 1] * Ci[3 + m] + E[3 * a + 2] * Ci[6 + m];
-    double* D = S + (bv.row_start[row] + (row - bv.first[row])) * 36;
     for (int a = 0; a < 6; ++a) {
       const double gc = Jc[a] * r[0] + Jc[6 + a] * r[1];
-      big::atomic_add_f64(rhs + 6 * (int64_t)row + a, -(gc - (E[3 * a] * p[9] + E[3 * a + 1] * p[10] + E[3 * a + 2] * p[11])));
-      big::atomic_add_f64(cam_colsq + 6 * (int64_t)row + a, Jc[a] * Jc[a] + Jc[6 + a] * Jc[6 + a]);
-      big::atomic_add_f64(cam_grad + 6 * (int64_t)row + a, gc);
-      for (int c = 0; c < 6; ++c)
-        big::atomic_add_f64(D + 6 * a + c, Jc[a] * Jc[c] + Jc[6 + a] * Jc[6 + c]
-                                           - (Y[3 * a] * E[3 * c] + Y[3 * a + 1] * E[3 * c + 1] + Y[3 * a + 2] * E[3 * c + 2]));
+      const double ra = -(gc - (E[3 * a] * p[9] + E[3 * a + 1] * p[10] + E[3 * a + 2] * p[11]));
+      const double ca = Jc[a] * Jc[a] + Jc[6 + a] * Jc[6 + a];
+      if constexpr (kDet) {
+        double* G = rhs + 18 * i;
+        G[a] = ra; G[6 + a] = ca; G[12 + a] = gc;
+      } else {
+        big::atomic_add_f64(rhs + 6 * (int64_t)row + a, ra);
+        big::atomic_add_f64(cam_colsq + 6 * (int64_t)row + a, ca);
+        big::atomic_add_f64(cam_grad + 6 * (int64_t)row + a, gc);
+      }
+      for (int c = 0; c < 6; ++c) {
+        const double d = Jc[a] * Jc[c] + Jc[6 + a] * Jc[6 + c]
+                       - (Y[3 * a] * E[3 * c] + Y[3 * a + 1] * E[3 * c + 1] + Y[3 * a + 2] * E[3 * c + 2]);
+        if constexpr (kDet) S[36 * i + 6 * a + c] = d;
+        else big::atomic_add_f64(S + (bv.row_start[row] + (row - bv.first[row])) * 36 + 6 * a + c, d);
+      }
     }
   }
 };
 
-struct PairsF {                // one item per ordered observation pair (x, y), x != y, of a big landmark
+// ordered observation pair p (x != y) of the big landmarks: its two observations in the local CSR
+LVBA_BHD void pair_obs(const VisualView& vv, const View& bv, int64_t p, int64_t& sx, int64_t& sy) {
+  int64_t b = 0, hi = bv.n_big;
+  while (hi - b > 1) { const int64_t m = (b + hi) >> 1; if (bv.pair_ptr[m] <= p) b = m; else hi = m; }
+  const int64_t k = bv.t0 + b;
+  const int64_t r = p - bv.pair_ptr[b], K1 = vv.trk_ptr[k + 1] - vv.trk_ptr[k] - 1;
+  const int64_t x = r / K1, y0 = r - x * K1, y = y0 + (y0 >= x);
+  sx = vv.trk_ptr[k] + x; sy = vv.trk_ptr[k] + y;
+}
+
+// kDet = false: the block goes into S by atomics; true: S = the pairs' records [n_pairs][36] (see SlotsPass)
+template <bool kDet>
+struct PairsPass {             // one item per ordered observation pair (x, y), x != y, of a big landmark
   VisualView vv; View bv; const double* obs; double* S;
   LVBA_BHD void operator()(int64_t p) const {
-    int64_t b = 0, hi = bv.n_big;
-    while (hi - b > 1) { const int64_t m = (b + hi) >> 1; if (bv.pair_ptr[m] <= p) b = m; else hi = m; }
-    const int64_t k = bv.t0 + b, base = vv.trk_ptr[bv.t0];
-    const int64_t r = p - bv.pair_ptr[b], K1 = vv.trk_ptr[k + 1] - vv.trk_ptr[k] - 1;
-    const int64_t x = r / K1, y0 = r - x * K1, y = y0 + (y0 >= x);
-    const int64_t sx = vv.trk_ptr[k] + x, sy = vv.trk_ptr[k] + y;
+    const int64_t base = vv.trk_ptr[bv.t0];
+    int64_t sx, sy;
+    pair_obs(vv, bv, p, sx, sy);
     const int rx = vv.obs_row[sx], ry = vv.obs_row[sy];
     if (!(ry >= 0 && rx >= ry)) return;
     const double* Yx = obs + kObs * (sx - base) + kObY;
     const double* Ey = obs + kObs * (sy - base) + kObE;
-    double* B = S + (bv.row_start[rx] + (ry - bv.first[rx])) * 36;
+    double* B = kDet ? S + 36 * p : S + (bv.row_start[rx] + (ry - bv.first[rx])) * 36;
     for (int a = 0; a < 6; ++a)
-      for (int c = 0; c < 6; ++c)
-        big::atomic_add_f64(B + 6 * a + c, -(Yx[3 * a] * Ey[3 * c] + Yx[3 * a + 1] * Ey[3 * c + 1] + Yx[3 * a + 2] * Ey[3 * c + 2]));
+      for (int c = 0; c < 6; ++c) {
+        const double d = -(Yx[3 * a] * Ey[3 * c] + Yx[3 * a + 1] * Ey[3 * c + 1] + Yx[3 * a + 2] * Ey[3 * c + 2]);
+        if constexpr (kDet) B[6 * a + c] = d;
+        else big::atomic_add_f64(B + 6 * a + c, d);
+      }
   }
 };
 
-struct ColObsF {               // unscaled column norms, one item per observation: camera columns by atomics, point columns kept
+// kDet = false: camera columns into cam_colsq by atomics; true: cam_colsq = the observations' records [n_obs][6]
+template <bool kDet>
+struct ColObsPass {            // unscaled column norms, one item per observation: camera columns by atomics, point columns kept
   VisualView vv; View bv; VisualState st; double* obs; double* cam_colsq;
   LVBA_BHD void operator()(int64_t i) const {
     const int64_t s = vv.trk_ptr[bv.t0] + i, k = track_of(vv, bv, s);
@@ -183,7 +210,39 @@ struct ColObsF {               // unscaled column norms, one item per observatio
     sg[1] = o.JX[1] * o.JX[1] + o.JX[4] * o.JX[4];
     sg[2] = o.JX[2] * o.JX[2] + o.JX[5] * o.JX[5];
     if (row >= 0)
-      for (int a = 0; a < 6; ++a) big::atomic_add_f64(cam_colsq + 6 * (int64_t)row + a, o.Jc[a] * o.Jc[a] + o.Jc[6 + a] * o.Jc[6 + a]);
+      for (int a = 0; a < 6; ++a) {
+        const double c = o.Jc[a] * o.Jc[a] + o.Jc[6 + a] * o.Jc[6 + a];
+        if constexpr (kDet) cam_colsq[6 * i + a] = c;
+        else big::atomic_add_f64(cam_colsq + 6 * (int64_t)row + a, c);
+      }
+  }
+};
+
+using SlotsF = SlotsPass<false>;
+using PairsF = PairsPass<false>;
+using ColObsF = ColObsPass<false>;
+using SlotsDetF = SlotsPass<true>;
+using PairsDetF = PairsPass<true>;
+using ColObsDetF = ColObsPass<true>;
+
+// Destinations of the deterministic records of SlotsDetF / ColObsDetF (the observation's diagonal S block and its row) and of
+// PairsDetF (the lower S block of the pair), in the units of tiles::FixedSum; n_blocks / n_rows mark a record without one
+// (a constant camera, or a pair that is not in the lower envelope)
+struct ObsDstF {
+  VisualView vv; View bv; long long n_blocks; int n_rows; int64_t* dst_S; int64_t* dst_row;
+  LVBA_BHD void operator()(int64_t i) const {
+    const int row = vv.obs_row[vv.trk_ptr[bv.t0] + i];
+    dst_S[i] = row >= 0 ? bv.row_start[row] + (row - bv.first[row]) : n_blocks;
+    dst_row[i] = row >= 0 ? row : n_rows;
+  }
+};
+struct PairDstF {
+  VisualView vv; View bv; long long n_blocks; int64_t* dst_S;
+  LVBA_BHD void operator()(int64_t p) const {
+    int64_t sx, sy;
+    pair_obs(vv, bv, p, sx, sy);
+    const int rx = vv.obs_row[sx], ry = vv.obs_row[sy];
+    dst_S[p] = (ry >= 0 && rx >= ry) ? bv.row_start[rx] + (ry - bv.first[rx]) : n_blocks;
   }
 };
 

@@ -85,5 +85,27 @@ struct ObsKeyF {
   }
 };
 
+// Destinations of the records of the deterministic visual build (visual_build_kernel<true>, visual_colnorm_kernel<true>), in
+// the units of FixedSum (lidar_tiles.h): one item per pair run (its lower S block), one per row run (the row's diagonal S block
+// and its rhs / column-norm / gradient row).  tile_run / run_ptr / code: a Runs.
+struct VisPairRunDstF {
+  VisTableIn in; const int64_t* tile_run; const int64_t* run_ptr; const uint32_t* code; int64_t* dst_S;
+  LVBA_THD void operator()(int64_t r) const {
+    const int s0 = in.trk_ptr[in.tile_trk[tile_of_run(tile_run, in.n_tiles, r)]];
+    const uint32_t c = code[run_ptr[r]];
+    const int rx = in.obs_row[s0 + (int)(c & 0xffff)], ry = in.obs_row[s0 + (int)(c >> 16)];
+    dst_S[r] = in.row_start[rx] + (ry - in.first[rx]);
+  }
+};
+struct ObsRunDstF {
+  VisTableIn in; const int64_t* tile_run; const int64_t* run_ptr; const uint32_t* code; int64_t* dst_S; int64_t* dst_row;
+  LVBA_THD void operator()(int64_t r) const {
+    const int s0 = in.trk_ptr[in.tile_trk[tile_of_run(tile_run, in.n_tiles, r)]];
+    const int row = in.obs_row[s0 + (int)code[run_ptr[r]]];
+    dst_S[r] = in.row_start[row] + (row - in.first[row]);
+    dst_row[r] = row;
+  }
+};
+
 }  // namespace tiles
 }  // namespace lvba

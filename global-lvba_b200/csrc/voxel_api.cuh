@@ -271,8 +271,11 @@ int lvba_voxel_map_lidar_lm_batch(lvba_voxel_map* m, double* poses, int32_t min_
   p->opts = o;
   lvba_summary tot;
   memset(&tot, 0, sizeof tot);
-  try { rc = lvba::lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
-  catch (...) { rc = lvba::fail(LVBA_ERR_NOMEM, "host allocation failed in lvba_voxel_map_lidar_lm_batch"); }
+  rc = lvba::lidar_set_mode(p, o);
+  if (rc == LVBA_OK) {
+    try { rc = lvba::lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
+    catch (...) { rc = lvba::fail(LVBA_ERR_NOMEM, "host allocation failed in lvba_voxel_map_lidar_lm_batch"); }
+  }
   if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);
   if (rc == LVBA_OK && total) {
     *total = tot;

@@ -394,11 +394,11 @@ struct VisualResult {
 
 // runVisualBAWithLidarAssist (:144-154) minus the drawing / publishing calls.  x_buf_opt / x_buf_before: the LiDAR poses after
 // and before runLidarBA (equal when it was disabled); eigen_in_force: the eigen-ratio array the last set_eigen_ratio_array call
-// left behind (stage 2's after runLidarBA, bavoxel.hpp:17 otherwise).
+// left behind (stage 2's after runLidarBA, bavoxel.hpp:17 otherwise).  opts: the visual LM's options (null: the defaults).
 inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls, const std::vector<Pose>& x_buf_opt,
                          const std::vector<Pose>& x_buf_before, const std::vector<double>& images_ids, const std::vector<Pose>& image_poses,
                          const KeypointImages& all_keypoints, const MatchTable& all_matches, const float eigen_in_force[4],
-                         VisualResult& res, std::string* err = nullptr) {
+                         VisualResult& res, std::string* err = nullptr, const lvba_visual_opts* opts = nullptr) {
   const int M = (int)images_ids.size();
   if ((int)image_poses.size() != M) { if (err) *err = "Number of images and poses do not match"; return LVBA_ERR_INVALID_ARG; }      // :458-461
   if ((int)all_keypoints.size() != M) { if (err) *err = "all_keypoints.size() must equal #cameras"; return LVBA_ERR_INVALID_ARG; }  // :1429
@@ -518,7 +518,7 @@ inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls,
       obs[(size_t)pi].push_back({cam, all_keypoints[(size_t)cam][(size_t)kp].x, all_keypoints[(size_t)cam][(size_t)kp].y});
     }
   }
-  rc = solve_visual(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01, nullptr, &res.solve);
+  rc = solve_visual(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01, opts, &res.solve);
   if (rc != LVBA_OK) { if (err) *err = std::string("visual LM: ") + lvba_last_error(); return rc; }
   if (res.solve.termination == LVBA_TERM_INVALID_STEPS) return LVBA_OK;                                // ceres::FAILURE, :1647-1650: nothing written back
   for (int k = 0; k < M; ++k) {                                                                       // :1652-1656

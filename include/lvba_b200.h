@@ -48,6 +48,11 @@ typedef struct lvba_lidar_opts {
   double rel_tol;      /* 1e-6  |r1-r2|/r1 stop            (bavoxel.hpp:760); <0 disables the test */
   int32_t device;      /* CUDA device ordinal; -1 = current */
   int32_t verbose;     /* 1: print one line per LM iteration to stderr */
+  int32_t deterministic; /* 0; 1: every device sum in a fixed order, so that identical inputs give bit-identical
+                          * results on every run and in every process on the same GPU model and library build.
+                          * Costs device memory for one record per summed contribution (allocated when a call or
+                          * lvba_lidar_reset_lm first asks for the mode) and build / solve time.  One GPU only: with an
+                          * active communicator (lvba_comm_init) the call returns LVBA_ERR_UNSUPPORTED. */
 } lvba_lidar_opts;
 
 /* ---- path B options: the ceres::Solver::Options in force at src/lvba_system.cpp:1572-1576
@@ -66,6 +71,10 @@ typedef struct lvba_visual_opts {
   int32_t jacobi_scaling;        /* 1 */
   int32_t device;
   int32_t verbose;
+  int32_t deterministic;         /* 0; 1: every device sum in a fixed order, as lvba_lidar_opts::deterministic (the
+                                  * same bits on every run on one GPU model and library build, memory allocated when a
+                                  * call or lvba_visual_reset_lm first asks for it, LVBA_ERR_UNSUPPORTED with an active
+                                  * communicator) */
 } lvba_visual_opts;
 
 typedef enum lvba_termination {

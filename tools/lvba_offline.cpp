@@ -26,6 +26,9 @@
 //                build of the reference (default) or ascending image id (library independent)
 //   --lidar-opt F   skip the LiDAR stage and take its result from F (TUM lines, one per scan — what a previous run wrote)
 //   --check --visual   also load images, image poses and the database, and print their summary and the updated camera poses' checksum
+//   --deterministic   every LM solve (window stage, both global LiDAR stages, the visual stage) in the deterministic mode of
+//                lvba_lidar_opts / lvba_visual_opts: the same dataset gives a byte-identical trajectory, images.txt and points3D.txt on
+//                every run on one GPU model.
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -44,7 +47,7 @@ int main(int argc, char** argv) {
   double voxel[2] = {0.5, 0.5};                                              // BALM_stage1/2 root_voxel_size defaults (dataset_io.cpp:55-57)
   float eigen[2][4] = {{0.3f, 0.1f, 0.06f, 0.03f}, {0.3f, 0.1f, 0.06f, 0.03f}};   // bavoxel.hpp:17
   bool stage1 = true, check = false, window_rel = false, visual = false, lidar = true, have_config = false;
-  bool points3d_lidar = false;
+  bool points3d_lidar = false, deterministic = false;
   int fuse_order = LVBA_FUSE_ORDER_LIBSTDCXX;         // the library's default: what a g++ build of the reference does
   int window = 0;
   double anchor_leaf = 0.1;
@@ -66,6 +69,7 @@ int main(int argc, char** argv) {
     else if (a == "--check") check = true;
     else if (a == "--visual") visual = true;
     else if (a == "--no-lidar") lidar = false;
+    else if (a == "--deterministic") deterministic = true;
     else if (a == "--fuse-order") { const std::string v = next(); if (v == "libstdcxx") fuse_order = LVBA_FUSE_ORDER_LIBSTDCXX; else if (v == "ascending") fuse_order = LVBA_FUSE_ORDER_ASCENDING; else return 64; }
     else if (a == "--points3d") { const std::string v = next(); if (v == "lidar") points3d_lidar = true; else if (v == "landmarks") points3d_lidar = false; else return 64; }
     else if (a == "--db") db_path = next();
@@ -85,6 +89,12 @@ int main(int argc, char** argv) {
   }
   if (data.empty()) { std::fprintf(stderr, "usage: lvba_offline --data DIR [--out FILE] [--check] ...\n"); return 64; }
   if (visual && !have_config) { std::fprintf(stderr, "--visual needs --config FILE (camera model and extrinsics)\n"); return 64; }
+  lvba_lidar_opts lidar_opts;
+  lvba_lidar_default_opts(&lidar_opts);
+  lidar_opts.deterministic = deterministic ? 1 : 0;
+  lvba_visual_opts visual_opts;
+  lvba_visual_default_opts(&visual_opts);
+  visual_opts.deterministic = deterministic ? 1 : 0;
   if (data.back() != '/') data += '/';
   LidarDataset ds;
   std::string err;
@@ -112,7 +122,7 @@ int main(int argc, char** argv) {
   std::vector<lvba_b200::AnchorCloud*> anchor_clouds;
   const bool windows = lidar && window > 0;
   if (windows) {                                                             // runWindowBA (:205-316)
-    const int rc = lvba_b200::run_window_ba(frame_clouds, frames, window, voxel[0], eigen[0], anchor_leaf, window_rel, wba);
+    const int rc = lvba_b200::run_window_ba(frame_clouds, frames, window, voxel[0], eigen[0], anchor_leaf, window_rel, wba, &lidar_opts);
     if (rc != LVBA_OK) { std::fprintf(stderr, "window BA failed (%d): %s\n", rc, lvba_last_error()); return rc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
     size_t pts = 0;
     for (auto& c : wba.anchor_clouds) { anchor_clouds.push_back(&c); pts += c.points.size(); }
@@ -127,7 +137,7 @@ int main(int argc, char** argv) {
     lvba_b200::SurfMap<std::vector<Pose>> surf;
     rc = windows ? surf.build(anchor_clouds, poses, voxel[idx], eigen[idx], &vs) : surf.build(frame_clouds, poses, voxel[idx], eigen[idx], &vs);
     if (rc != LVBA_OK) { std::fprintf(stderr, "stage %d voxel map failed (%d): %s\n", idx + 1, rc, lvba_last_error()); return rc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
-    rc = surf.damping_iter(poses, 0, nullptr, &s);
+    rc = surf.damping_iter(poses, 0, &lidar_opts, &s);
     if (rc != LVBA_OK) { std::fprintf(stderr, "stage %d LM failed (%d): %s\n", idx + 1, rc, lvba_last_error()); return 1; }
     std::printf("{\"stage\": %d, \"voxels\": %lld, \"clusters\": %lld, \"map_ms\": %.3f, \"iterations\": %d, \"accepted\": %d, \"cost_first\": %.9e, \"cost_last\": %.9e, \"lm_ms\": %.3f}\n",
                 idx + 1, (long long)vs.n_voxels, (long long)vs.nnz, vs.ms_total, s.iterations, s.accepted, s.cost_first, s.cost_last, s.ms_total);
@@ -209,7 +219,7 @@ int main(int argc, char** argv) {
   off::VisualResult vr;
   cfg.fuse_map_order = fuse_order;
   const int vrc = off::run_visual_ba(cfg, frame_clouds, frames, frames_before, images_ids, image_poses, keypoints, matches,
-                                     lidar ? eigen[1] : default_eigen, vr, &err);
+                                     lidar ? eigen[1] : default_eigen, vr, &err, &visual_opts);
   if (vrc != LVBA_OK) { std::fprintf(stderr, "visual stage failed (%d): %s\n", vrc, err.c_str()); return vrc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
   std::printf("{\"stage\": \"visual\", \"images\": %zu, \"keypoints\": %lld, \"matches\": %lld, \"depth_valid\": %lld, \"components\": %lld, \"tracks\": %lld, "
               "\"usable_tracks\": %lld, \"anchors\": %d, \"anchor_points\": %lld, \"surf_voxels\": %lld, \"points_kept\": %lld, \"iterations\": %d, "
