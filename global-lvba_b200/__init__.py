@@ -66,7 +66,13 @@ class VisualOpts(C.Structure):
                 ("min_relative_decrease", C.c_double), ("function_tolerance", C.c_double),
                 ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double),
                 ("jacobi_scaling", C.c_int32), ("device", C.c_int32), ("verbose", C.c_int32),
-                ("deterministic", C.c_int32)]
+                ("deterministic", C.c_int32),
+                ("reproj_loss", C.c_int32), ("reproj_loss_scale", C.c_double),
+                ("plane_loss", C.c_int32), ("plane_loss_scale", C.c_double)]
+
+
+# lvba_loss_kind: the robust loss of the reprojection / plane residual blocks (VisualOpts.reproj_loss / plane_loss)
+LOSS_NONE, LOSS_HUBER, LOSS_CAUCHY = 0, 1, 2
 
 
 class Summary(C.Structure):
@@ -166,9 +172,17 @@ def lidar_default_opts():
     return o
 
 
-def visual_default_opts():
+def visual_default_opts(reproj_loss=None, plane_loss=None):
+    """lvba_visual_default_opts; reproj_loss / plane_loss: None (no loss), a kind (LOSS_*, the default scale) or (kind, scale)."""
     o = VisualOpts()
     load_library().lvba_visual_default_opts(C.byref(o))
+    for loss, kind, scale in ((reproj_loss, "reproj_loss", "reproj_loss_scale"), (plane_loss, "plane_loss", "plane_loss_scale")):
+        if loss is None:
+            continue
+        if isinstance(loss, tuple):
+            setattr(o, kind, int(loss[0])); setattr(o, scale, float(loss[1]))
+        else:
+            setattr(o, kind, int(loss))
     return o
 
 

@@ -45,7 +45,9 @@ constexpr int kVFStride = 37;      // Y(18) E(18) + pad
 //   [0..5] Cinv  [6..8] g_p  [9..11] w = Cinv g_p ; returns this thread's observation in `o` (scaled)
 // The CTA (kThreads threads) takes the landmarks t0 .. t1 (<= kThreads observations, <= 256 landmarks).  With `env`, the
 // envelope row_start / first of the observation's row are loaded beside its camera state (rs, fr; untouched when row < 0).
-template <int kThreads, bool kNeedJac>
+// kLoss: the robust losses of vv; cost_part is then sum rho and the residuals (and, with kNeedJac, the Jacobians) are the
+// corrected ones, before the Jacobi scaling.  The plain instantiations (kLoss = false) never read the loss fields.
+template <int kThreads, bool kNeedJac, bool kLoss = false>
 LVBA_DEV void visual_front(const VisualView& vv, const VisualState& st, const VisualLM& lm, int t0, int t1,
                            double* stage, double* sT, ObsEval& o, int& row, int& ltrk, double* Xown,
                            double& cost_part, const EnvView* env = nullptr, long long* rs = nullptr, int* fr = nullptr) {
@@ -68,7 +70,8 @@ LVBA_DEV void visual_front(const VisualView& vv, const VisualState& st, const Vi
     if (env && row >= 0) { *rs = env->row_start[row]; *fr = env->first[row]; }
     Xown[0] = st.X[3 * (long long)tr]; Xown[1] = st.X[3 * (long long)tr + 1]; Xown[2] = st.X[3 * (long long)tr + 2];
     obs_eval<kNeedJac>(vv, st.q + 4 * (long long)cam, st.t + 3 * (long long)cam, Xown, vv.obs_uv[s0 + tid], o);
-    cost_part = o.r[0] * o.r[0] + o.r[1] * o.r[1];
+    if constexpr (kLoss) cost_part = obs_loss<kNeedJac>(vv, o);
+    else cost_part = o.r[0] * o.r[0] + o.r[1] * o.r[1];
     if (kNeedJac) {
       const double* sp = lm.s_pt + 3 * (long long)(t0 + ltrk);
 #pragma unroll
@@ -104,7 +107,8 @@ LVBA_DEV void visual_front(const VisualView& vv, const VisualState& st, const Vi
     const double Xp[3] = {st.X[3 * (long long)tr], st.X[3 * (long long)tr + 1], st.X[3 * (long long)tr + 2]};
     double rp, Jpl[3];
     plane_eval(vv, vv.plane + 4 * (long long)(t0 + tid), Xp, rp, Jpl);
-    cost_part += rp * rp;
+    if constexpr (kLoss) cost_part += plane_loss(vv, rp, Jpl);
+    else cost_part += rp * rp;
     if (kNeedJac) {
       const double* sp = lm.s_pt + 3 * (long long)(t0 + tid);
       Jpl[0] *= sp[0]; Jpl[1] *= sp[1]; Jpl[2] *= sp[2];
@@ -147,13 +151,27 @@ visual_cost_kernel(VisualView vv, VisualState st, double* __restrict__ batch_cos
   const double tot = block_sum<kSlots>(cp, red);
   if (threadIdx.x == 0) batch_cost[blockIdx.x] = 0.5 * tot;
 }
+// 1/2 sum rho partial per batch with the robust losses of vv.  A kernel of its own rather than an instantiation of the one above:
+// that keeps the plain kernel's static shared memory, and with it its code, as it was.
+__global__ void __launch_bounds__(kSlots)
+visual_cost_loss_kernel(VisualView vv, VisualState st, double* __restrict__ batch_cost) {
+  __shared__ double red[32];
+  __shared__ double dummyT[1];
+  ObsEval o;
+  int row, ltrk;
+  double Xown[3], cp;
+  VisualLM lm{1.0, 0.0, 0.0, nullptr, nullptr};
+  visual_front<kSlots, false, true>(vv, st, lm, vv.batch_trk[blockIdx.x], vv.batch_trk[blockIdx.x + 1], nullptr, dummyT, o, row, ltrk, Xown, cp);
+  const double tot = block_sum<kSlots>(cp, red);
+  if (threadIdx.x == 0) batch_cost[blockIdx.x] = 0.5 * tot;
+}
 
 // ------------------------------------------------------------------------------------------------
 // unscaled squared column norms (Jacobi scaling, computed when the scale is reset).  One CTA per build tile: the camera
 // columns are summed per row of the tile (row runs of the destination table) before one RED per element.  kDet = true
 // (deterministic mode): cam_colsq holds records of 6 doubles, and row run r of the tiles stores its sum into record r with a
-// plain store (summed per row by tiles::GatherF in record order).
-template <bool kDet>
+// plain store (summed per row by tiles::GatherF in record order).  kLoss: the norms of the corrected Jacobian.
+template <bool kDet, bool kLoss = false>
 __global__ void __launch_bounds__(kVisTileSlots)
 visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_colsq, double* __restrict__ pt_colsq) {
   constexpr int NS = kVisTileSlots, kC = 9;              // per observation: 3 point columns, 6 camera columns
@@ -175,6 +193,7 @@ visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_co
     const double X[3] = {st.X[3 * (long long)tr], st.X[3 * (long long)tr + 1], st.X[3 * (long long)tr + 2]};
     ObsEval o;
     obs_eval<true>(vv, st.q + 4 * (long long)cam, st.t + 3 * (long long)cam, X, vv.obs_uv[s0 + tid], o);
+    if constexpr (kLoss) obs_loss<true>(vv, o);
     double* sg = stage + tid * kC;
     sg[0] = o.JX[0] * o.JX[0] + o.JX[3] * o.JX[3];
     sg[1] = o.JX[1] * o.JX[1] + o.JX[4] * o.JX[4];
@@ -191,6 +210,7 @@ visual_colnorm_kernel(VisualView vv, VisualState st, double* __restrict__ cam_co
     const double X[3] = {st.X[3 * (long long)tr], st.X[3 * (long long)tr + 1], st.X[3 * (long long)tr + 2]};
     double rp, J[3];
     plane_eval(vv, vv.plane + 4 * (long long)(t0 + tid), X, rp, J);
+    if constexpr (kLoss) plane_loss(vv, rp, J);
     double a0 = J[0] * J[0], a1 = J[1] * J[1], a2 = J[2] * J[2];
     for (int s = lo; s < hi; ++s) { a0 += stage[s * kC]; a1 += stage[s * kC + 1]; a2 += stage[s * kC + 2]; }
     double* o = pt_colsq + 3 * (long long)(t0 + tid);
@@ -217,8 +237,9 @@ __global__ void visual_scale_kernel(long long n, const double* __restrict__ cols
 // kDet = false: every run's sum goes into S, rhs, cam_colsq and cam_grad by RED.  kDet = true (deterministic mode): S and rhs
 // are the records of tiles::FixedSum and every run stores its sum into its own record: the pair runs' blocks at S[r], the row
 // runs' diagonal blocks at S[n_pair_runs + r] and their rhs | column-norm | gradient rows at rhs[18 r]; cam_colsq and cam_grad
-// are not used.  tiles::GatherF adds the records up in a fixed order.
-template <bool kDet>
+// are not used.  tiles::GatherF adds the records up in a fixed order.  kLoss: from the corrected residuals and Jacobians
+// (visual_front), through the same sums.
+template <bool kDet, bool kLoss = false>
 __global__ void __launch_bounds__(kVisTileSlots, 1)
 visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, double* __restrict__ S,
                     double* __restrict__ rhs, double* __restrict__ cam_colsq, double* __restrict__ cam_grad,
@@ -259,7 +280,7 @@ visual_build_kernel(VisualView vv, EnvView env, VisualState st, VisualLM lm, dou
   long long rs = 0;
   int fr = 0;
   double Xown[3], cp;
-  visual_front<NS, true>(vv, st, lm, t0, t1, stage, sT, o, row, ltrk, Xown, cp, &env, &rs, &fr);
+  visual_front<NS, true, kLoss>(vv, st, lm, t0, t1, stage, sT, o, row, ltrk, Xown, cp, &env, &rs, &fr);
   // gradient max-norm (unscaled) of the point blocks
   double gm = 0.0;
   if (tid < nt) {
@@ -404,7 +425,9 @@ constexpr size_t visual_build_smem_bytes() {
 static_assert(visual_build_smem_bytes() + kVisTileSlots <= 227 * 1024, "visual_build_kernel: shared memory above the 227 kB an H100 CTA may hold");
 
 // ------------------------------------------------------------------------------------------------
-// back-substitution y_p = -C^-1 (g_p + sum E^T y_c), model cost change, candidate landmarks
+// back-substitution y_p = -C^-1 (g_p + sum E^T y_c), model cost change, candidate landmarks.  kLoss: the model cost change
+// -(J~ y)^T (r~ + 1/2 J~ y) of the corrected residuals and Jacobians.
+template <bool kLoss>
 __global__ void __launch_bounds__(kSlots)
 visual_backsub_kernel(VisualView vv, VisualState st, VisualLM lm, const double* __restrict__ y_cam,
                       double* __restrict__ X_cand, double* __restrict__ pt_step,
@@ -419,7 +442,7 @@ visual_backsub_kernel(VisualView vv, VisualState st, VisualLM lm, const double* 
   ObsEval o;
   int row, ltrk;
   double Xown[3], cp;
-  visual_front<kSlots, true>(vv, st, lm, t0, t1, stage, sT, o, row, ltrk, Xown, cp);
+  visual_front<kSlots, true, kLoss>(vv, st, lm, t0, t1, stage, sT, o, row, ltrk, Xown, cp);
   double yc[6] = {0, 0, 0, 0, 0, 0};
   if (tid < ns) {
     if (row >= 0)
@@ -456,6 +479,7 @@ visual_backsub_kernel(VisualView vv, VisualState st, VisualLM lm, const double* 
     // plane residual contribution to the model cost change
     double rp, Jpl[3];
     plane_eval(vv, vv.plane + 4 * (long long)(t0 + tid), X, rp, Jpl);
+    if constexpr (kLoss) plane_loss(vv, rp, Jpl);
     const double jy = Jpl[0] * d[0] + Jpl[1] * d[1] + Jpl[2] * d[2];   // J~ y = J (s o y)
     model -= jy * (rp + 0.5 * jy);
   }

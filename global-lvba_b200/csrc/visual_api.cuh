@@ -39,6 +39,11 @@ struct lvba_visual_problem {
   bool det = false, det_ready = false;
   lvba::tiles::FixedSum<lvba::CudaExec> det_S, det_G;
   lvba::DevBuf<double> det_C;                       // [det_G.n_rec][6] records of the column-norm pass
+  // ---- robust losses (lvba_visual_opts::reproj_loss / plane_loss), set by lvba_visual_reset_lm; with either one the passes
+  // run their kLoss instantiations
+  int loss_px = LVBA_LOSS_NONE, loss_pl = LVBA_LOSS_NONE;
+  double loss_a_px = 1.0, loss_a_pl = 0.1;
+  bool robust() const { return loss_px != LVBA_LOSS_NONE || loss_pl != LVBA_LOSS_NONE; }
   lvba::PhaseTimers timers;
   double* h_scal = nullptr;
   int64_t launches = 0, h2d = 0, d2h = 0;
@@ -59,6 +64,7 @@ struct lvba_visual_problem {
     for (int i = 0; i < 8; ++i) v.intr[i] = intr[i];
     v.inv_sigma_px = 1.0 / sigma_px;
     v.inv_sigma_pl = 1.0 / std::max(1e-9, sigma_pl);        // utils.hpp:131
+    v.loss_px = loss_px; v.loss_pl = loss_pl; v.loss_a_px = loss_a_px; v.loss_a_pl = loss_a_pl;
     return v;
   }
   lvba::vbig::View big_view() const { return lvba::vbig::View{(int64_t)n_big, (int64_t)Tv_small, big_pair_ptr.p, env.d_first.p, env.d_row_start.p}; }
@@ -337,8 +343,10 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
   LVBA_TRY(P->scal.alloc(16)); LVBA_TRY(P->scal.zero(s));
   LVBA_TRY(P->cam_step.alloc((size_t)M * 6)); LVBA_TRY(P->pt_step.alloc((size_t)std::max<int64_t>(T, 1) * 3));
-  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
-  LVBA_CUDA(cudaFuncSetAttribute(visual_backsub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_backsub_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_backsub_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_backsub_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_backsub_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_backsub_smem_bytes()));
   LVBA_CUDA(cudaStreamSynchronize(s));
   lap("uploads + allocations");
   lvba_visual_default_opts(&P->opts);
@@ -386,14 +394,30 @@ inline int visual_det_setup(lvba_visual_problem* P) {
   }
   LVBA_TRY(tiles::fixed_sum_index(ex, P->det_S, P->env.nblocks));
   LVBA_TRY(tiles::fixed_sum_index(ex, P->det_G, P->n_rows));
-  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
   P->launches += ex.launches;
   P->det_ready = true;
   return LVBA_OK;
 }
 
-// the LM mode of the handle (lvba_visual_reset_lm and the one-shot call)
+// the robust losses of lvba_visual_opts: a known kind, and for a loss a finite scale > 0 (checked before any device work)
+inline int visual_check_loss(const lvba_visual_opts& o) {
+  const int32_t kinds[2] = {o.reproj_loss, o.plane_loss};
+  const double scales[2] = {o.reproj_loss_scale, o.plane_loss_scale};
+  const char* names[2] = {"reproj_loss", "plane_loss"};
+  for (int i = 0; i < 2; ++i) {
+    if (kinds[i] != LVBA_LOSS_NONE && kinds[i] != LVBA_LOSS_HUBER && kinds[i] != LVBA_LOSS_CAUCHY)
+      return fail(LVBA_ERR_INVALID_ARG, "%s = %d is not an lvba_loss_kind", names[i], (int)kinds[i]);
+    if (kinds[i] != LVBA_LOSS_NONE && !(std::isfinite(scales[i]) && scales[i] > 0.0))
+      return fail(LVBA_ERR_INVALID_ARG, "%s_scale = %g: a loss needs a finite scale > 0", names[i], scales[i]);
+  }
+  return LVBA_OK;
+}
+
+// the LM mode of the handle (lvba_visual_reset_lm and the one-shot call): deterministic mode and the robust losses
 inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
+  LVBA_TRY(visual_check_loss(o));
   if (o.deterministic && comm().active())
     return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode runs on one GPU: the multi-GPU sums of NCCL have no fixed order");
   if (o.deterministic) {
@@ -406,24 +430,28 @@ inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   }
   P->det = o.deterministic != 0;
   P->solver.set_deterministic(P->det);
+  P->loss_px = o.reproj_loss; P->loss_a_px = o.reproj_loss_scale;
+  P->loss_pl = o.plane_loss; P->loss_a_pl = o.plane_loss_scale;
   return LVBA_OK;
 }
 
 // Jacobi scaling vectors from the Jacobian at the current state (Ceres: once, at iteration 0)
-inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
+template <bool kLoss>
+inline int visual_compute_scale_t(lvba_visual_problem* P, int enabled) {
   cudaStream_t s = P->stream;
   LVBA_TRY(P->cam_colsq.zero(s));
   if (P->n_tiles > 0) {
-    if (P->det) visual_colnorm_kernel<true><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->det_C.p, P->pt_colsq.p);
-    else visual_colnorm_kernel<false><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
+    if (P->det) visual_colnorm_kernel<true, kLoss><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->det_C.p, P->pt_colsq.p);
+    else visual_colnorm_kernel<false, kLoss><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
     ++P->launches;
   }
   if (P->n_big > 0) {
     if (P->det)
-      visual_big_launch(P, P->n_big_obs, vbig::ColObsDetF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->det_C.p + 6 * P->drun.n_runs});
+      visual_big_launch(P, P->n_big_obs, vbig::ColObsPass<true, kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p,
+                                                                       P->det_C.p + 6 * P->drun.n_runs});
     else
-      visual_big_launch(P, P->n_big_obs, vbig::ColObsF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p});
-    visual_big_launch(P, P->n_big, vbig::ColTrackF{P->view(), P->big_view(), P->state(), P->big_obs.p, P->pt_colsq.p});
+      visual_big_launch(P, P->n_big_obs, vbig::ColObsPass<false, kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p});
+    visual_big_launch(P, P->n_big, vbig::ColTrackPass<kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p, P->pt_colsq.p});
   }
   if (P->det) {
     CudaExec ex;
@@ -440,6 +468,23 @@ inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
   P->have_scale = true;
   return LVBA_OK;
 }
+inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
+  return P->robust() ? visual_compute_scale_t<true>(P, enabled) : visual_compute_scale_t<false>(P, enabled);
+}
+
+// 1/2 sum r^2 (with a loss: 1/2 sum rho) at the state `st` into *out (device): batches, big landmarks, reduction
+template <bool kLoss>
+inline void visual_cost_t(lvba_visual_problem* P, const VisualState& st, double* out) {
+  cudaStream_t s = P->stream;
+  if (P->n_batches > 0) {
+    if constexpr (kLoss) visual_cost_loss_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), st, P->batch_cost.p);
+    else visual_cost_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), st, P->batch_cost.p);
+    ++P->launches;
+  }
+  if (P->n_big > 0) visual_big_launch(P, P->n_big, vbig::CostPass<kLoss>{P->view(), P->big_view(), st, P->batch_cost.p + P->n_batches});
+  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_batches + P->n_big), out);
+  ++P->launches;
+}
 
 inline VisualLM visual_lm_params(const lvba_visual_problem* P, double radius) {
   return VisualLM{radius, P->opts.min_lm_diagonal, P->opts.max_lm_diagonal, P->s_cam.p, P->s_pt.p};
@@ -447,7 +492,8 @@ inline VisualLM visual_lm_params(const lvba_visual_problem* P, double radius) {
 
 // scal layout: [0] cost  [1] gmax  [2] model  [3] step^2 (pts)  [4] x^2 (pts)  [5] -  [6] step^2 (cams) [7] x^2 (cams)
 //              [8] candidate cost
-inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool want_steps) {
+template <bool kLoss>
+inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool want_steps) {
   cudaStream_t s = P->stream;
   const VisualLM lm = visual_lm_params(P, radius);
   const EnvView ev = P->env.view();
@@ -457,19 +503,19 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
   LVBA_CUDA(cudaMemsetAsync(P->scal.p + 1, 0, sizeof(double), s));
   if (P->n_tiles > 0) {
     if (P->det)
-      visual_build_kernel<true><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
+      visual_build_kernel<true, kLoss><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
           P->view(), ev, P->state(), lm, P->det_S.rec.p, P->det_G.rec.p, nullptr, nullptr, P->batch_cost.p, P->batch_gmax.p);
     else
-      visual_build_kernel<false><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
+      visual_build_kernel<false, kLoss><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
           P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
     ++P->launches;
   }
   if (P->n_big > 0) {        // cost and gradient max of landmark b in the partial slots n_tiles + b
     const VisualView vv = P->view();
     const vbig::View bv = P->big_view();
-    visual_big_launch(P, P->n_big_obs, vbig::ObsF{vv, bv, P->state(), lm, P->big_obs.p});
-    visual_big_launch(P, P->n_big, vbig::TrackF{vv, bv, P->state(), lm, P->big_obs.p, P->big_params.p, P->batch_cost.p + P->n_tiles,
-                                                P->batch_gmax.p + P->n_tiles});
+    visual_big_launch(P, P->n_big_obs, vbig::ObsPass<kLoss>{vv, bv, P->state(), lm, P->big_obs.p});
+    visual_big_launch(P, P->n_big, vbig::TrackPass<kLoss>{vv, bv, P->state(), lm, P->big_obs.p, P->big_params.p,
+                                                          P->batch_cost.p + P->n_tiles, P->batch_gmax.p + P->n_tiles});
     if (P->det) {
       const int64_t s0 = P->prun.n_runs + P->drun.n_runs, g0 = P->drun.n_runs;
       visual_big_launch(P, P->n_big_obs, vbig::SlotsDetF{vv, bv, P->big_params.p, P->big_obs.p, P->det_S.rec.p + 36 * s0,
@@ -515,13 +561,14 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
   P->timers.end();
   P->timers.begin(PH_RESID);
   if (P->n_batches > 0) {
-    visual_backsub_kernel<<<P->n_batches, kSlots, visual_backsub_smem_bytes(), s>>>(
+    visual_backsub_kernel<kLoss><<<P->n_batches, kSlots, visual_backsub_smem_bytes(), s>>>(
         P->view(), P->state(), lm, P->y.p, P->Xc.p, want_steps ? P->pt_step.p : nullptr, P->batch_out.p);
     ++P->launches;
   }
   if (P->n_big > 0)
-    visual_big_launch(P, P->n_big, vbig::BacksubF{P->view(), P->big_view(), P->state(), lm, P->big_obs.p, P->big_params.p, P->y.p, P->Xc.p,
-                                                  want_steps ? P->pt_step.p : nullptr, P->batch_out.p + 4 * (int64_t)P->n_batches});
+    visual_big_launch(P, P->n_big, vbig::BacksubPass<kLoss>{P->view(), P->big_view(), P->state(), lm, P->big_obs.p, P->big_params.p, P->y.p,
+                                                            P->Xc.p, want_steps ? P->pt_step.p : nullptr,
+                                                            P->batch_out.p + 4 * (int64_t)P->n_batches});
   reduce_cols_kernel<<<1, 256, 0, s>>>(P->batch_out.p, (int)(P->n_batches + P->n_big), 4, 3, P->scal.p + 2);
   ++P->launches;
   const int ncb = (P->n_rows + 127) / 128;
@@ -533,14 +580,7 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
   reduce_cols_kernel<<<1, 256, 0, s>>>(P->cam_out.p, ncb, 2, 2, P->scal.p + 6);
   ++P->launches;
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 2, 3, s));   // model, step^2, x^2 of the landmark shard
-  // candidate cost
-  if (P->n_batches > 0) {
-    visual_cost_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->cand(), P->batch_cost.p);
-    ++P->launches;
-  }
-  if (P->n_big > 0) visual_big_launch(P, P->n_big, vbig::CostF{P->view(), P->big_view(), P->cand(), P->batch_cost.p + P->n_batches});
-  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_batches + P->n_big), P->scal.p + 8);
-  ++P->launches;
+  visual_cost_t<kLoss>(P, P->cand(), P->scal.p + 8);                      // candidate cost
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 8, 1, s));
   P->timers.end();
   LVBA_CUDA(cudaGetLastError());
@@ -549,6 +589,9 @@ inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool wa
   LVBA_CUDA(cudaStreamSynchronize(s));
   P->d2h += 16 * sizeof(double);
   return LVBA_OK;
+}
+inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool want_steps) {
+  return P->robust() ? visual_linearize_solve_t<true>(P, radius, want_steps) : visual_linearize_solve_t<false>(P, radius, want_steps);
 }
 
 inline int visual_iterate_impl(lvba_visual_problem* P, int n_iter, lvba_summary* sum) {
@@ -623,6 +666,9 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
   o->min_lm_diagonal = 1e-6; o->max_lm_diagonal = 1e32; o->min_relative_decrease = 1e-3;
   o->function_tolerance = 1e-6; o->gradient_tolerance = 1e-10; o->parameter_tolerance = 1e-8;
   o->jacobi_scaling = 1; o->device = -1; o->verbose = 0; o->deterministic = 0;
+  // no loss (src/lvba_system.cpp:1630, :1639); the scales of the reference's HuberLoss objects (:1585-1586)
+  o->reproj_loss = LVBA_LOSS_NONE; o->reproj_loss_scale = 1.0;
+  o->plane_loss = LVBA_LOSS_NONE; o->plane_loss_scale = 0.1;
 }
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
@@ -680,10 +726,8 @@ int lvba_visual_cost(lvba_visual_problem* p, double* cost) LVBA_ABI_BEGIN {
   if (!p || !cost) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
   LVBA_CUDA(cudaSetDevice(p->device));
   cudaStream_t s = p->stream;
-  if (p->n_batches > 0) { lvba::visual_cost_kernel<<<p->n_batches, lvba::kSlots, 0, s>>>(p->view(), p->state(), p->batch_cost.p); ++p->launches; }
-  if (p->n_big > 0) lvba::visual_big_launch(p, p->n_big, lvba::vbig::CostF{p->view(), p->big_view(), p->state(), p->batch_cost.p + p->n_batches});
-  lvba::reduce_partials_kernel<<<1, 256, 0, s>>>(p->batch_cost.p, (int)(p->n_batches + p->n_big), p->scal.p + 8);
-  ++p->launches;
+  if (p->robust()) lvba::visual_cost_t<true>(p, p->state(), p->scal.p + 8);
+  else lvba::visual_cost_t<false>(p, p->state(), p->scal.p + 8);
   if (lvba::comm().active()) LVBA_TRY(lvba::comm().allreduce_sum(p->scal.p + 8, 1, s));
   LVBA_CUDA(cudaMemcpyAsync(p->h_scal, p->scal.p + 8, sizeof(double), cudaMemcpyDeviceToHost, s));
   LVBA_CUDA(cudaStreamSynchronize(s));
@@ -781,6 +825,7 @@ int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const 
   const double t0 = lvba::wall_ms();
   lvba_visual_opts o;
   if (opts) o = *opts; else lvba_visual_default_opts(&o);
+  LVBA_TRY(lvba::visual_check_loss(o));                       // before any device work: the buffers stay untouched
   lvba_visual_problem* p = nullptr;
   int rc = lvba_visual_create(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, o.device, &p);
   if (rc != LVBA_OK) return rc;

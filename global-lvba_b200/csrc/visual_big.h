@@ -28,8 +28,12 @@
 namespace lvba {
 namespace vbig {
 
-// per observation: r (2), J_c (12), J_X (6) scaled, J_X^T J_X (6) J_X^T r (3) (the point column norms in ColObsF), Y (18), E (18)
+// per observation: r (2), J_c (12), J_X (6) scaled, J_X^T J_X (6) J_X^T r (3) (the point column norms in ColObsF), Y (18), E (18).
+// With a robust loss (kLoss) r, J_c and J_X are the corrected ones, and the slot kObRho holds rho(|r|^2) of the observation
+// from ObsPass until SlotsPass overwrites it with Y (TrackPass reads it in between).
 constexpr int kObR = 0, kObJc = 2, kObJX = 14, kObStage = 20, kObY = 29, kObE = 47, kObs = 65;
+constexpr int kObRho = kObY;
+static_assert(kObRho >= kObY && kObRho < kObY + 18, "rho must sit in the Y slot, which SlotsPass rewrites before any read of Y");
 
 struct View {
   int64_t n_big;                // landmarks with more than kSlots observations
@@ -46,7 +50,9 @@ LVBA_BHD int64_t track_of(const VisualView& vv, const View& bv, int64_t s) {
   return lo;
 }
 
-struct ObsF {                  // one item per observation of the big landmarks
+// kLoss (here and below): the robust losses of vv, the corrected residuals and Jacobians, cost terms rho
+template <bool kLoss>
+struct ObsPass {               // one item per observation of the big landmarks
   VisualView vv; View bv; VisualState st; VisualLM lm; double* obs;
   LVBA_BHD void operator()(int64_t i) const {
     const int64_t s = vv.trk_ptr[bv.t0] + i, k = track_of(vv, bv, s);
@@ -55,6 +61,7 @@ struct ObsF {                  // one item per observation of the big landmarks
     const double X[3] = {st.X[3 * tr], st.X[3 * tr + 1], st.X[3 * tr + 2]};
     ObsEval o;
     obs_eval<true>(vv, st.q + 4 * (int64_t)cam, st.t + 3 * (int64_t)cam, X, vv.obs_uv[s], o);
+    if constexpr (kLoss) obs[kObs * i + kObRho] = obs_loss<true>(vv, o);
     const double* sp = lm.s_pt + 3 * k;
     for (int rho = 0; rho < 2; ++rho)
       for (int m = 0; m < 3; ++m) o.JX[3 * rho + m] *= sp[m];
@@ -82,7 +89,8 @@ struct ObsF {                  // one item per observation of the big landmarks
   }
 };
 
-struct TrackF {                // one item per big landmark; cost[b] = 1/2 sum r^2, gmax[b] = max |g_p| (unscaled)
+template <bool kLoss>
+struct TrackPass {             // one item per big landmark; cost[b] = 1/2 sum r^2 (kLoss: 1/2 sum rho), gmax[b] = max |g_p| (unscaled)
   VisualView vv; View bv; VisualState st; VisualLM lm; const double* obs; double* params; double* cost; double* gmax;
   LVBA_BHD void operator()(int64_t b) const {
     const int64_t k = bv.t0 + b, base = vv.trk_ptr[bv.t0];
@@ -93,12 +101,14 @@ struct TrackF {                // one item per big landmark; cost[b] = 1/2 sum r
     for (int q = 0; q < 9; ++q) acc[q] = 0.0;
     for (int64_t i = lo; i < hi; ++i) {
       const double* f = obs + kObs * i;
-      c += f[kObR] * f[kObR] + f[kObR + 1] * f[kObR + 1];
+      if constexpr (kLoss) c += f[kObRho];
+      else c += f[kObR] * f[kObR] + f[kObR + 1] * f[kObR + 1];
       for (int q = 0; q < 9; ++q) acc[q] += f[kObStage + q];
     }
     double rp, Jpl[3];
     plane_eval(vv, vv.plane + 4 * k, X, rp, Jpl);
-    c += rp * rp;
+    if constexpr (kLoss) c += plane_loss(vv, rp, Jpl);
+    else c += rp * rp;
     const double* sp = lm.s_pt + 3 * k;
     Jpl[0] *= sp[0]; Jpl[1] *= sp[1]; Jpl[2] *= sp[2];
     acc[0] += Jpl[0] * Jpl[0]; acc[1] += Jpl[0] * Jpl[1]; acc[2] += Jpl[0] * Jpl[2];
@@ -123,6 +133,9 @@ struct TrackF {                // one item per big landmark; cost[b] = 1/2 sum r
 // kDet = false: the camera-side sums go into S, rhs, cam_colsq and cam_grad by atomics.  true (deterministic mode): S = the
 // observations' records [n_obs][36] and rhs = [n_obs][18] (rhs | column norms | gradient), one record per observation, summed per
 // destination by tiles::GatherF (lidar_tiles.h) in observation order; cam_colsq and cam_grad are not used.
+// With a loss, kObRho (inside Y) still holds rho from ObsPass when this pass runs, after TrackPass; this pass writes Y and E of
+// every observation of a non-constant camera, the only ones PairsPass reads.  Keep that order: ObsPass, TrackPass, SlotsPass,
+// PairsPass.
 template <bool kDet>
 struct SlotsPass {             // one item per observation of the big landmarks
   VisualView vv; View bv; const double* params; double* obs; double* S; double* rhs; double* cam_colsq; double* cam_grad;
@@ -181,7 +194,7 @@ struct PairsPass {             // one item per ordered observation pair (x, y), 
     int64_t sx, sy;
     pair_obs(vv, bv, p, sx, sy);
     const int rx = vv.obs_row[sx], ry = vv.obs_row[sy];
-    if (!(ry >= 0 && rx >= ry)) return;
+    if (!(ry >= 0 && rx >= ry)) return;                  // both rows >= 0: SlotsPass wrote Y_x over ObsPass' rho (kObRho)
     const double* Yx = obs + kObs * (sx - base) + kObY;
     const double* Ey = obs + kObs * (sy - base) + kObE;
     double* B = kDet ? S + 36 * p : S + (bv.row_start[rx] + (ry - bv.first[rx])) * 36;
@@ -195,7 +208,7 @@ struct PairsPass {             // one item per ordered observation pair (x, y), 
 };
 
 // kDet = false: camera columns into cam_colsq by atomics; true: cam_colsq = the observations' records [n_obs][6]
-template <bool kDet>
+template <bool kDet, bool kLoss = false>
 struct ColObsPass {            // unscaled column norms, one item per observation: camera columns by atomics, point columns kept
   VisualView vv; View bv; VisualState st; double* obs; double* cam_colsq;
   LVBA_BHD void operator()(int64_t i) const {
@@ -205,6 +218,7 @@ struct ColObsPass {            // unscaled column norms, one item per observatio
     const double X[3] = {st.X[3 * tr], st.X[3 * tr + 1], st.X[3 * tr + 2]};
     ObsEval o;
     obs_eval<true>(vv, st.q + 4 * (int64_t)cam, st.t + 3 * (int64_t)cam, X, vv.obs_uv[s], o);
+    if constexpr (kLoss) obs_loss<true>(vv, o);
     double* sg = obs + kObs * i + kObStage;
     sg[0] = o.JX[0] * o.JX[0] + o.JX[3] * o.JX[3];
     sg[1] = o.JX[1] * o.JX[1] + o.JX[4] * o.JX[4];
@@ -218,6 +232,8 @@ struct ColObsPass {            // unscaled column norms, one item per observatio
   }
 };
 
+using ObsF = ObsPass<false>;
+using TrackF = TrackPass<false>;
 using SlotsF = SlotsPass<false>;
 using PairsF = PairsPass<false>;
 using ColObsF = ColObsPass<false>;
@@ -246,7 +262,8 @@ struct PairDstF {
   }
 };
 
-struct ColTrackF {             // one item per big landmark: its three point columns
+template <bool kLoss>
+struct ColTrackPass {          // one item per big landmark: its three point columns
   VisualView vv; View bv; VisualState st; const double* obs; double* pt_colsq;
   LVBA_BHD void operator()(int64_t b) const {
     const int64_t k = bv.t0 + b, base = vv.trk_ptr[bv.t0];
@@ -254,6 +271,7 @@ struct ColTrackF {             // one item per big landmark: its three point col
     const double X[3] = {st.X[3 * tr], st.X[3 * tr + 1], st.X[3 * tr + 2]};
     double rp, J[3];
     plane_eval(vv, vv.plane + 4 * k, X, rp, J);
+    if constexpr (kLoss) plane_loss(vv, rp, J);
     double a0 = J[0] * J[0], a1 = J[1] * J[1], a2 = J[2] * J[2];
     for (int64_t i = vv.trk_ptr[k] - base; i < vv.trk_ptr[k + 1] - base; ++i) {
       const double* sg = obs + kObs * i + kObStage;
@@ -264,8 +282,10 @@ struct ColTrackF {             // one item per big landmark: its three point col
   }
 };
 
-// one item per big landmark, after ObsF / TrackF at the same state and scale: out[4 b ..] = model-cost change, step^2, x^2, 0
-struct BacksubF {
+// one item per big landmark, after ObsPass / TrackPass at the same state and scale: out[4 b ..] = model-cost change, step^2,
+// x^2, 0
+template <bool kLoss>
+struct BacksubPass {
   VisualView vv; View bv; VisualState st; VisualLM lm; const double* obs; double* params; const double* y_cam;
   double* X_cand; double* pt_step; double* out;
   LVBA_BHD void operator()(int64_t b) const {
@@ -292,6 +312,7 @@ struct BacksubF {
     if (pt_step) { pt_step[3 * tr] = d[0]; pt_step[3 * tr + 1] = d[1]; pt_step[3 * tr + 2] = d[2]; }
     double rp, Jpl[3];
     plane_eval(vv, vv.plane + 4 * k, X, rp, Jpl);
+    if constexpr (kLoss) plane_loss(vv, rp, Jpl);
     const double jy = Jpl[0] * d[0] + Jpl[1] * d[1] + Jpl[2] * d[2];   // J~ y = J (s o y)
     double model = -jy * (rp + 0.5 * jy);
     for (int64_t i = lo; i < hi; ++i) {
@@ -317,7 +338,8 @@ struct BacksubF {
   }
 };
 
-struct CostF {                 // one item per big landmark: cost[b] = 1/2 (sum r^2 + r_p^2) at the state `st`
+template <bool kLoss>
+struct CostPass {              // one item per big landmark: cost[b] = 1/2 (sum r^2 + r_p^2) (kLoss: 1/2 sum rho) at the state `st`
   VisualView vv; View bv; VisualState st; double* cost;
   LVBA_BHD void operator()(int64_t b) const {
     const int64_t k = bv.t0 + b;
@@ -328,13 +350,19 @@ struct CostF {                 // one item per big landmark: cost[b] = 1/2 (sum 
       const int cam = vv.obs_cam[s];
       ObsEval o;
       obs_eval<false>(vv, st.q + 4 * (int64_t)cam, st.t + 3 * (int64_t)cam, X, vv.obs_uv[s], o);
-      c += o.r[0] * o.r[0] + o.r[1] * o.r[1];
+      if constexpr (kLoss) c += obs_loss<false>(vv, o);
+      else c += o.r[0] * o.r[0] + o.r[1] * o.r[1];
     }
     double rp, J[3];
     plane_eval(vv, vv.plane + 4 * k, X, rp, J);
-    cost[b] = 0.5 * (c + rp * rp);
+    if constexpr (kLoss) cost[b] = 0.5 * (c + plane_loss(vv, rp, J));
+    else cost[b] = 0.5 * (c + rp * rp);
   }
 };
+
+using ColTrackF = ColTrackPass<false>;
+using BacksubF = BacksubPass<false>;
+using CostF = CostPass<false>;
 
 }  // namespace vbig
 }  // namespace lvba

@@ -1,11 +1,12 @@
 // visual_math.h — path B arithmetic shared by the kernels of visual.cuh and the passes of visual_big.h: the reprojection and
-// point-to-plane residuals with their analytic Jacobians and the 3x3 landmark block inverse.  Compiled for the device and, for
+// point-to-plane residuals with their analytic Jacobians, the robust losses and the 3x3 landmark block inverse.  Compiled for the device and, for
 // the CPU tests of tests/emu/, for the host.
 //
 // Restates (analytic Jacobians instead of ceres::Jet auto-diff):
 //   ReprojErrorWhitenedDistorted::operator()   reference include/utils.hpp:61-111
 //   PointPlaneErrorWhitened::operator()        reference include/utils.hpp:133-139
 #pragma once
+#include <float.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -40,7 +41,12 @@ struct VisualView {
   const double* plane;       // [Tv*4]
   double intr[8];
   double inv_sigma_px, inv_sigma_pl;
+  int loss_px, loss_pl;      // robust loss (kLoss*) of the reprojection / plane blocks; read by the kLoss instantiations only
+  double loss_a_px, loss_a_pl;   // their scales
 };
+
+// lvba_loss_kind (include/lvba_b200.h)
+constexpr int kLossNone = 0, kLossHuber = 1, kLossCauchy = 2;
 
 struct VisualState {
   const double* q;   // [M*4]
@@ -154,6 +160,50 @@ LVBA_HD void plane_eval(const VisualView& vv, const double* pl, const double* X,
   r = root * vv.inv_sigma_pl;
   const double k = (e / root) * vv.inv_sigma_pl;
   J[0] = -k * pl[0]; J[1] = -k * pl[1]; J[2] = -k * pl[2];
+}
+
+// rho(s) and rho'(s) of a robust loss with scale a at the squared norm s of a residual block: ceres-solver 2.1.0 HuberLoss and
+// CauchyLoss (loss_function.cc), b = a^2.  Both have rho'' <= 0 everywhere, so Ceres' Corrector (corrector.cc) reduces to
+// scaling the residual and the Jacobian by sqrt(rho'); rho'' is never needed.  kLossNone: rho = s, rho' = 1.
+LVBA_HD void loss_eval(int kind, double a, double s, double& rho, double& rho1) {
+  const double b = a * a;
+  if (kind == kLossHuber && s > b) {
+    const double r = sqrt(s);
+    rho = 2.0 * a * r - b;
+    rho1 = fmax(DBL_MIN, a / r);
+  } else if (kind == kLossCauchy) {
+    const double c = 1.0 / b, u = 1.0 + s * c;
+    rho = b * log(u);
+    rho1 = fmax(DBL_MIN, 1.0 / u);
+  } else {
+    rho = s;
+    rho1 = 1.0;
+  }
+}
+
+// Corrector of one reprojection block: returns its cost term rho(|r|^2); with kCorrect, r, J_c and J_X times sqrt(rho')
+template <bool kCorrect>
+LVBA_HD double obs_loss(const VisualView& vv, ObsEval& o) {
+  double rho, rho1;
+  loss_eval(vv.loss_px, vv.loss_a_px, o.r[0] * o.r[0] + o.r[1] * o.r[1], rho, rho1);
+  if (kCorrect) {
+    const double w = sqrt(rho1);
+    o.r[0] *= w; o.r[1] *= w;
+LVBA_UNROLL
+    for (int i = 0; i < 12; ++i) o.Jc[i] *= w;
+LVBA_UNROLL
+    for (int i = 0; i < 6; ++i) o.JX[i] *= w;
+  }
+  return rho;
+}
+
+// Corrector of one plane block (r, J of plane_eval): returns rho(r^2); r and J times sqrt(rho')
+LVBA_HD double plane_loss(const VisualView& vv, double& r, double J[3]) {
+  double rho, rho1;
+  loss_eval(vv.loss_pl, vv.loss_a_pl, r * r, rho, rho1);
+  const double w = sqrt(rho1);
+  r *= w; J[0] *= w; J[1] *= w; J[2] *= w;
+  return rho;
 }
 
 LVBA_HD void sym3_inverse(const double* c /*xx xy xz yy yz zz*/, double* o) {

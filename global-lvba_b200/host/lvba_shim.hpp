@@ -453,6 +453,9 @@ class DepthRenderer {
 //      observation list it walks at :1614-1631.  obs_of_point[pi] = list of (cam_id, u, v).
 struct Observation { int cam; float u, v; };
 
+// opts: null = lvba_visual_default_opts, plain least squares as the reference's nullptr losses (:1630, :1639).  Its
+// loss_function_reproj / loss_function_plane (HuberLoss(1.0) / HuberLoss(0.1), :1585-1586) map to reproj_loss = plane_loss =
+// LVBA_LOSS_HUBER with the default scales 1.0 / 0.1 (INTEGRATION.md, B2).
 inline int solve_visual(std::vector<std::array<double, 4>>& qs, std::vector<std::array<double, 3>>& ts,
                         std::vector<std::array<double, 3>>& Xs, const std::vector<std::array<double, 3>>& plane_n,
                         const std::vector<double>& plane_d, const std::vector<std::vector<Observation>>& obs_of_point,

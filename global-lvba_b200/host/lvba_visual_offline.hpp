@@ -21,6 +21,7 @@
 #include <cmath>
 #include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <filesystem>
 #include <fstream>
 #include <map>
@@ -63,6 +64,32 @@ struct Config {
     scaled = true;
   }
 };
+
+// A robust loss of the visual stage as `KIND[:A]`, KIND none|huber|cauchy (lvba_loss_kind), A a finite number > 0 (default
+// `default_scale`).  Anything else is refused with a message in *err; kind / scale are then untouched.
+inline bool parse_loss(const char* text, double default_scale, int32_t& kind, double& scale, std::string* err = nullptr) {
+  const std::string s = text ? text : "";
+  const size_t colon = s.find(':');
+  const std::string name = s.substr(0, colon);
+  int32_t k;
+  if (name == "none") k = LVBA_LOSS_NONE;
+  else if (name == "huber") k = LVBA_LOSS_HUBER;
+  else if (name == "cauchy") k = LVBA_LOSS_CAUCHY;
+  else { if (err) *err = "'" + s + "': the kind must be none, huber or cauchy"; return false; }
+  double a = default_scale;
+  if (colon != std::string::npos) {
+    const std::string num = s.substr(colon + 1);
+    char* end = nullptr;
+    a = num.empty() ? 0.0 : std::strtod(num.c_str(), &end);
+    if (num.empty() || *end != '\0' || !std::isfinite(a) || !(a > 0.0)) {
+      if (err) *err = "'" + s + "': the scale after ':' must be a finite number > 0";
+      return false;
+    }
+  }
+  kind = k;
+  scale = a;
+  return true;
+}
 
 // The subset of YAML the reference's config files use: `section:` lines, `  key: value` lines, flow lists that may run over
 // several lines, `#` comments, quoted strings.  Returns "section/key" -> raw value text (lists without the brackets).
@@ -392,13 +419,50 @@ struct VisualResult {
   int anchors = 0;
 };
 
+// The visual problem of one solve_visual call in a file, to re-run or inspect the solve elsewhere.  Native byte order:
+//   char[8] "LVBAVP01"; int64 M, T, nnz; double intr[8], sigma_px, sigma_plane;
+//   the state before the solve: double q[M*4] (w x y z), t[M*3], X[T*3]; double plane_nd[T*4]; int64 obs_ptr[T+1];
+//   int32 obs_cam[nnz]; float obs_uv[nnz*2]; the state after the solve: double q[M*4], t[M*3], X[T*3]
+// (the arguments of lvba_visual_lm, fixed_cam = 0).
+inline bool write_visual_problem(const std::string& path, const std::vector<std::array<double, 4>>& q0,
+                                 const std::vector<std::array<double, 3>>& t0, const std::vector<std::array<double, 3>>& X0,
+                                 const std::vector<std::array<double, 3>>& plane_n, const std::vector<double>& plane_d,
+                                 const std::vector<std::vector<Observation>>& obs, const double intr[8], double sigma_px,
+                                 double sigma_plane, const std::vector<std::array<double, 4>>& q1,
+                                 const std::vector<std::array<double, 3>>& t1, const std::vector<std::array<double, 3>>& X1) {
+  std::ofstream f(path, std::ios::binary);
+  if (!f) return false;
+  auto put = [&](const void* p, size_t n) { if (n) f.write(static_cast<const char*>(p), (std::streamsize)n); };
+  const int64_t M = (int64_t)q0.size(), T = (int64_t)X0.size();
+  std::vector<int64_t> obs_ptr((size_t)T + 1, 0);
+  std::vector<int32_t> obs_cam;
+  std::vector<float> obs_uv;
+  std::vector<double> plane_nd((size_t)T * 4);
+  for (int64_t i = 0; i < T; ++i) {
+    for (const auto& o : obs[(size_t)i]) { obs_cam.push_back(o.cam); obs_uv.push_back(o.u); obs_uv.push_back(o.v); }
+    obs_ptr[(size_t)i + 1] = (int64_t)obs_cam.size();
+    for (int k = 0; k < 3; ++k) plane_nd[4 * (size_t)i + k] = plane_n[(size_t)i][(size_t)k];
+    plane_nd[4 * (size_t)i + 3] = plane_d[(size_t)i];
+  }
+  const int64_t nnz = (int64_t)obs_cam.size();
+  const double sig[2] = {sigma_px, sigma_plane};
+  put("LVBAVP01", 8); put(&M, 8); put(&T, 8); put(&nnz, 8); put(intr, 64); put(sig, 16);
+  put(q0.data(), (size_t)M * 32); put(t0.data(), (size_t)M * 24); put(X0.data(), (size_t)T * 24);
+  put(plane_nd.data(), plane_nd.size() * 8); put(obs_ptr.data(), obs_ptr.size() * 8);
+  put(obs_cam.data(), obs_cam.size() * 4); put(obs_uv.data(), obs_uv.size() * 4);
+  put(q1.data(), (size_t)M * 32); put(t1.data(), (size_t)M * 24); put(X1.data(), (size_t)T * 24);
+  return (bool)f;
+}
+
 // runVisualBAWithLidarAssist (:144-154) minus the drawing / publishing calls.  x_buf_opt / x_buf_before: the LiDAR poses after
 // and before runLidarBA (equal when it was disabled); eigen_in_force: the eigen-ratio array the last set_eigen_ratio_array call
 // left behind (stage 2's after runLidarBA, bavoxel.hpp:17 otherwise).  opts: the visual LM's options (null: the defaults).
+// problem_path: when not empty, the problem of the solve and its result go there (write_visual_problem).
 inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls, const std::vector<Pose>& x_buf_opt,
                          const std::vector<Pose>& x_buf_before, const std::vector<double>& images_ids, const std::vector<Pose>& image_poses,
                          const KeypointImages& all_keypoints, const MatchTable& all_matches, const float eigen_in_force[4],
-                         VisualResult& res, std::string* err = nullptr, const lvba_visual_opts* opts = nullptr) {
+                         VisualResult& res, std::string* err = nullptr, const lvba_visual_opts* opts = nullptr,
+                         const std::string& problem_path = std::string()) {
   const int M = (int)images_ids.size();
   if ((int)image_poses.size() != M) { if (err) *err = "Number of images and poses do not match"; return LVBA_ERR_INVALID_ARG; }      // :458-461
   if ((int)all_keypoints.size() != M) { if (err) *err = "all_keypoints.size() must equal #cameras"; return LVBA_ERR_INVALID_ARG; }  // :1429
@@ -518,8 +582,17 @@ inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls,
       obs[(size_t)pi].push_back({cam, all_keypoints[(size_t)cam][(size_t)kp].x, all_keypoints[(size_t)cam][(size_t)kp].y});
     }
   }
+  const std::vector<std::array<double, 4>> qs0 = qs;
+  const std::vector<std::array<double, 3>> ts0 = ts, Xs0 = Xs;
   rc = solve_visual(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01, opts, &res.solve);
   if (rc != LVBA_OK) { if (err) *err = std::string("visual LM: ") + lvba_last_error(); return rc; }
+  if (!problem_path.empty()) {
+    const double intr[8] = {cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3};
+    if (!write_visual_problem(problem_path, qs0, ts0, Xs0, plane_n, plane_d, obs, intr, 0.5, 0.01, qs, ts, Xs)) {
+      if (err) *err = "cannot write " + problem_path;
+      return LVBA_ERR_INVALID_ARG;
+    }
+  }
   if (res.solve.termination == LVBA_TERM_INVALID_STEPS) return LVBA_OK;                                // ceres::FAILURE, :1647-1650: nothing written back
   for (int k = 0; k < M; ++k) {                                                                       // :1652-1656
     const auto& q = qs[(size_t)k];

@@ -55,6 +55,21 @@ typedef struct lvba_lidar_opts {
                           * active communicator (lvba_comm_init) the call returns LVBA_ERR_UNSUPPORTED. */
 } lvba_lidar_opts;
 
+/* ---- path B robust losses: the ceres::LossFunction of a residual block (src/lvba_system.cpp:1585-1586, :1630, :1639).
+ *      A block with squared whitened norm s = |r|^2 (the 2-vector of a reprojection, r_p^2 of a plane) costs 1/2 rho(s);
+ *      with scale a, b = a^2:
+ *        LVBA_LOSS_HUBER   s <= b: rho = s;  else rho = 2 a sqrt(s) - b, rho' = max(DBL_MIN, a / sqrt(s))   (ceres::HuberLoss)
+ *        LVBA_LOSS_CAUCHY  rho = b log(1 + s / b), rho' = max(DBL_MIN, 1 / (1 + s / b))                    (ceres::CauchyLoss)
+ *      Both have rho'' <= 0 everywhere, so Ceres' Corrector only scales the residual and the Jacobian by sqrt(rho') (no
+ *      second-order term); losses whose rho'' can be positive are not offered.  The loss acts on the whitened residual:
+ *      Huber 1.0 on the reprojection is 1 sigma_px, Huber 0.1 on the plane is 0.1 sigma_plane.  The loss is applied per
+ *      residual block, before any sum; it has not been run on more than one GPU. */
+typedef enum lvba_loss_kind {
+  LVBA_LOSS_NONE = 0,
+  LVBA_LOSS_HUBER = 1,
+  LVBA_LOSS_CAUCHY = 2
+} lvba_loss_kind;
+
 /* ---- path B options: the ceres::Solver::Options in force at src/lvba_system.cpp:1572-1576
  *      (ceres-solver 2.1.0 defaults everywhere else, SURVEY.md Q10) */
 typedef struct lvba_visual_opts {
@@ -75,6 +90,14 @@ typedef struct lvba_visual_opts {
                                   * same bits on every run on one GPU model and library build, memory allocated when a
                                   * call or lvba_visual_reset_lm first asks for it, LVBA_ERR_UNSUPPORTED with an active
                                   * communicator) */
+  /* Robust losses (lvba_loss_kind), as `deterministic`: the one-shot call takes them from its opts, a handle from
+   * lvba_visual_reset_lm (lvba_visual_cost / lvba_visual_step then follow the handle; a new handle has none).  An unknown
+   * kind, or a kind other than LVBA_LOSS_NONE whose scale is not finite and > 0, is LVBA_ERR_INVALID_ARG before any
+   * device work.  The default scales are the reference's HuberLoss(1.0) / HuberLoss(0.1) (src/lvba_system.cpp:1585-1586). */
+  int32_t reproj_loss;           /* LVBA_LOSS_NONE (loss_function = nullptr, :1630) */
+  double reproj_loss_scale;      /* 1.0 */
+  int32_t plane_loss;            /* LVBA_LOSS_NONE (:1639) */
+  double plane_loss_scale;       /* 0.1 */
 } lvba_visual_opts;
 
 typedef enum lvba_termination {
@@ -92,7 +115,8 @@ typedef struct lvba_summary {
   int32_t accepted;          /* accepted steps */
   int32_t hessian_builds;    /* passes that rebuilt H/g (A) or J/S (B) */
   int32_t termination;       /* lvba_termination */
-  double cost_first;         /* A: sum(lambda0)/V at entry ; B: 1/2 sum r^2 at entry */
+  double cost_first;         /* A: sum(lambda0)/V at entry ; B: 1/2 sum rho(|r|^2) over the residual blocks at entry
+                              *    (rho(s) = s without a loss: 1/2 sum r^2) */
   double cost_last;          /* same quantity at the returned state */
   double damping_last;       /* A: u ; B: trust-region radius */
   double ms_total;           /* wall time inside the call (host clock) */
@@ -206,7 +230,8 @@ int lvba_visual_create(int32_t M, int64_t T, const double* q_wxyz, const double*
 int lvba_visual_destroy(lvba_visual_problem* p);
 int lvba_visual_set_state(lvba_visual_problem* p, const double* q_wxyz, const double* t, const double* X);
 int lvba_visual_get_state(lvba_visual_problem* p, double* q_wxyz, double* t, double* X);
-/* 1/2 sum r^2 over all residual blocks at the current device state */
+/* 1/2 sum rho(|r|^2) over all residual blocks at the current device state, with the losses of the last
+ * lvba_visual_reset_lm (1/2 sum r^2 without) */
 int lvba_visual_cost(lvba_visual_problem* p, double* cost);
 /* One linearisation + Schur elimination + reduced solve + back-substitution at the current state
  * with the given trust-region radius; writes the (unscaled) tangent step: cam_step [M*6] (zeros for

@@ -29,6 +29,11 @@
 //   --deterministic   every LM solve (window stage, both global LiDAR stages, the visual stage) in the deterministic mode of
 //                lvba_lidar_opts / lvba_visual_opts: the same dataset gives a byte-identical trajectory, images.txt and points3D.txt on
 //                every run on one GPU model.
+//   --reproj-loss KIND[:A]   --plane-loss KIND[:A]   robust loss of the visual stage's reprojection / plane residuals
+//                (lvba_visual_opts::reproj_loss / plane_loss), KIND none|huber|cauchy; A defaults to the reference's 1.0 / 0.1
+//                (HuberLoss, src/lvba_system.cpp:1585-1586).  The reference passes no loss (:1630, :1639): the default is none.
+//   --visual-problem F   write the visual stage's problem, its state before and after the solve, to F
+//                (lvba_visual_offline.hpp write_visual_problem), to re-run or inspect that solve elsewhere
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -51,8 +56,10 @@ int main(int argc, char** argv) {
   int fuse_order = LVBA_FUSE_ORDER_LIBSTDCXX;         // the library's default: what a g++ build of the reference does
   int window = 0;
   double anchor_leaf = 0.1;
-  std::string db_path, sparse_dir, lidar_opt;
+  std::string db_path, sparse_dir, lidar_opt, visual_problem;
   lvba_b200::offline::Config cfg;
+  lvba_visual_opts visual_opts;
+  lvba_visual_default_opts(&visual_opts);
   for (int i = 1; i < argc; ++i) {
     const std::string a = argv[i];
     auto next = [&]() -> const char* { if (i + 1 >= argc) { std::fprintf(stderr, "missing value after %s\n", a.c_str()); std::exit(64); } return argv[++i]; };
@@ -75,6 +82,16 @@ int main(int argc, char** argv) {
     else if (a == "--db") db_path = next();
     else if (a == "--lidar-opt") lidar_opt = next();
     else if (a == "--sparse-dir") sparse_dir = next();
+    else if (a == "--visual-problem") visual_problem = next();
+    else if (a == "--reproj-loss" || a == "--plane-loss") {
+      const bool reproj = a == "--reproj-loss";
+      std::string e;
+      if (!lvba_b200::offline::parse_loss(next(), reproj ? 1.0 : 0.1, reproj ? visual_opts.reproj_loss : visual_opts.plane_loss,
+                                          reproj ? visual_opts.reproj_loss_scale : visual_opts.plane_loss_scale, &e)) {
+        std::fprintf(stderr, "%s: %s\n", a.c_str(), e.c_str());
+        return 64;
+      }
+    }
     else if (a == "--config") {
       std::string e;
       if (!lvba_b200::offline::load_config(next(), cfg, &e)) { std::fprintf(stderr, "config: %s\n", e.c_str()); return 64; }
@@ -92,8 +109,6 @@ int main(int argc, char** argv) {
   lvba_lidar_opts lidar_opts;
   lvba_lidar_default_opts(&lidar_opts);
   lidar_opts.deterministic = deterministic ? 1 : 0;
-  lvba_visual_opts visual_opts;
-  lvba_visual_default_opts(&visual_opts);
   visual_opts.deterministic = deterministic ? 1 : 0;
   if (data.back() != '/') data += '/';
   LidarDataset ds;
@@ -219,7 +234,7 @@ int main(int argc, char** argv) {
   off::VisualResult vr;
   cfg.fuse_map_order = fuse_order;
   const int vrc = off::run_visual_ba(cfg, frame_clouds, frames, frames_before, images_ids, image_poses, keypoints, matches,
-                                     lidar ? eigen[1] : default_eigen, vr, &err, &visual_opts);
+                                     lidar ? eigen[1] : default_eigen, vr, &err, &visual_opts, visual_problem);
   if (vrc != LVBA_OK) { std::fprintf(stderr, "visual stage failed (%d): %s\n", vrc, err.c_str()); return vrc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
   std::printf("{\"stage\": \"visual\", \"images\": %zu, \"keypoints\": %lld, \"matches\": %lld, \"depth_valid\": %lld, \"components\": %lld, \"tracks\": %lld, "
               "\"usable_tracks\": %lld, \"anchors\": %d, \"anchor_points\": %lld, \"surf_voxels\": %lld, \"points_kept\": %lld, \"iterations\": %d, "
