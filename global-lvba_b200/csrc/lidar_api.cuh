@@ -5,6 +5,7 @@
 #include <unordered_set>
 
 #include "runtime.cuh"   // (pulls comm.cuh in)
+#include "balm_rule.h"
 #include "exec.cuh"
 #include "lidar.cuh"
 #include "lidar_big.h"
@@ -110,12 +111,11 @@ struct lvba_lidar_problem {
   double* h_scal = nullptr;       // pinned: [0] r1 sum, [1] q1, [2] dx non-finite flag, [3] r2 sum, [4] factor status
   int64_t launches = 0, h2d = 0, d2h = 0;
   double ms_setup = 0.0;
-  // LM state (bavoxel.hpp:664-671)
+  // LM state
   lvba_lidar_opts opts;
-  double u = 0.01, v = 2.0, residual1 = 0.0;
-  bool is_calc_hess = true, have_first = false, converged = false;
-  double cost_first = 0.0, cost_last = 0.0;
-  int iters = 0, accepted = 0, builds = 0, termination = LVBA_TERM_MAX_ITER;
+  lvba::BalmState lm;
+  bool is_calc_hess = true;
+  int builds = 0;
   // ---- batched window BA: n_groups independent windows in one block-diagonal system
   int n_groups = 0;
   std::vector<int> grp_ptr;            // [G+1] pose offsets
@@ -502,11 +502,7 @@ inline int lidar_set_mode(lvba_lidar_problem* P, const lvba_lidar_opts& o) {
 inline int lidar_big_passes(lvba_lidar_problem* P, const double* d_poses, bool residual_only, int n_before) {
   cudaStream_t s = P->stream;
   const big::View bv = P->big_view();
-  auto launch = [&](int64_t items, const auto& f) {
-    const int grid = (int)std::min<int64_t>((items + 127) / 128, kNumSMs * 16);
-    env_wide_pass_kernel<<<grid, 128, 0, s>>>(items, f);
-    ++P->launches;
-  };
+  auto launch = [&](int64_t items, const auto& f) { wide_pass(s, items, f, &P->launches); };
   launch((int64_t)P->n_big, big::ParamsF{bv, d_poses, P->big_params.p, P->batch_res.p + n_before});
   if (!residual_only && P->det) {
     const int64_t h0 = P->prun.n_runs + P->drun.n_runs, g0 = P->drun.n_runs;
@@ -613,8 +609,9 @@ inline int lidar_iterate_impl(lvba_lidar_problem* P, int n_iter, lvba_summary* s
   const double t0 = wall_ms();
   const int64_t l0 = P->launches, h0 = P->h2d, d0 = P->d2h;
   const double V = (double)P->V_total;
-  const int iters0 = P->iters, acc0 = P->accepted, builds0 = P->builds;
-  for (int it = 0; it < n_iter && !P->converged; ++it) {
+  BalmState& lm = P->lm;
+  const int iters0 = lm.iters, acc0 = lm.accepted, builds0 = P->builds;
+  for (int it = 0; it < n_iter && !lm.converged; ++it) {
     if (P->is_calc_hess) {                                   // divide_thread, :688-689
       P->timers.begin(PH_BUILD);
       LVBA_TRY(lidar_build_dev(P, P->poses.p, 0));
@@ -622,7 +619,7 @@ inline int lidar_iterate_impl(lvba_lidar_problem* P, int n_iter, lvba_summary* s
       ++P->builds;
     }
     P->timers.begin(PH_SOLVE);
-    LVBA_TRY(lidar_solve_dev(P, P->u));                      // :692-710, :729
+    LVBA_TRY(lidar_solve_dev(P, lm.u));                      // :692-710, :729
     P->timers.end();
     P->timers.begin(PH_RESID);
     lidar_retract_kernel<<<(P->W + 127) / 128, 128, 0, P->stream>>>(P->W, P->poses.p, P->dx.p, P->trial.p);   // :722-727
@@ -630,46 +627,16 @@ inline int lidar_iterate_impl(lvba_lidar_problem* P, int n_iter, lvba_summary* s
     LVBA_TRY(lidar_residual_dev(P, P->trial.p, 3));          // only_residual, :731
     P->timers.end();
     LVBA_TRY(lidar_fetch_scal(P));
-    if (P->is_calc_hess) P->residual1 = P->h_scal[0] / V;    // AVG_THR, :635
-    if (!P->have_first) { P->cost_first = P->residual1; P->cost_last = P->residual1; P->have_first = true; }
-    const double q1 = P->h_scal[1] / V;                      // :732
-    double residual2 = P->h_scal[3] / V;
-    const bool bad = P->h_scal[2] != 0.0 || !std::isfinite(residual2) || !std::isfinite(q1);
-    if (bad) residual2 = NAN;
-    double q = P->residual1 - residual2;
-    ++P->iters;
-    if (P->opts.verbose)
-      fprintf(stderr, "[lvba lidar] iter %d: (%.9g %.9g) u: %g v: %g q: %g q1: %g\n", P->iters - 1, P->residual1, residual2, P->u, P->v, q, q1);
-    if (q > 0) {                                             // :744-752
-      std::swap(P->poses.p, P->trial.p);
-      q = q / q1;
-      P->v = 2;
-      q = 1 - std::pow(2 * q - 1, 3);
-      P->u *= (q < (1.0 / 3.0) ? (1.0 / 3.0) : q);
-      P->is_calc_hess = true;
-      ++P->accepted;
-      P->cost_last = residual2;
-    } else {                                                 // :753-758
-      P->u = P->u * P->v;
-      P->v = 2 * P->v;
-      P->is_calc_hess = false;
-    }
-    if (P->opts.rel_tol >= 0 && std::fabs(P->residual1 - residual2) / P->residual1 < P->opts.rel_tol) {   // :760
-      P->converged = true;
-      P->termination = LVBA_TERM_FUNCTION_TOL;
-    }
+    // residual1 is refreshed after a build only; an accepted step rebuilds H at the new poses (:744-758)
+    P->is_calc_hess = balm_step(lm, P->h_scal, V, P->is_calc_hess, P->opts, "lvba lidar");
+    if (P->is_calc_hess) std::swap(P->poses.p, P->trial.p);
   }
   if (sum) {
-    memset(sum, 0, sizeof *sum);
     LVBA_CUDA(cudaStreamSynchronize(P->stream));
     double ms[PH_COUNT] = {0, 0, 0};
     P->timers.collect(ms);
-    sum->iterations = P->iters - iters0; sum->accepted = P->accepted - acc0; sum->hessian_builds = P->builds - builds0;
-    sum->termination = P->termination;
-    sum->cost_first = P->cost_first; sum->cost_last = P->cost_last; sum->damping_last = P->u;
-    sum->ms_total = wall_ms() - t0; sum->ms_setup = 0.0;
-    sum->ms_build = ms[PH_BUILD]; sum->ms_solve = ms[PH_SOLVE]; sum->ms_residual = ms[PH_RESID];
-    sum->kernel_launches = P->launches - l0; sum->h2d_bytes = P->h2d - h0; sum->d2h_bytes = P->d2h - d0;
+    write_summary(sum, lm.iters - iters0, lm.accepted - acc0, P->builds - builds0, lm.term, lm.cost_first, lm.cost_last, lm.u, ms,
+                  wall_ms() - t0, P->launches - l0, P->h2d - h0, P->d2h - d0);
   }
   return LVBA_OK;
 }
@@ -683,7 +650,7 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
   const double t0 = wall_ms();
   const int G = P->n_groups;
   cudaStream_t s = P->stream;
-  struct WinState { double u, v, residual1, cost_first, cost_last; bool active, converged, have_first, skipped; int iters, accepted, term; };
+  struct WinState : BalmState { bool active = false, skipped = false; };
   std::vector<WinState> ws((size_t)G);
   std::vector<double> u_host((size_t)G);
   std::vector<int> acc_host((size_t)G);
@@ -691,8 +658,7 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
   for (int g = 0; g < G; ++g) {
     const int Wg = P->grp_ptr[g + 1] - P->grp_ptr[g];
     WinState& w = ws[g];
-    w.u = P->opts.u0; w.v = P->opts.v0; w.residual1 = 0; w.cost_first = w.cost_last = 0;
-    w.converged = false; w.have_first = false; w.iters = w.accepted = 0; w.term = LVBA_TERM_MAX_ITER;
+    w.reset(P->opts);
     w.skipped = Wg <= 0 || P->grp_V[g] == 0 || P->grp_V[g] < (long long)min_voxels_per_pose * Wg;   // src/lvba_system.cpp:262-266
     w.active = !w.skipped;
     if (w.skipped) w.term = LVBA_TERM_SKIPPED;
@@ -741,33 +707,10 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
       WinState& w = ws[g];
       acc_host[g] = 0;
       if (!w.active) continue;
-      const double Vg = (double)P->grp_V[g];
-      const double* sc = P->h_grp_scal + 4 * g;
-      w.residual1 = sc[0] / Vg;                                // AVG_THR, :635
-      if (!w.have_first) { w.cost_first = w.cost_last = w.residual1; w.have_first = true; }
-      const double q1 = sc[1] / Vg;                            // :732
-      double residual2 = sc[3] / Vg;
-      const bool bad = sc[2] != 0.0 || !std::isfinite(residual2) || !std::isfinite(q1);
-      if (bad) residual2 = NAN;
-      double q = w.residual1 - residual2;
-      ++w.iters;
-      if (P->opts.verbose)
-        fprintf(stderr, "[lvba window %d] iter %d: (%.9g %.9g) u: %g v: %g q: %g q1: %g\n", g, w.iters - 1, w.residual1, residual2, w.u, w.v, q, q1);
-      if (q > 0) {                                             // :744-752
-        acc_host[g] = 1;
-        q = q / q1;
-        w.v = 2;
-        q = 1 - std::pow(2 * q - 1, 3);
-        w.u *= (q < (1.0 / 3.0) ? (1.0 / 3.0) : q);
-        ++w.accepted;
-        w.cost_last = residual2;
-      } else {                                                 // :753-758
-        w.u = w.u * w.v;
-        w.v = 2 * w.v;
-      }
-      if (P->opts.rel_tol >= 0 && std::fabs(w.residual1 - residual2) / w.residual1 < P->opts.rel_tol) {   // :760
-        w.converged = true; w.active = false; w.term = LVBA_TERM_FUNCTION_TOL; --n_active;
-      }
+      char label[32] = "";
+      if (P->opts.verbose) snprintf(label, sizeof label, "lvba window %d", g);
+      acc_host[g] = balm_step(w, P->h_grp_scal + 4 * g, (double)P->grp_V[g], /*rebuilt=*/true, P->opts, label);
+      if (w.converged) { w.active = false; --n_active; }
     }
     LVBA_CUDA(cudaMemcpyAsync(P->d_accept.p, acc_host.data(), (size_t)G * sizeof(int), cudaMemcpyHostToDevice, s));
     P->h2d += (int64_t)G * 4;
@@ -777,20 +720,35 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
   }
   double ms[PH_COUNT] = {0, 0, 0};
   P->timers.collect(ms);
-  if (sums)
-    for (int g = 0; g < G; ++g) {
-      lvba_summary& o = sums[g];
-      memset(&o, 0, sizeof o);
-      o.iterations = ws[g].iters; o.accepted = ws[g].accepted; o.hessian_builds = ws[g].iters; o.termination = ws[g].term;
-      o.cost_first = ws[g].cost_first; o.cost_last = ws[g].cost_last; o.damping_last = ws[g].u;
-    }
-  if (total) {
-    memset(total, 0, sizeof *total);
-    total->iterations = passes; total->hessian_builds = passes;
-    for (int g = 0; g < G; ++g) total->accepted += ws[g].accepted;
-    total->ms_total = wall_ms() - t0; total->ms_build = ms[PH_BUILD]; total->ms_solve = ms[PH_SOLVE]; total->ms_residual = ms[PH_RESID];
+  int accepted = 0;
+  for (int g = 0; g < G; ++g) {
+    const WinState& w = ws[g];
+    if (sums) write_summary(&sums[g], w.iters, w.accepted, w.iters, w.term, w.cost_first, w.cost_last, w.u);
+    accepted += w.accepted;
   }
+  if (total) write_summary(total, passes, accepted, passes, /*term=*/0, 0.0, 0.0, 0.0, ms, wall_ms() - t0);
   return LVBA_OK;
+}
+
+// The rest of lvba_lidar_lm_batch and lvba_voxel_map_lidar_lm_batch once the call has created its batched handle p (`name`
+// in the error message): every window's LM, the poses written back and the totals in *total on success; p destroyed.
+inline int lidar_batch_one_shot(lvba_lidar_problem* p, const lvba_lidar_opts& o, int min_voxels_per_pose, double* poses,
+                                lvba_summary* summaries, lvba_summary* total, double t0, const char* name) {
+  p->opts = o;
+  lvba_summary tot;
+  memset(&tot, 0, sizeof tot);
+  int rc = lidar_set_mode(p, o);
+  if (rc == LVBA_OK) {
+    try { rc = lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
+    catch (...) { rc = fail(LVBA_ERR_NOMEM, "host allocation failed in %s", name); }
+  }
+  if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);     // written back only on success; skipped windows are unchanged on the device
+  if (rc == LVBA_OK && total) {
+    *total = tot;
+    one_shot_totals(total, p, t0);
+  }
+  lvba_lidar_destroy(p);
+  return rc;
 }
 
 }  // namespace lvba
@@ -895,8 +853,9 @@ int lvba_lidar_reset_lm(lvba_lidar_problem* p, const lvba_lidar_opts* opts) LVBA
   if (opts) o = *opts; else lvba_lidar_default_opts(&o);
   LVBA_TRY(lvba::lidar_set_mode(p, o));
   p->opts = o;
-  p->u = p->opts.u0; p->v = p->opts.v0; p->is_calc_hess = true; p->have_first = false; p->converged = false;
-  p->iters = p->accepted = p->builds = 0; p->termination = LVBA_TERM_MAX_ITER; p->residual1 = 0.0;
+  p->lm.reset(o);
+  p->is_calc_hess = true;
+  p->builds = 0;
   return LVBA_OK;
 } LVBA_ABI_END("lvba_lidar_reset_lm")
 
@@ -945,19 +904,8 @@ int lvba_lidar_lm(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* p
   catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
   catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_lidar_lm"); }
   if (rc != LVBA_OK) return rc;
-  lvba_summary s;
-  memset(&s, 0, sizeof s);
-  rc = lvba_lidar_reset_lm(p, &o);
-  if (rc == LVBA_OK && V > 0) rc = lvba_lidar_iterate(p, o.max_iter, &s);
-  if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);     // x_stats written back only on success
-  if (rc == LVBA_OK && summary) {
-    *summary = s;
-    summary->ms_setup = p->ms_setup;
-    summary->kernel_launches = p->launches; summary->h2d_bytes = p->h2d; summary->d2h_bytes = p->d2h;
-    summary->ms_total = lvba::wall_ms() - t0;
-  }
-  lvba_lidar_destroy(p);
-  return rc;
+  return lvba::lm_one_shot(p, o, V > 0, lvba_lidar_reset_lm, lvba_lidar_iterate, lvba_lidar_destroy,
+                           [&] { return lvba_lidar_get_poses(p, poses); }, t0, summary);     // x_stats written back only on success
 }
 
 int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
@@ -977,23 +925,7 @@ int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, co
   catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
   catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_lidar_lm_batch"); }
   if (rc != LVBA_OK) return rc;
-  p->opts = o;
-  lvba_summary tot;
-  memset(&tot, 0, sizeof tot);
-  rc = lvba::lidar_set_mode(p, o);
-  if (rc == LVBA_OK) {
-    try { rc = lvba::lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
-    catch (...) { rc = lvba::fail(LVBA_ERR_NOMEM, "host allocation failed in lvba_lidar_lm_batch"); }
-  }
-  if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);     // written back only on success; skipped windows are unchanged on the device
-  if (rc == LVBA_OK && total) {
-    *total = tot;
-    total->ms_setup = p->ms_setup;
-    total->kernel_launches = p->launches; total->h2d_bytes = p->h2d; total->d2h_bytes = p->d2h;
-    total->ms_total = lvba::wall_ms() - t0;
-  }
-  lvba_lidar_destroy(p);
-  return rc;
+  return lvba::lidar_batch_one_shot(p, o, min_voxels_per_pose, poses, summaries, total, t0, "lvba_lidar_lm_batch");
 }
 
 }  // extern "C"

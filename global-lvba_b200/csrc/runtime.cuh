@@ -27,6 +27,14 @@ template <class F>
 __global__ void __launch_bounds__(128) env_wide_pass_kernel(int64_t n, F f) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) f(i);
 }
+// one such pass over `items` items on `s`, counted in *launches (nothing to launch for no items)
+template <class F>
+inline void wide_pass(cudaStream_t s, int64_t items, const F& f, int64_t* launches) {
+  if (items <= 0) return;
+  const int grid = (int)std::min<int64_t>((items + 127) / 128, kNumSMs * 16);
+  env_wide_pass_kernel<<<grid, 128, 0, s>>>(items, f);
+  ++*launches;
+}
 
 // ---------------------------------------------------------------- errors
 inline std::string& last_error_ref() {
@@ -252,6 +260,47 @@ struct StreamDrain {
 inline double wall_ms() {
   using namespace std::chrono;
   return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
+}
+
+// ---------------------------------------------------------------- LM summaries and the one-shot calls
+// *s from the LM counts, costs and damping of a call; with `ms` (collected PhaseTimers) also its phase times, wall time
+// and the launches and bytes it moved
+inline void write_summary(lvba_summary* s, int iters, int accepted, int builds, int term, double cost_first, double cost_last,
+                          double damping, const double* ms = nullptr, double ms_total = 0.0, int64_t launches = 0, int64_t h2d = 0,
+                          int64_t d2h = 0) {
+  memset(s, 0, sizeof *s);
+  s->iterations = iters; s->accepted = accepted; s->hessian_builds = builds; s->termination = term;
+  s->cost_first = cost_first; s->cost_last = cost_last; s->damping_last = damping;
+  if (ms) { s->ms_build = ms[PH_BUILD]; s->ms_solve = ms[PH_SOLVE]; s->ms_residual = ms[PH_RESID]; }
+  s->ms_total = ms_total;
+  s->kernel_launches = launches; s->h2d_bytes = h2d; s->d2h_bytes = d2h;
+}
+
+// the summary of a one-shot call: the handle's set-up time and everything it launched and moved, the call's wall time from t0
+template <class Problem>
+inline void one_shot_totals(lvba_summary* s, const Problem* p, double t0) {
+  s->ms_setup = p->ms_setup;
+  s->kernel_launches = p->launches; s->h2d_bytes = p->h2d; s->d2h_bytes = p->d2h;
+  s->ms_total = wall_ms() - t0;
+}
+
+// A one-shot call once it has created its handle p: reset the LM to `o`, run o.max_iter passes if `solve`, write the result
+// back (write_back()) and fill *summary only while every step succeeds, and destroy the handle in every case.
+template <class Problem, class Opts, class WriteBack>
+inline int lm_one_shot(Problem* p, const Opts& o, bool solve, int (*reset_lm)(Problem*, const Opts*),
+                       int (*iterate)(Problem*, int32_t, lvba_summary*), int (*destroy)(Problem*), const WriteBack& write_back,
+                       double t0, lvba_summary* summary) {
+  lvba_summary s;
+  memset(&s, 0, sizeof s);
+  int rc = reset_lm(p, &o);
+  if (rc == LVBA_OK && solve) rc = iterate(p, o.max_iter, &s);
+  if (rc == LVBA_OK) rc = write_back();
+  if (rc == LVBA_OK && summary) {
+    *summary = s;
+    one_shot_totals(summary, p, t0);
+  }
+  destroy(p);
+  return rc;
 }
 
 // ---------------------------------------------------------------- block envelope (host build + device copy)
@@ -676,14 +725,8 @@ struct EnvSolver {
     if (path == LVBA_SOLVE_ANY_WIDTH) {
       // ---------------- any width: every column step spread over the device (envelope_wide.h); 4 launches per block row
       const wide::View wv{env.n, env.d_first.p, env.d_row_start.p};                                       // z holds the right-hand side (written by the caller)
-      int64_t n_launch = 0;
-      auto launch = [&](int64_t items, const auto& f) {
-        const int grid = (int)std::min<int64_t>((items + 127) / 128, kNumSMs * 16);
-        env_wide_pass_kernel<<<grid, 128, 0, s>>>(items, f);
-        ++n_launch;
-      };
+      auto launch = [&](int64_t items, const auto& f) { wide_pass(s, items, f, launches); };
       wide::factor_and_solve(launch, wv, env.first.data(), env.last.data(), L.p, dinv.p, z.p, colT.p, x, status.p);
-      *launches += n_launch;
       LVBA_CUDA(cudaGetLastError());
       return LVBA_OK;
     }

@@ -231,17 +231,8 @@ int lvba_voxel_map_lidar_lm(lvba_voxel_map* m, double* poses, int32_t min_voxels
   lvba_lidar_problem* p = nullptr;
   int rc = lvba_voxel_map_lidar_create(m, poses, &p);
   if (rc != LVBA_OK) return rc;
-  rc = lvba_lidar_reset_lm(p, &o);
-  if (rc == LVBA_OK) rc = lvba_lidar_iterate(p, o.max_iter, &s);
-  if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);
-  if (rc == LVBA_OK && summary) {
-    *summary = s;
-    summary->ms_setup = p->ms_setup;
-    summary->kernel_launches = p->launches; summary->h2d_bytes = p->h2d; summary->d2h_bytes = p->d2h;
-    summary->ms_total = lvba::wall_ms() - t0;
-  }
-  lvba_lidar_destroy(p);
-  return rc;
+  return lvba::lm_one_shot(p, o, /*solve=*/true, lvba_lidar_reset_lm, lvba_lidar_iterate, lvba_lidar_destroy,
+                           [&] { return lvba_lidar_get_poses(p, poses); }, t0, summary);
 } LVBA_ABI_END("lvba_voxel_map_lidar_lm")
 
 // The whole window stage of runWindowBA (src/lvba_system.cpp:232-266) from a windowed map: tras_opt + damping_iter of every
@@ -268,23 +259,7 @@ int lvba_voxel_map_lidar_lm_batch(lvba_voxel_map* m, double* poses, int32_t min_
   catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
   catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_voxel_map_lidar_lm_batch"); }
   if (rc != LVBA_OK) return rc;
-  p->opts = o;
-  lvba_summary tot;
-  memset(&tot, 0, sizeof tot);
-  rc = lvba::lidar_set_mode(p, o);
-  if (rc == LVBA_OK) {
-    try { rc = lvba::lidar_batch_lm_impl(p, min_voxels_per_pose, summaries, &tot); }
-    catch (...) { rc = lvba::fail(LVBA_ERR_NOMEM, "host allocation failed in lvba_voxel_map_lidar_lm_batch"); }
-  }
-  if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses);
-  if (rc == LVBA_OK && total) {
-    *total = tot;
-    total->ms_setup = p->ms_setup;
-    total->kernel_launches = p->launches; total->h2d_bytes = p->h2d; total->d2h_bytes = p->d2h;
-    total->ms_total = lvba::wall_ms() - t0;
-  }
-  lvba_lidar_destroy(p);
-  return rc;
+  return lvba::lidar_batch_one_shot(p, o, min_voxels_per_pose, poses, summaries, total, t0, "lvba_voxel_map_lidar_lm_batch");
 }
 
 int lvba_voxel_map_destroy(lvba_voxel_map* m) LVBA_ABI_BEGIN {

@@ -21,6 +21,7 @@ Each function restates, line for line, the cited reference code:
   only_residual        evaluate_only_residual          include/BALM/bavoxel.hpp:176-203
   so3_exp              Exp                             include/BALM/tools.hpp:62-77
   damping_iter         BALM2::damping_iter             include/BALM/bavoxel.hpp:662-767
+  balm_update          its accept / reject and stop    include/BALM/bavoxel.hpp:733-762
 
 Storage differs from the reference on purpose (SURVEY.md §0.3): the reference
 keeps a dense vector<PointCluster>(win_size) per voxel and a dense 6W x 6W
@@ -214,6 +215,26 @@ def lm_step(H, g, u):
     return dx, d
 
 
+def balm_update(u, v, residual1, residual2, q1, rel_tol, bad=False):
+    """The decision of one damping_iter pass (bavoxel.hpp:733-762): accept the trial poses when the residual drops, and the new
+    damping u, v; then the stop test (:760, off for rel_tol < 0).  A non-finite trial residual or model, or `bad` (a non-finite
+    step or singular pivot on the device), counts as no decrease.  Returns (u, v, accepted, stop)."""
+    if bad or not (np.isfinite(residual2) and np.isfinite(q1)):
+        residual2 = np.nan
+    q = residual1 - residual2
+    accepted = q > 0
+    if accepted:
+        rho = q / q1
+        v = 2.0
+        qq = 1 - (2 * rho - 1) ** 3
+        u *= (1.0 / 3.0) if qq < 1.0 / 3.0 else qq
+    else:
+        u *= v
+        v *= 2
+    stop = rel_tol >= 0 and abs(residual1 - residual2) / residual1 < rel_tol
+    return u, v, bool(accepted), bool(stop)
+
+
 def damping_iter(vox_ptr, pose_idx, clusters, poses, u0=0.01, v0=2.0, max_iter=10, rel_tol=1e-6,
                  log=None):
     """bavoxel.hpp:662-767 incl. quirks Q1-Q3 of SURVEY.md §8a.  Returns (poses, info)."""
@@ -237,28 +258,19 @@ def damping_iter(vox_ptr, pose_idx, clusters, poses, u0=0.01, v0=2.0, max_iter=1
         q1 = 0.5 * dx.dot(u * d * dx - g.ravel())       # line 729
         residual2 = only_residual(vox_ptr, pose_idx, clusters, trial) / V
         q1 /= V                                         # line 732
-        q = residual1 - residual2
-        info["trace"].append(dict(it=it, r1=residual1, r2=residual2, u=u, v=v, q=q, q1=q1,
+        info["trace"].append(dict(it=it, r1=residual1, r2=residual2, u=u, v=v, q=residual1 - residual2, q1=q1,
                                   dx_inf=float(np.abs(dx).max())))
         if log:
             log(info["trace"][-1])
         info["iters"] = it + 1
-        if q > 0:
+        u, v, is_calc_hess, stop = balm_update(u, v, residual1, residual2, q1, rel_tol)
+        if is_calc_hess:
             poses = trial
-            rho = q / q1
-            v = 2.0
-            qq = 1 - (2 * rho - 1) ** 3
-            u *= (1.0 / 3.0) if qq < 1.0 / 3.0 else qq
-            is_calc_hess = True
             info["accepted"] += 1
             info["r_last"] = residual2
-        else:
-            u *= v
-            v *= 2
-            is_calc_hess = False
-            if info["r_last"] is None:
-                info["r_last"] = residual1
-        if abs(residual1 - residual2) / residual1 < rel_tol:   # line 760
+        elif info["r_last"] is None:
+            info["r_last"] = residual1
+        if stop:
             break
     info["u_last"], info["v_last"] = u, v
     return poses, info

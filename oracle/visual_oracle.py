@@ -236,14 +236,15 @@ def schur_system(J, r, D, nc):
     return S, rhs
 
 
-def ceres_lm(prob: VisualProblem, max_iter=50, radius0=1e4, log=None, scaling=True):
-    """Ceres 2.1 TrustRegionMinimizer + LevenbergMarquardtStrategy, restated."""
+def ceres_lm(prob: VisualProblem, max_iter=50, radius0=1e4, log=None, scaling=True, f_tol=1e-6, g_tol=1e-10, p_tol=1e-8):
+    """Ceres 2.1 TrustRegionMinimizer + LevenbergMarquardtStrategy, restated.  Every cost is prob.cost() (with a loss,
+    tests/visual_loss_oracle.py, 1/2 sum rho rather than 1/2 r.r of the corrected residuals).  The tolerances default to the
+    library's (lvba_visual_default_opts)."""
     min_diag, max_diag = 1e-6, 1e32
-    f_tol, g_tol, p_tol = 1e-6, 1e-10, 1e-8
     radius, nu = radius0, 2.0
     info = {"iters": 0, "accepted": 0, "trace": [], "term": "max_iter"}
     res, J = prob.residuals(jac=True)
-    cost = 0.5 * float(res @ res)
+    cost = prob.cost()
     info["cost0"] = cost
     if scaling:
         scale = 1.0 / (1.0 + np.sqrt(np.asarray(J.multiply(J).sum(0)).ravel()))
@@ -319,7 +320,7 @@ def single_step(prob: VisualProblem, radius=1e4, scaling=True, min_diag=1e-6, ma
     """One linearisation + LM solve at the current state (what lvba_visual_step computes).
     Returns dict(cost, model, cam_step[M,6], pt_step[T,3], scale, S, rhs) — S/rhs only for small problems."""
     res, J = prob.residuals(jac=True)
-    cost = 0.5 * float(res @ res)
+    cost = prob.cost()
     scale = 1.0 / (1.0 + np.sqrt(np.asarray(J.multiply(J).sum(0)).ravel())) if scaling else np.ones(prob.ncols)
     Js = (J @ sp.diags(scale)).tocsr()
     diag = np.clip(np.asarray(Js.multiply(Js).sum(0)).ravel(), min_diag, max_diag)

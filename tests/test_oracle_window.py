@@ -34,6 +34,8 @@ def test_skip_rule_and_untouched_windows():
 
 
 def test_cpp_port_agrees_window_by_window():
+    """The port sums H, g and the residual per thread, so its last bits follow the thread count: it runs with the reference's
+    own 16 (bavoxel.hpp:25), not the host's core count."""
     wp = GOLD["win_ptr"]
     first = GOLD["pose_idx"][GOLD["vox_ptr"][:-1]]
     win_of_vox = np.searchsorted(wp, first, side="right") - 1
@@ -45,7 +47,7 @@ def test_cpp_port_agrees_window_by_window():
         vp = np.zeros(len(vs) + 1, np.int64); vp[1:] = np.cumsum([len(x) for x in sl])
         idx = np.concatenate(sl)
         poses, s = cpu_ref.lidar_lm(vp, (GOLD["pose_idx"][idx] - wp[w]).astype(np.int32), GOLD["clusters"][idx],
-                                    GOLD["poses"][wp[w]:wp[w + 1]])
+                                    GOLD["poses"][wp[w]:wp[w + 1]], threads=16)
         assert s["iterations"] == GOLD["W_iters"][w] and s["accepted"] == GOLD["W_accepted"][w]
         assert abs(s["cost_last"] - GOLD["W_cost_last"][w]) <= 1e-9 * GOLD["W_cost_last"][w]
         assert np.abs(poses - GOLD["W_poses"][wp[w]:wp[w + 1]]).max() <= 1e-9

@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 
 from oracle import synth
+from oracle import visual_oracle as vo
 import visual_big_scene as vs
 import visual_loss_oracle as vl
 
@@ -94,7 +95,7 @@ def test_offline_visual_stage_with_losses_matches_oracle(gpu_pkg, tmp_path):
     vis = [x for x in (json.loads(ln) for ln in r.stdout.strip().splitlines()) if x.get("stage") == "visual"][0]
     p, (q1, t1, X1) = read_problem(prob)
     assert int(vl.vo.valid_tracks(p["plane_nd"]).sum()) == vis["points_kept"] and vis["points_kept"] >= 80
-    pr, info = vl.ceres_lm(vl.RobustProblem(*vs.args(p), fixed_cam=0, loss_reproj=(vl.HUBER, 1.0), loss_plane=(vl.HUBER, 0.1)))
+    pr, info = vo.ceres_lm(vl.RobustProblem(*vs.args(p), fixed_cam=0, loss_reproj=(vl.HUBER, 1.0), loss_plane=(vl.HUBER, 0.1)))
     plain = vl.RobustProblem(*vs.args(p), fixed_cam=0).cost()
     assert info["cost0"] < (1 - 1e-6) * plain                     # the losses change the cost: the flags reached the solve
     assert vis["iterations"] == info["iters"] and vis["termination"] == vl.TERM[info["term"]]

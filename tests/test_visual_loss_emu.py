@@ -12,6 +12,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+from oracle import visual_oracle as vo
 import visual_big_scene as vs
 import visual_loss_oracle as vl
 from test_visual_big_emu import Local
@@ -76,7 +77,7 @@ def check(emu, p, lr, lp, fixed_cam=0, radius=1e4, scaling=True):
     L = Local(p, fixed_cam)
     L.pr = pr = vl.RobustProblem(*vs.args(p), fixed_cam=fixed_cam, loss_reproj=lr, loss_plane=lp)
     kind, a = _loss_args(lr, lp)
-    ref = vl.single_step(pr, radius, scaling)
+    ref = vo.single_step(pr, radius, scaling)
     nc6 = 6 * pr.nc
     o = _step(emu, L, kind, a, radius, scaling, ref["y"][:nc6] if nc6 else np.zeros(6))
     assert abs(o["out"][0] - ref["cost"]) <= 1e-10 * ref["cost"]

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from oracle import synth
+from oracle import visual_oracle as vo
 import visual_big_scene as vs
 import visual_loss_oracle as vl
 from test_visual_big_gpu import _mixed
@@ -60,7 +61,7 @@ def test_cost_and_step_match_oracle(gpu_pkg, scene, losses, fixed_cam):
     c = P.cost()
     assert abs(c - pr.cost()) <= 1e-10 * pr.cost() and c < plain
     cs, ps, model, cost = P.step(1e4)
-    ref = vl.single_step(pr, 1e4, True)
+    ref = vo.single_step(pr, 1e4, True)
     assert abs(cost - ref["cost"]) <= 1e-10 * ref["cost"]
     assert abs(model - ref["model"]) <= 1e-7 * abs(ref["model"])
     assert np.abs(cs - ref["cam_step"]).max() <= 1e-6 * np.abs(ref["cam_step"]).max()
@@ -88,7 +89,7 @@ def test_full_lm_matches_oracle(gpu_pkg, scene, losses):
     which differ in rounding, then accept one step apart.  Its cost and step are checked above on the mixed scene.)"""
     p = LM_SCENES[scene]()
     q, t, X, s = gpu_pkg.visual_lm(*vs.args(p), opts=_opts(gpu_pkg, losses))
-    pr, info = vl.ceres_lm(vl.RobustProblem(*vs.args(p), loss_reproj=losses[0], loss_plane=losses[1]))
+    pr, info = vo.ceres_lm(vl.RobustProblem(*vs.args(p), loss_reproj=losses[0], loss_plane=losses[1]))
     assert s["iterations"] == info["iters"]
     assert s["accepted"] == info["accepted"]
     assert s["termination"] == vl.TERM[info["term"]]

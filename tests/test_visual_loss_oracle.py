@@ -66,7 +66,7 @@ def test_no_loss_is_the_plain_oracle_bit_for_bit():
     rb, Jb = b.residuals(jac=True)
     assert np.array_equal(ra, rb) and (Ja != Jb).nnz == 0 and a.cost() == b.cost()
     _, ia = vo.ceres_lm(a)
-    _, ib = vl.ceres_lm(b)
+    _, ib = vo.ceres_lm(b)
     assert (ia["iters"], ia["accepted"], ia["term"], ia["cost0"], ia["cost"]) == (ib["iters"], ib["accepted"], ib["term"], ib["cost0"], ib["cost"])
 
 
@@ -81,7 +81,7 @@ def test_robust_lm_on_wrong_matches(kind):
     p = _problem(seed=9, n_poses=10, n_tracks=60, outliers=True)
     pr = vl.RobustProblem(*_args(p), fixed_cam=0, loss_reproj=(kind, 1.0), loss_plane=(kind, 0.1))
     g0 = vl.tangent_gradient_fd(pr)
-    pr, info = vl.ceres_lm(pr, max_iter=300, f_tol=-1.0, p_tol=-1.0)     # until the radius collapses at the rounding floor
+    pr, info = vo.ceres_lm(pr, max_iter=300, f_tol=-1.0, p_tol=-1.0)     # until the radius collapses at the rounding floor
     assert info["accepted"] > 0
     # at the optimum the plane residuals are near 0, where sqrt(e^2 + 1e-12) bends within |e| ~ 1e-6: a smaller step
     g1 = vl.tangent_gradient_fd(pr, h=1e-8)

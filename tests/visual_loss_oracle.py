@@ -7,15 +7,13 @@ Restated from ceres-solver 2.1.0 (not vendored; nothing to hold it against here)
                                 multiplied by sqrt(rho'(s)), s = |r|^2 of the block, and nothing else changes
   cost                          1/2 sum rho(s) over the blocks, also for the candidate of the trust-region test
 Everything downstream (Jacobi scaling, LM diagonal, Schur system, gradient, model cost change) uses the corrected residuals and
-Jacobian, so oracle/visual_oracle.py's single_step and trust-region loop apply to them unchanged, except where they take the cost
-as 1/2 r.r of the returned residuals: ceres_lm and single_step below take it from RobustProblem.cost().  With both losses None
-everything equals oracle/visual_oracle.py bit for bit.
+Jacobian, so oracle/visual_oracle.py's single_step and trust-region loop apply to them unchanged: they take every cost from
+RobustProblem.cost().  With both losses None everything equals oracle/visual_oracle.py bit for bit.
 """
 from __future__ import annotations
 
 import numpy as np
 import scipy.sparse as sp
-import scipy.sparse.linalg as spla
 
 from oracle import visual_oracle as vo
 
@@ -80,81 +78,6 @@ class RobustProblem(vo.VisualProblem):
         res, _ = vo.VisualProblem.residuals(self, q, t, X, jac=False)
         _, rho_o, _, rho_p, _ = self._rho(res)
         return 0.5 * float(rho_o.sum() + rho_p.sum())
-
-
-def single_step(prob: RobustProblem, radius=1e4, scaling=True, min_diag=1e-6, max_diag=1e32):
-    """vo.single_step on the corrected residuals and Jacobian, with cost = 1/2 sum rho."""
-    out = vo.single_step(prob, radius, scaling, min_diag, max_diag)
-    out["cost"] = prob.cost()
-    return out
-
-
-def ceres_lm(prob: RobustProblem, max_iter=50, radius0=1e4, scaling=True, f_tol=1e-6, g_tol=1e-10, p_tol=1e-8):
-    """vo.ceres_lm (Ceres 2.1 TrustRegionMinimizer + LevenbergMarquardtStrategy) with every cost from prob.cost().  The
-    tolerances default to the library's (lvba_visual_default_opts)."""
-    min_diag, max_diag = 1e-6, 1e32
-    radius, nu = radius0, 2.0
-    info = {"iters": 0, "accepted": 0, "trace": [], "term": "max_iter"}
-    res, J = prob.residuals(jac=True)
-    cost = prob.cost()
-    info["cost0"] = cost
-    scale = 1.0 / (1.0 + np.sqrt(np.asarray(J.multiply(J).sum(0)).ravel())) if scaling else np.ones(prob.ncols)
-    info["scale"] = scale
-    Js = (J @ sp.diags(scale)).tocsr()
-    grad = J.T @ res
-    info["grad0"] = grad
-    if np.abs(grad).max() <= g_tol:
-        info["term"] = "gradient"; info["cost"] = cost
-        return prob, info
-    reuse_diag, diag, invalid = False, None, 0
-    for it in range(1, max_iter + 1):
-        info["iters"] = it
-        if not reuse_diag:
-            diag = np.clip(np.asarray(Js.multiply(Js).sum(0)).ravel(), min_diag, max_diag)
-        lm = np.sqrt(diag / radius)
-        A = (Js.T @ Js + sp.diags(lm * lm)).tocsc()
-        y = spla.spsolve(A, -(Js.T @ res))
-        reuse_diag = True
-        Jy = Js @ y
-        model = -float(Jy @ (res + 0.5 * Jy))
-        if not np.all(np.isfinite(y)) or model <= 0:
-            invalid += 1
-            radius *= 0.5
-            if invalid >= 5:
-                info["term"] = "invalid_steps"; break
-            continue
-        invalid = 0
-        qn, tn, Xn = prob.plus(y * scale)
-        cand = prob.cost(qn, tn, Xn)
-        ca, tv = prob.cam_active, prob.tv
-        step_norm = float(np.sqrt(((qn[ca] - prob.q[ca]) ** 2).sum() + ((tn[ca] - prob.t[ca]) ** 2).sum()
-                                  + ((Xn[tv] - prob.X[tv]) ** 2).sum()))
-        rho = (cost - cand) / model
-        info["trace"].append(dict(it=it, cost=cost, cand=cand, rho=rho, radius=radius, step=step_norm, model=model))
-        if step_norm <= p_tol * (prob.x_norm() + p_tol):
-            info["term"] = "parameter"; break
-        if abs(cost - cand) <= f_tol * cost:
-            info["term"] = "function"; break
-        if rho > 1e-3:
-            prob.q, prob.t, prob.X = qn, tn, Xn
-            cost = cand
-            info["accepted"] += 1
-            res, J = prob.residuals(jac=True)
-            Js = (J @ sp.diags(scale)).tocsr()
-            grad = J.T @ res
-            radius = min(1e16, radius / max(1.0 / 3.0, 1.0 - (2 * rho - 1) ** 3))
-            nu = 2.0
-            reuse_diag = False
-            if np.abs(grad).max() <= g_tol:
-                info["term"] = "gradient"; break
-        else:
-            radius /= nu
-            nu *= 2
-            if radius < 1e-32:
-                info["term"] = "radius"; break
-    info["cost"] = cost
-    info["radius"] = radius
-    return prob, info
 
 
 TERM = {"max_iter": 0, "function": 1, "parameter": 2, "gradient": 3, "radius": 4, "invalid_steps": 5}
