@@ -33,8 +33,7 @@ namespace lvba {
 
 using tiles::kTileSlots;
 using tiles::kMaxVoxPerTile;
-constexpr int kSlots = 128;            // slots (threads) per batch CTA of the residual pass and of the visual kernels; the most poses a
-                                       // voxel of the tiles may have (more: lidar_big.h)
+using tiles::kSlots;
 constexpr int kStageStride = 37;       // visual build: doubles per slot in the staging buffer (36 + 1 pad: odd => no LDS.64 bank conflicts)
 constexpr int kLStage = 19;            // LiDAR build: 10 cluster values, then HALF a diagonal block (18 + 1 pad)
 constexpr int kFStride = 19;           // 18 factor doubles + 1 pad

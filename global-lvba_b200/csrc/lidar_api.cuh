@@ -8,8 +8,7 @@
 #include "balm_rule.h"
 #include "exec.cuh"
 #include "lidar.cuh"
-#include "lidar_big.h"
-#include "lidar_tiles.h"
+#include "lidar_plan.h"
 
 namespace lvba {
 
@@ -137,6 +136,10 @@ struct lvba_lidar_problem {
     return lvba::big::View{(int64_t)n_big, big_vox_ptr.p, big_pose.p, big_cl.p, big_pair_ptr.p, env.d_first.p, env.d_row_start.p};
   }
 
+  // the tiles' CSR for the passes of lidar_tiles.h (vox_pair: set by lidar_tables)
+  lvba::tiles::TableIn table_in() const {
+    return lvba::tiles::TableIn{n_tiles, W, env.nblocks, tile_vox.p, vox_ptr.p, pidx.p, nullptr, env.d_first.p, env.d_row_start.p};
+  }
   lvba::LidarView view() const {
     lvba::LidarView v_;
     v_.W = W; v_.cl = cl.p; v_.nnz_pad = (long long)(cl.n / 5);
@@ -205,10 +208,8 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   LVBA_TRY(lidar_validate(W, V, vox_ptr, pose_idx, d_clusters ? d_clusters : clusters, poses));
   LVBA_TRY(select_device(device));
   const double t0 = wall_ms();
-  const bool tlog = getenv("LVBA_SETUP_TIMING") != nullptr;
-  double tprev = t0;
-  auto lap = [&](const char* what) { if (tlog) { cudaStreamSynchronize(nullptr); const double t = wall_ms(); fprintf(stderr, "[lidar setup] %-22s %8.2f ms\n", what, t - tprev); tprev = t; } };
-  if (tlog) fprintf(stderr, "[lidar setup] %-22s %8.2f ms\n", "validate", t0 - t_val0);
+  SetupLaps lap("lidar setup", 22, nullptr, t_val0);
+  lap.host("validate");
   std::unique_ptr<lvba_lidar_problem> P(new lvba_lidar_problem());
   P->W = W; P->V_total = V;
   LVBA_CUDA(cudaGetDevice(&P->device));
@@ -244,115 +245,53 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   lap("host copies");
 
   // ---- envelope structure over ALL voxels (identical on every rank)
-  std::vector<int> first_raw(W);
-  for (int r = 0; r < W; ++r) first_raw[r] = r;
-  {
-    std::vector<int> first_w((size_t)kMaxSetupThreads * (size_t)W);
-    for (int w = 0; w < kMaxSetupThreads; ++w) std::copy(first_raw.begin(), first_raw.end(), first_w.begin() + (size_t)w * (size_t)W);
-    parallel_chunks(V, 1 << 14, [&](int64_t a0, int64_t a1, int w) {
-      int* fr = first_w.data() + (size_t)w * (size_t)W;
-      for (int64_t a = a0; a < a1; ++a) {
-        const int m = pose_idx[vox_ptr[a]];
-        for (int64_t q = vox_ptr[a]; q < vox_ptr[a + 1]; ++q) fr[pose_idx[q]] = std::min(fr[pose_idx[q]], m);
-      }
-    });
-    for (int w = 0; w < kMaxSetupThreads; ++w)
-      for (int r = 0; r < W; ++r) first_raw[r] = std::min(first_raw[r], first_w[(size_t)w * (size_t)W + r]);
-  }
-  LVBA_TRY(P->env.build(first_raw, s, &P->h2d));
-  // ---- batched window BA: window of every pose, every voxel inside one window
-  std::vector<int> pose_grp;
+  LVBA_TRY(P->env.build(lidar_first_rows(W, V, vox_ptr, pose_idx), s, &P->h2d));
+  Comm& cm = comm();
+  const bool sharded = cm.active();
   if (n_groups > 0) {
-    if (comm().active()) return fail(LVBA_ERR_UNSUPPORTED, "the batched window BA runs on one GPU per call (windows are independent: shard them across ranks)");
+    if (sharded) return fail(LVBA_ERR_UNSUPPORTED, "the batched window BA runs on one GPU per call (windows are independent: shard them across ranks)");
     P->n_groups = n_groups;
     P->grp_ptr.assign(grp_ptr, grp_ptr + n_groups + 1);
-    pose_grp.resize((size_t)W);
-    for (int g = 0; g < n_groups; ++g)
-      for (int r = grp_ptr[g]; r < grp_ptr[g + 1]; ++r) pose_grp[r] = g;
-    P->grp_V.assign((size_t)n_groups, 0);
-    for (int64_t a = 0; a < V; ++a) {
-      const int g = pose_grp[pose_idx[vox_ptr[a]]];
-      if (pose_grp[pose_idx[vox_ptr[a + 1] - 1]] != g)
-        return fail(LVBA_ERR_INVALID_ARG, "voxel %lld spans two windows", (long long)a);
-      ++P->grp_V[g];
-    }
   }
-  LVBA_TRY(P->solver.prepare(P->env, s, LVBA_SOLVE_AUTO, 0, P->grp_ptr));     // grp_ptr empty: not batched
+  // a rank holds the voxels of its poses, cut by the solver's row split: the solver is prepared first.  The batched solve (one
+  // GPU) is prepared after the layout, which checks that no voxel spans two windows.
+  if (n_groups == 0) LVBA_TRY(P->solver.prepare(P->env, s));
   lap("envelope+solver alloc");
 
   // ---- shard: voxel -> owner of its lowest pose index (SURVEY.md §8e)
-  Comm& cm = comm();
-  // the voxels this rank holds (all of them on one rank: `owned` stays empty and stands for 0..V-1)
   std::vector<int64_t> owned;
-  const bool sharded = cm.active();
   if (sharded) {
     owned.reserve((size_t)V);
     for (int64_t a = 0; a < V; ++a)
       if ((P->solver.dist() ? P->solver.dist_owner(pose_idx[vox_ptr[a]]) : shard_owner(pose_idx[vox_ptr[a]], W, cm.n_ranks)) == cm.rank)
         owned.push_back(a);
   }
-  // voxels seen from more than kSlots poses do not fit a batch CTA: they leave `owned` and take the passes of lidar_big.h
-  std::vector<int64_t> bigv;
-  {
-    const int64_t n_own = sharded ? (int64_t)owned.size() : V;
-    bool has_big = false;
-    for (int64_t j = 0; j < n_own && !has_big; ++j) { const int64_t a = sharded ? owned[j] : j; has_big = vox_ptr[a + 1] - vox_ptr[a] > kSlots; }
-    if (has_big) {
-      std::vector<int64_t> small;
-      for (int64_t j = 0; j < n_own; ++j) {
-        const int64_t a = sharded ? owned[j] : j;
-        (vox_ptr[a + 1] - vox_ptr[a] > kSlots ? bigv : small).push_back(a);
-      }
-      owned.swap(small);
-    }
-    // the batched window LM (lidar_batch_lm_impl) has no big-voxel passes: such a voxel would silently drop out of H, g and the
-    // residual sums while still counting in the AVG_THR divisor.  A window holds <= 31 poses (EnvSolver::prepare), so this cannot
-    // happen today; refuse loudly if that ever changes (ADVICE r1).
-    if (n_groups > 0 && !bigv.empty())
-      return fail(LVBA_ERR_UNSUPPORTED, "batched window BA: voxel %lld is seen from %lld poses (more than %d)", (long long)bigv[0],
-                  (long long)(vox_ptr[bigv[0] + 1] - vox_ptr[bigv[0]]), kSlots);
+  LidarLayout L;
+  switch (lidar_layout(W, V, vox_ptr, pose_idx, sharded ? &owned : nullptr, n_groups, grp_ptr, L)) {
+    case kLayoutSpansWindows: return fail(LVBA_ERR_INVALID_ARG, "voxel %lld spans two windows", (long long)L.err_vox);
+    case kLayoutBigInBatch:
+      return fail(LVBA_ERR_UNSUPPORTED, "batched window BA: voxel %lld is seen from %lld poses (more than %d)", (long long)L.err_vox,
+                  (long long)(vox_ptr[L.err_vox + 1] - vox_ptr[L.err_vox]), kSlots);
   }
-  const bool all = !sharded && bigv.empty();
-  // voxels in the order of their lowest pose: the voxels of a build tile then share pose pairs, whose H blocks the tile sums on
-  // chip (lidar_tiles.h); the windows of the batched window BA, consecutive pose ranges, come out contiguous and in order
-  std::vector<int> slot0, l_vox_ptr;                           // first caller slot / first local slot of every local voxel
-  const int64_t Vl = all ? V : (int64_t)owned.size();
-  const long long nnz = tiles::order_by_lowest_pose(W, all ? nullptr : owned.data(), Vl, vox_ptr, pose_idx, slot0, l_vox_ptr);
-  bool identity = all;                                         // the caller's voxels, in the caller's order
-  long long np = 0;                                            // pose pairs
-  for (int64_t i = 0; i < Vl; ++i) {
-    const long long K = l_vox_ptr[i + 1] - l_vox_ptr[i];
-    np += K * (K - 1) / 2;
-    identity = identity && slot0[i] == l_vox_ptr[i];
-  }
-  P->V_local = Vl; P->nnz_local = nnz; P->n_pairs = np;
-
-  // ---- residual batches (<= kSlots slots) and build tiles (<= kTileSlots slots): consecutive voxels, never across a window
-  std::vector<int> vox_grp(n_groups > 0 ? (size_t)Vl : (size_t)0);
-  for (int64_t i = 0; i < (int64_t)vox_grp.size(); ++i) vox_grp[i] = pose_grp[pose_idx[slot0[i]]];
-  const int* grp = n_groups > 0 ? vox_grp.data() : nullptr;
-  const std::vector<int> batch_vox = tiles::cut_ranges(Vl, l_vox_ptr.data(), grp, kSlots, kSlots);
-  const std::vector<int> tile_vox = tiles::cut_ranges(Vl, l_vox_ptr.data(), grp, kTileSlots, kMaxVoxPerTile);
-  P->n_batches = (int)batch_vox.size() - 1;
-  P->n_tiles = (int)tile_vox.size() - 1;
+  const int64_t Vl = (int64_t)L.slot0.size();
+  const long long nnz = L.nnz;
+  P->V_local = Vl; P->nnz_local = nnz; P->n_pairs = L.n_pairs;
+  P->n_batches = (int)L.batch_vox.size() - 1;
+  P->n_tiles = (int)L.tile_vox.size() - 1;
   if (n_groups > 0) {
-    auto per_window = [&](const std::vector<int>& cut) {      // range of batches / tiles of every window
-      std::vector<int> r((size_t)n_groups + 1, 0);
-      for (size_t k = 0; k + 1 < cut.size(); ++k) ++r[(size_t)vox_grp[cut[k]] + 1];
-      for (int g = 0; g < n_groups; ++g) r[g + 1] += r[g];
-      return r;
-    };
-    LVBA_TRY(P->d_grp_batch.upload(per_window(batch_vox), s, &P->h2d));
-    LVBA_TRY(P->d_grp_tile.upload(per_window(tile_vox), s, &P->h2d));
+    LVBA_TRY(P->solver.prepare(P->env, s, LVBA_SOLVE_AUTO, 0, P->grp_ptr));
+    P->grp_V = L.grp_V;
+    LVBA_TRY(P->d_grp_batch.upload(L.grp_batch, s, &P->h2d));
+    LVBA_TRY(P->d_grp_tile.upload(L.grp_tile, s, &P->h2d));
     LVBA_TRY(P->d_grp_ptr.upload(P->grp_ptr, s, &P->h2d));
-    LVBA_TRY(P->d_pose_grp.upload(pose_grp, s, &P->h2d));
+    LVBA_TRY(P->d_pose_grp.upload(L.pose_grp, s, &P->h2d));
     LVBA_TRY(P->d_accept.alloc((size_t)n_groups));
     LVBA_TRY(P->d_u_grp.alloc((size_t)n_groups));
     LVBA_TRY(P->d_grp_scal.alloc((size_t)4 * n_groups));
     LVBA_TRY(P->d_grp_scal.zero(s));
     P->h_grp_scal_bytes = (size_t)4 * n_groups * sizeof(double);
     LVBA_TRY(pinned_pool().take(P->h_grp_scal_bytes, (void**)&P->h_grp_scal));
-    LVBA_CUDA(cudaStreamSynchronize(s));                       // local vectors
+    LVBA_CUDA(cudaStreamSynchronize(s));                       // L's vectors are uploaded
   }
 
   lap("order+batches+tiles");
@@ -361,10 +300,10 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   const long long nnz_pad = ((nnz + 31) / 32) * 32 + 32;
   LVBA_TRY(P->cl.alloc((size_t)5 * nnz_pad));
   LVBA_TRY(P->cl.zero(s));
-  LVBA_TRY(P->vox_ptr.upload(l_vox_ptr, s, &P->h2d));
+  LVBA_TRY(P->vox_ptr.upload(L.l_vox_ptr, s, &P->h2d));
   if (lane.done) LVBA_CUDA(cudaStreamWaitEvent(s, lane.done, 0));            // the kernels below read the records
   {
-    if (identity) {
+    if (L.identity) {
       if (nnz > 0) {
         lidar_aos_to_soa_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(nnz, nnz_pad, aos_dev, P->cl.p);
         ++P->launches;
@@ -373,56 +312,39 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
       // reordered (or a shard's scattered) voxels: the ONE copy of the caller's records and pose indices + a device-side gather
       DevBuf<int> d_slot0, d_caller_pidx;
       if (nnz > 0) {
-        LVBA_TRY(d_slot0.upload(slot0, s, &P->h2d));
+        LVBA_TRY(d_slot0.upload(L.slot0, s, &P->h2d));
         LVBA_TRY(d_caller_pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)vox_ptr[V], s, &P->h2d));
         LVBA_TRY(P->pidx.alloc((size_t)nnz));
         lidar_gather_slots_kernel<<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(nnz, nnz_pad, (int)Vl, P->vox_ptr.p, d_slot0.p, d_caller_pidx.p,
                                                                                 aos_dev, P->pidx.p, P->cl.p);
         ++P->launches;
       }
-      if (!bigv.empty()) {                   // the big voxels' records stay AoS (lidar_big.h reads them slot by slot)
-        std::vector<int64_t> bvp{0}, bpp{0};
-        std::vector<int32_t> bpose;
-        std::vector<int> bsrc;
-        for (int64_t a : bigv) {
-          for (int64_t q = vox_ptr[a]; q < vox_ptr[a + 1]; ++q) { bsrc.push_back((int)q); bpose.push_back(pose_idx[q]); }
-          const int64_t K = vox_ptr[a + 1] - vox_ptr[a];
-          bvp.push_back((int64_t)bsrc.size());
-          bpp.push_back(bpp.back() + K * (K - 1) / 2);
-        }
-        P->n_big = (long long)bigv.size(); P->n_big_slots = (long long)bsrc.size(); P->n_big_pairs = bpp.back();
+      if (!L.big_vox.empty()) {              // the big voxels' records stay AoS (lidar_big.h reads them slot by slot)
+        P->n_big = (long long)L.big_vox.size(); P->n_big_slots = (long long)L.big_src.size(); P->n_big_pairs = L.big_pair_ptr.back();
         DevBuf<int> d_bsrc;
-        LVBA_TRY(d_bsrc.upload(bsrc, s, &P->h2d));
-        LVBA_TRY(P->big_vox_ptr.upload(bvp, s, &P->h2d));
-        LVBA_TRY(P->big_pair_ptr.upload(bpp, s, &P->h2d));
-        LVBA_TRY(P->big_pose.upload(bpose, s, &P->h2d));
+        LVBA_TRY(d_bsrc.upload(L.big_src, s, &P->h2d));
+        LVBA_TRY(P->big_vox_ptr.upload(L.big_vox_ptr, s, &P->h2d));
+        LVBA_TRY(P->big_pair_ptr.upload(L.big_pair_ptr, s, &P->h2d));
+        LVBA_TRY(P->big_pose.upload(L.big_pose, s, &P->h2d));
         LVBA_TRY(P->big_cl.alloc((size_t)P->n_big_slots * 10));
         LVBA_TRY(P->big_params.alloc((size_t)P->n_big * big::kParams));
         LVBA_TRY(P->big_feat.alloc((size_t)P->n_big_slots * big::kFeat));
         lidar_gather_aos_kernel<<<(unsigned)((P->n_big_slots + 255) / 256), 256, 0, s>>>(P->n_big_slots, d_bsrc.p, aos_dev, P->big_cl.p);
         ++P->launches;
-        LVBA_CUDA(cudaStreamSynchronize(s)); // the host vectors and d_bsrc go out of scope
+        LVBA_CUDA(cudaStreamSynchronize(s)); // d_bsrc goes out of scope
       }
       LVBA_CUDA(cudaStreamSynchronize(s));   // d_slot0 and d_caller_pidx are freed on scope exit
     }
   }
-  if (tlog) { cudaStreamSynchronize(s); } lap("cluster upload+SoA");
+  lap("cluster upload+SoA", s);
   static_assert(sizeof(int) == sizeof(int32_t), "pose_idx is uploaded as it is");
-  if (identity) LVBA_TRY(P->pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)nnz, s, &P->h2d));
-  LVBA_TRY(P->batch_vox.upload(batch_vox, s, &P->h2d));
-  LVBA_TRY(P->tile_vox.upload(tile_vox, s, &P->h2d));
-  if (P->n_tiles > 0) {                                        // destination table of the build, on the device from the CSR just uploaded
+  if (L.identity) LVBA_TRY(P->pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)nnz, s, &P->h2d));
+  LVBA_TRY(P->batch_vox.upload(L.batch_vox, s, &P->h2d));
+  LVBA_TRY(P->tile_vox.upload(L.tile_vox, s, &P->h2d));
+  {                                                            // destination table of the build, on the device from the CSR just uploaded
     CudaExec ex;
     ex.stream = s;
-    DevBuf<long long> d_pair_cnt, d_vox_pair;                  // pose pairs before every local voxel
-    LVBA_TRY(d_pair_cnt.alloc((size_t)Vl + 1));
-    LVBA_TRY(d_vox_pair.alloc((size_t)Vl + 1));
-    LVBA_TRY(ex.for_each(Vl + 1, tiles::PairCountF{P->vox_ptr.p, Vl, d_pair_cnt.p}));
-    LVBA_TRY(ex.exclusive_scan(d_pair_cnt.p, d_vox_pair.p, Vl + 1));
-    const tiles::TableIn tin{P->n_tiles, W, P->env.nblocks, P->tile_vox.p, P->vox_ptr.p, P->pidx.p, d_vox_pair.p,
-                             P->env.d_first.p, P->env.d_row_start.p};
-    LVBA_TRY(tiles::build_runs(ex, tin, /*by_slot=*/false, np, P->prun));
-    LVBA_TRY(tiles::build_runs(ex, tin, /*by_slot=*/true, nnz, P->drun));
+    LVBA_TRY(lidar_tables(ex, P->table_in(), Vl, L.n_pairs, nnz, P->prun, P->drun));
     P->launches += ex.launches;
   }
   lap("destination table");
@@ -447,32 +369,14 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   return LVBA_OK;
 }
 
-// Deterministic mode: the records of the build and their destinations.  Records of H: the tiles' pair runs, the tiles' pose
-// runs, the big voxels' slots, the big voxels' pairs; records of g: the tiles' pose runs, the big voxels' slots.  Each set in
-// its enumeration order, so that every destination's records come in ascending (tile, run) order, then in item order.
+// Deterministic mode: the records of the build and their destinations (lidar_det_index)
 inline int lidar_det_setup(lvba_lidar_problem* P) {
   if (P->det_ready) return LVBA_OK;
-  const int64_t npr = P->prun.n_runs, ndr = P->drun.n_runs;
-  const int64_t nH = npr + ndr + P->n_big_slots + P->n_big_pairs, ng = ndr + P->n_big_slots;
+  const int64_t nH = P->prun.n_runs + P->drun.n_runs + P->n_big_slots + P->n_big_pairs;
   if (nH >= (int64_t)1 << 32) return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode: %lld contributions to H (at most 2^32)", (long long)nH);
   CudaExec ex;
   ex.stream = P->stream;
-  LVBA_TRY(tiles::fixed_sum_alloc(P->det_H, nH, 36));
-  LVBA_TRY(tiles::fixed_sum_alloc(P->det_g, ng, 6));
-  if (P->n_tiles > 0) {
-    const tiles::TableIn tin{P->n_tiles, P->W, P->env.nblocks, P->tile_vox.p, P->vox_ptr.p, P->pidx.p, nullptr,
-                             P->env.d_first.p, P->env.d_row_start.p};
-    LVBA_TRY(ex.for_each(npr, tiles::PairRunDstF{tin, P->prun.tile_run.p, P->prun.run_ptr.p, P->prun.code.p, P->det_H.dst.p}));
-    LVBA_TRY(ex.for_each(ndr, tiles::SlotRunDstF{tin, P->drun.tile_run.p, P->drun.run_ptr.p, P->drun.code.p, P->det_H.dst.p + npr,
-                                                 P->det_g.dst.p}));
-  }
-  if (P->n_big > 0) {
-    const big::View bv = P->big_view();
-    LVBA_TRY(ex.for_each(P->n_big_slots, big::SlotDstF{bv, P->det_H.dst.p + npr + ndr, P->det_g.dst.p + ndr}));
-    LVBA_TRY(ex.for_each(P->n_big_pairs, big::PairDstF{bv, P->det_H.dst.p + npr + ndr + P->n_big_slots}));
-  }
-  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_H, P->env.nblocks));
-  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_g, P->W));
+  LVBA_TRY(lidar_det_index(ex, P->table_in(), P->prun, P->drun, P->big_view(), P->n_big_slots, P->n_big_pairs, P->det_H, P->det_g));
   LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
   P->launches += ex.launches;
   P->det_ready = true;
@@ -762,11 +666,9 @@ void lvba_lidar_default_opts(lvba_lidar_opts* o) {
 }
 
 int lvba_lidar_create(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
-                      const double* clusters, const double* poses, int32_t device, lvba_lidar_problem** out) {
-  try { return lvba::lidar_create_impl(W, V, vox_ptr, pose_idx, clusters, poses, device, out); }
-  catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
-  catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_lidar_create"); }
-}
+                      const double* clusters, const double* poses, int32_t device, lvba_lidar_problem** out) LVBA_ABI_BEGIN {
+  return lvba::lidar_create_impl(W, V, vox_ptr, pose_idx, clusters, poses, device, out);
+} LVBA_ABI_END("lvba_lidar_create")
 
 int lvba_lidar_destroy(lvba_lidar_problem* p) LVBA_ABI_BEGIN {
   if (!p) return LVBA_OK;
@@ -894,23 +796,19 @@ int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env
 } LVBA_ABI_END("lvba_lidar_counts")
 
 int lvba_lidar_lm(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx, const double* clusters,
-                  double* poses, const lvba_lidar_opts* opts, lvba_summary* summary) {
+                  double* poses, const lvba_lidar_opts* opts, lvba_summary* summary) LVBA_ABI_BEGIN {
   const double t0 = lvba::wall_ms();
   lvba_lidar_opts o;
   if (opts) o = *opts; else lvba_lidar_default_opts(&o);
   lvba_lidar_problem* p = nullptr;
-  int rc;
-  try { rc = lvba::lidar_create_impl(W, V, vox_ptr, pose_idx, clusters, poses, o.device, &p, 0, nullptr, nullptr, /*keep_structure=*/false); }
-  catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
-  catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_lidar_lm"); }
-  if (rc != LVBA_OK) return rc;
+  LVBA_TRY(lvba::lidar_create_impl(W, V, vox_ptr, pose_idx, clusters, poses, o.device, &p, 0, nullptr, nullptr, /*keep_structure=*/false));
   return lvba::lm_one_shot(p, o, V > 0, lvba_lidar_reset_lm, lvba_lidar_iterate, lvba_lidar_destroy,
                            [&] { return lvba_lidar_get_poses(p, poses); }, t0, summary);     // x_stats written back only on success
-}
+} LVBA_ABI_END("lvba_lidar_lm")
 
 int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
                         const double* clusters, double* poses, int32_t min_voxels_per_pose, const lvba_lidar_opts* opts,
-                        lvba_summary* summaries, lvba_summary* total) {
+                        lvba_summary* summaries, lvba_summary* total) LVBA_ABI_BEGIN {
   const double t0 = lvba::wall_ms();
   if (n_windows <= 0 || !win_ptr) return lvba::fail(LVBA_ERR_INVALID_ARG, "n_windows=%d must be positive and win_ptr non-null", n_windows);
   if (win_ptr[0] != 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "win_ptr[0] must be 0");
@@ -920,12 +818,8 @@ int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, co
   lvba_lidar_opts o;
   if (opts) o = *opts; else lvba_lidar_default_opts(&o);
   lvba_lidar_problem* p = nullptr;
-  int rc;
-  try { rc = lvba::lidar_create_impl(win_ptr[n_windows], V, vox_ptr, pose_idx, clusters, poses, o.device, &p, n_windows, win_ptr); }
-  catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
-  catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_lidar_lm_batch"); }
-  if (rc != LVBA_OK) return rc;
+  LVBA_TRY(lvba::lidar_create_impl(win_ptr[n_windows], V, vox_ptr, pose_idx, clusters, poses, o.device, &p, n_windows, win_ptr));
   return lvba::lidar_batch_one_shot(p, o, min_voxels_per_pose, poses, summaries, total, t0, "lvba_lidar_lm_batch");
-}
+} LVBA_ABI_END("lvba_lidar_lm_batch")
 
 }  // extern "C"

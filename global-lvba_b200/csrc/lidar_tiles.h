@@ -27,6 +27,8 @@ namespace tiles {
 
 constexpr int kTileSlots = 256;              // slots (threads) per tile CTA of the Hessian build (faster than 512 on the H100)
 constexpr int kMaxVoxPerTile = kTileSlots / 2;
+constexpr int kSlots = 128;                  // slots (threads) per batch CTA of the residual pass and of the visual kernels; the most
+                                             // poses a voxel of the tiles may have (more: lidar_big.h)
 
 // The voxels `in[0..n)` (all voxels 0..n-1 when `in` is null), stably ordered by their lowest pose index (pose_idx is ascending
 // inside a voxel), as a local CSR: slot0[i] = first slot of local voxel i in the caller's arrays, l_vox_ptr[i] = its first local

@@ -83,9 +83,6 @@ inline int select_device(int device) {
   return LVBA_OK;
 }
 
-// ---------------------------------------------------------------- host parallel loop (symbolic set-up)
-constexpr int kMaxSetupThreads = 8;
-
 // ---------------------------------------------------------------- device memory pool
 // cudaMalloc / cudaFree cost milliseconds each (cudaFree also synchronises the device); the one-shot ABI calls
 // create and destroy ~40 buffers per call.  Freed buffers are therefore parked in a per-device, size-bucketed
@@ -261,6 +258,25 @@ inline double wall_ms() {
   using namespace std::chrono;
   return duration<double, std::milli>(steady_clock::now().time_since_epoch()).count();
 }
+// LVBA_SETUP_TIMING=1: the host laps of a set-up on stderr, one line "[tag] what  ms" per lap, each taken once the work queued
+// on `stream` (and on `also`, when given) is done
+struct SetupLaps {
+  const char* tag; int width; cudaStream_t stream; double prev; bool on;
+  SetupLaps(const char* tag_, int width_, cudaStream_t stream_, double t0)
+      : tag(tag_), width(width_), stream(stream_), prev(t0), on(getenv("LVBA_SETUP_TIMING") != nullptr) {}
+  void operator()(const char* what, cudaStream_t also = nullptr) {
+    if (!on) return;
+    if (also) cudaStreamSynchronize(also);
+    cudaStreamSynchronize(stream);
+    host(what);
+  }
+  void host(const char* what) {                                // a lap of host work only: no synchronisation
+    if (!on) return;
+    const double t = wall_ms();
+    fprintf(stderr, "[%s] %-*s %8.2f ms\n", tag, width, what, t - prev);
+    prev = t;
+  }
+};
 
 // ---------------------------------------------------------------- LM summaries and the one-shot calls
 // *s from the LM counts, costs and damping of a call; with `ms` (collected PhaseTimers) also its phase times, wall time

@@ -13,6 +13,8 @@
 
 namespace lvba {
 
+constexpr int kMaxSetupThreads = 8;      // the most threads of a parallel_chunks region (its `worker` is below this)
+
 // fn(begin, end, worker) over [0, n) split into contiguous chunks on up to 8 threads.  The set-up of a one-shot call
 // (validation, envelope structure, gathers) is a few milliseconds of host loops next to ~15 ms of device work, and a call has
 // several of them: the helpers are a PERSISTENT pool (created on first use, parked on a condition variable between regions) —
@@ -83,7 +85,7 @@ class SetupPool {
 template <class Fn>
 inline void parallel_chunks(int64_t n, int64_t min_chunk, Fn fn) {
   unsigned hw = std::thread::hardware_concurrency();
-  int nt = (int)std::min<int64_t>(std::min<unsigned>(hw ? hw : 1u, 8u), std::max<int64_t>(1, n / std::max<int64_t>(min_chunk, 1)));
+  int nt = (int)std::min<int64_t>(std::min<unsigned>(hw ? hw : 1u, (unsigned)kMaxSetupThreads), std::max<int64_t>(1, n / std::max<int64_t>(min_chunk, 1)));
   if (nt <= 1) { fn((int64_t)0, n, 0); return; }
   SetupPool::get().run(nt, [&](int w) { fn(n * w / nt, n * (w + 1) / nt, w); });
 }

@@ -37,7 +37,7 @@ namespace lvba {
 
 using tiles::kVisTileSlots;
 using tiles::kMaxTrkPerTile;
-constexpr int kMaxTrkPerBatch = 128;
+using tiles::kMaxTrkPerBatch;
 constexpr int kVFStride = 37;      // Y(18) E(18) + pad
 
 // ------------------------------------------------------------------------------------------------

@@ -8,7 +8,7 @@
 #include "exec.cuh"
 #include "runtime.cuh"   // (pulls comm.cuh in)
 #include "visual.cuh"
-#include "visual_big.h"
+#include "visual_plan.h"
 
 namespace lvba {
 // the trust-region state of one solve (Ceres TrustRegionMinimizer + LevenbergMarquardtStrategy)
@@ -80,6 +80,10 @@ struct lvba_visual_problem {
     v.loss_px = loss_px; v.loss_pl = loss_pl; v.loss_a_px = loss_a_px; v.loss_a_pl = loss_a_pl;
     return v;
   }
+  // the tiles' CSR for the passes of visual_tiles.h (trk_pair: set by visual_tables)
+  lvba::tiles::VisTableIn table_in() const {
+    return lvba::tiles::VisTableIn{n_tiles, n_rows, env.nblocks, tile_trk.p, trk_ptr.p, obs_row.p, nullptr, env.d_first.p, env.d_row_start.p};
+  }
   lvba::vbig::View big_view() const { return lvba::vbig::View{(int64_t)n_big, (int64_t)Tv_small, big_pair_ptr.p, env.d_first.p, env.d_row_start.p}; }
   lvba::VisualState state() const { return lvba::VisualState{q.p, t.p, X.p}; }
   lvba::VisualState cand() const { return lvba::VisualState{qc.p, tc.p, Xc.p}; }
@@ -112,11 +116,6 @@ __global__ void visual_gather_kernel(long long Tv, const int* __restrict__ trk_i
   }
 }
 
-inline bool plane_valid(const double* p) {   // has_valid_plane, src/lvba_system.cpp:1598
-  for (int i = 0; i < 4; ++i) if (!std::isfinite(p[i])) return false;
-  return std::fabs(p[0]) > 1e-6 || std::fabs(p[1]) > 1e-6 || std::fabs(p[2]) > 1e-6;
-}
-
 inline int visual_create_impl(int32_t M, int64_t T, const double* q, const double* t, const double* X,
                               const double* plane_nd, const int64_t* obs_ptr, const int32_t* obs_cam,
                               const float* obs_uv, const double intr[8], double sigma_px, double sigma_plane,
@@ -145,9 +144,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   }
   LVBA_TRY(select_device(device));
   const double t_begin = wall_ms();
-  const bool tlog = getenv("LVBA_SETUP_TIMING") != nullptr;
-  double tprev = t_begin;
-  auto lap = [&](const char* what) { if (tlog) { cudaStreamSynchronize(nullptr); const double tn = wall_ms(); fprintf(stderr, "[visual setup] %-26s %8.2f ms\n", what, tn - tprev); tprev = tn; } };
+  SetupLaps lap("visual setup", 26, nullptr, t_begin);
   std::unique_ptr<lvba_visual_problem> P(new lvba_visual_problem());
   P->M = M; P->T = T; P->fixed_cam = fixed_cam;
   for (int i = 0; i < 8; ++i) P->intr[i] = intr[i];
@@ -160,58 +157,15 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
 
   // ---- valid landmarks, active cameras (src/lvba_system.cpp:1582-1583, 1598-1603; SURVEY.md Q11)
   std::vector<int64_t> valid;
-  std::vector<char> cam_used(M, 0);
-  {
-    std::vector<char> is_valid((size_t)T, 0), used_w((size_t)kMaxSetupThreads * (size_t)M, 0);
-    parallel_chunks(T, 1 << 13, [&](int64_t i0, int64_t i1, int w) {
-      char* used = used_w.data() + (size_t)w * (size_t)M;
-      for (int64_t i = i0; i < i1; ++i) {
-        if (!plane_valid(plane_nd + 4 * i)) continue;
-        is_valid[(size_t)i] = 1;
-        for (int64_t q_ = obs_ptr[i]; q_ < obs_ptr[i + 1]; ++q_) used[obs_cam[q_]] = 1;
-      }
-    });
-    for (int w = 0; w < kMaxSetupThreads; ++w)
-      for (int c = 0; c < M; ++c) cam_used[c] |= used_w[(size_t)w * (size_t)M + c];
-    for (int64_t i = 0; i < T; ++i) if (is_valid[(size_t)i]) valid.push_back(i);
-  }
-  if (fixed_cam >= 0 && fixed_cam < M) cam_used[fixed_cam] = 0;
-  std::vector<int> row_of_cam(M, -1);
-  for (int c = 0; c < M; ++c) if (cam_used[c]) { row_of_cam[c] = (int)P->cam_of_row.size(); P->cam_of_row.push_back(c); }
+  std::vector<int> row_of_cam;
+  visual_rows(M, T, plane_nd, obs_ptr, obs_cam, fixed_cam, valid, row_of_cam, P->cam_of_row);
   P->n_rows = (int)P->cam_of_row.size();
   const int64_t Tv_all = (int64_t)valid.size();
 
   lap("valid landmarks / rows");
   // ---- envelope of the reduced camera system over ALL valid landmarks
-  std::vector<int> first_raw(std::max(P->n_rows, 1));
-  for (int r = 0; r < P->n_rows; ++r) first_raw[r] = r;
-  std::vector<int> min_row(Tv_all, 0), min_sys_row(Tv_all, 0);
-  {
-    const size_t nr = first_raw.size();
-    std::vector<int> first_w((size_t)kMaxSetupThreads * nr);
-    for (int w = 0; w < kMaxSetupThreads; ++w) std::copy(first_raw.begin(), first_raw.end(), first_w.begin() + (size_t)w * nr);
-    parallel_chunks(Tv_all, 1 << 13, [&](int64_t k0, int64_t k1, int w) {
-      int* fr = first_w.data() + (size_t)w * nr;
-      for (int64_t k = k0; k < k1; ++k) {
-        const int64_t i = valid[k];
-        int m = INT32_MAX, mcam = INT32_MAX;
-        for (int64_t q_ = obs_ptr[i]; q_ < obs_ptr[i + 1]; ++q_) {
-          const int r = row_of_cam[obs_cam[q_]];
-          if (r >= 0) m = std::min(m, r);
-          mcam = std::min(mcam, (int)obs_cam[q_]);
-        }
-        min_row[k] = (mcam == INT32_MAX) ? 0 : mcam;      // shard key: lowest camera index
-        min_sys_row[k] = (m == INT32_MAX) ? 0 : m;        // row-owned reduced system: lowest row of the landmark's clique
-        if (m == INT32_MAX) continue;
-        for (int64_t q_ = obs_ptr[i]; q_ < obs_ptr[i + 1]; ++q_) {
-          const int r = row_of_cam[obs_cam[q_]];
-          if (r >= 0) fr[r] = std::min(fr[r], m);
-        }
-      }
-    });
-    for (int w = 0; w < kMaxSetupThreads; ++w)
-      for (size_t r = 0; r < nr; ++r) first_raw[r] = std::min(first_raw[r], first_w[(size_t)w * nr + r]);
-  }
+  std::vector<int> min_row, min_sys_row;     // shard key: lowest camera; row-owned reduced system: lowest row of the clique
+  std::vector<int> first_raw = visual_first_rows(P->n_rows, valid.data(), Tv_all, obs_ptr, obs_cam, row_of_cam.data(), min_row, min_sys_row);
   if (P->n_rows > 0) {
     first_raw.resize(P->n_rows);
     LVBA_TRY(P->env.build(first_raw, s, &P->h2d));
@@ -222,46 +176,26 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   // ---- shard (SURVEY.md §8e): landmark -> owner of its lowest camera index
   Comm& cm = comm();
   std::vector<int64_t> own;                                    // indices into valid
-  for (int64_t k = 0; k < Tv_all; ++k)
-    if (!cm.active() || (P->solver.dist() ? P->solver.dist_owner(min_sys_row[k]) : shard_owner(min_row[k], M, cm.n_ranks)) == cm.rank)
-      own.push_back(k);
-  const int64_t Tv = (int64_t)own.size();
-  // the landmarks in the order of the lowest system row of their clique: the landmarks of a build tile then share cameras,
-  // whose S blocks and rows the tile sums on chip (visual_tiles.h).  Landmarks with more than kSlots observations go after all
-  // small ones, in the same order: they take the passes of visual_big.h.
-  std::vector<int64_t> mine((size_t)Tv);
-  int64_t Tv_small = 0;
-  {
-    std::vector<int> key((size_t)Tv);
-    for (int64_t j = 0; j < Tv; ++j) key[j] = min_sys_row[own[j]];
-    const std::vector<int64_t> order = tiles::order_by_key(std::max(P->n_rows, 1), key.data(), Tv);
-    auto is_big = [&](int64_t i) { return obs_ptr[i + 1] - obs_ptr[i] > kSlots; };
-    for (int64_t j = 0; j < Tv; ++j) if (!is_big(valid[own[order[j]]])) mine[Tv_small++] = valid[own[order[j]]];
-    int64_t w = Tv_small;
-    for (int64_t j = 0; j < Tv; ++j) if (is_big(valid[own[order[j]]])) mine[w++] = valid[own[order[j]]];
-  }
+  if (cm.active())
+    for (int64_t k = 0; k < Tv_all; ++k)
+      if ((P->solver.dist() ? P->solver.dist_owner(min_sys_row[k]) : shard_owner(min_row[k], M, cm.n_ranks)) == cm.rank) own.push_back(k);
+  VisualLayout L;                                              // landmark order and list, batches and tiles
+  visual_layout(P->n_rows, valid.data(), Tv_all, cm.active() ? &own : nullptr, min_sys_row.data(), obs_ptr, obs_cam, row_of_cam.data(), L);
+  const int64_t Tv = L.Tv, Tv_small = L.Tv_small;
   P->Tv = Tv;
   P->Tv_small = Tv_small;
   P->n_big = Tv - Tv_small;
-  std::vector<int> trk_ptr(Tv + 1, 0), trk_id(Tv);
-  for (int64_t k = 0; k < Tv; ++k) {
-    trk_id[k] = (int)mine[k];
-    trk_ptr[k + 1] = trk_ptr[k] + (int)(obs_ptr[mine[k] + 1] - obs_ptr[mine[k]]);
-  }
-  const long long nnz = trk_ptr[Tv];
-  P->nnz = nnz;
+  P->nnz = L.nnz;
   lap("landmark list");
-  // ---- back-substitution / cost batches (<= kSlots observations) and build tiles (<= kVisTileSlots observations)
-  const std::vector<int> batch_trk = tiles::cut_ranges(Tv_small, trk_ptr.data(), nullptr, kSlots, kMaxTrkPerBatch);
-  const std::vector<int> tile_trk = tiles::cut_ranges(Tv_small, trk_ptr.data(), nullptr, kVisTileSlots, kMaxTrkPerTile);
-  P->n_batches = (int)batch_trk.size() - 1;
-  P->n_tiles = (int)tile_trk.size() - 1;
+  P->n_batches = (int)L.batch_trk.size() - 1;
+  P->n_tiles = (int)L.tile_trk.size() - 1;
   lap("batches + tiles");
 
   // ---- upload the caller's arrays as they are; gather the per-observation arrays and build the destination table on the device
-  LVBA_TRY(P->trk_ptr.upload(trk_ptr, s, &P->h2d));
-  LVBA_TRY(P->batch_trk.upload(batch_trk, s, &P->h2d));
-  LVBA_TRY(P->tile_trk.upload(tile_trk, s, &P->h2d));
+  LVBA_TRY(P->trk_ptr.upload(L.trk_ptr, s, &P->h2d));
+  LVBA_TRY(P->batch_trk.upload(L.batch_trk, s, &P->h2d));
+  LVBA_TRY(P->tile_trk.upload(L.tile_trk, s, &P->h2d));
+  P->n_pairs = 0;
   if (Tv > 0) {
     const int64_t nnz_all = obs_ptr[T];
     DevBuf<long long> d_obs_ptr;
@@ -274,62 +208,26 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
     LVBA_TRY(d_raw_uv.upload(reinterpret_cast<const float2*>(obs_uv), (size_t)nnz_all, s, &P->h2d));
     LVBA_TRY(d_raw_plane.upload(plane_nd, (size_t)T * 4, s, &P->h2d));
     LVBA_TRY(d_row_of_cam.upload(row_of_cam, s, &P->h2d));
-    LVBA_TRY(P->trk_id.upload(trk_id, s, &P->h2d));
-    LVBA_TRY(P->obs_cam.alloc((size_t)nnz)); LVBA_TRY(P->obs_row.alloc((size_t)nnz)); LVBA_TRY(P->obs_uv.alloc((size_t)nnz));
+    LVBA_TRY(P->trk_id.upload(L.trk_id, s, &P->h2d));
+    LVBA_TRY(P->obs_cam.alloc((size_t)P->nnz)); LVBA_TRY(P->obs_row.alloc((size_t)P->nnz)); LVBA_TRY(P->obs_uv.alloc((size_t)P->nnz));
     LVBA_TRY(P->plane.alloc((size_t)Tv * 4));
     visual_gather_kernel<<<(unsigned)((Tv + 127) / 128), 128, 0, s>>>(Tv, P->trk_id.p, P->trk_ptr.p, d_obs_ptr.p, d_raw_cam.p, d_raw_uv.p,
                                                                      d_raw_plane.p, d_row_of_cam.p, P->obs_cam.p, P->obs_row.p, P->obs_uv.p, P->plane.p);
     LVBA_CUDA(cudaGetLastError());
     ++P->launches;
-    if (Tv_small > 0) {                                        // the destination table covers the small landmarks only
-      CudaExec ex;
-      ex.stream = s;
-      DevBuf<long long> d_pair_cnt, d_trk_pair;                // ordered observation pairs before every local landmark
-      LVBA_TRY(d_pair_cnt.alloc((size_t)Tv_small + 1));
-      LVBA_TRY(d_trk_pair.alloc((size_t)Tv_small + 1));
-      LVBA_TRY(ex.for_each(Tv_small + 1, tiles::VisPairCountF{P->trk_ptr.p, Tv_small, d_pair_cnt.p}));
-      LVBA_TRY(ex.exclusive_scan(d_pair_cnt.p, d_trk_pair.p, Tv_small + 1));
-      long long n_ordered = 0;
-      for (int64_t k = 0; k < Tv_small; ++k) n_ordered += (long long)(trk_ptr[k + 1] - trk_ptr[k]) * (trk_ptr[k + 1] - trk_ptr[k] - 1);
-      const tiles::VisTableIn tin{P->n_tiles, P->n_rows, P->env.nblocks, P->tile_trk.p, P->trk_ptr.p, P->obs_row.p, d_trk_pair.p,
-                                  P->env.d_first.p, P->env.d_row_start.p};
-      LVBA_TRY(tiles::sort_runs(ex, n_ordered, P->n_tiles, (uint64_t)P->env.nblocks, tiles::VisPairKeyF{tin}, P->prun));
-      LVBA_TRY(tiles::sort_runs(ex, (int64_t)trk_ptr[Tv_small], P->n_tiles, (uint64_t)P->n_rows, tiles::ObsKeyF{tin}, P->drun));
-      int64_t np = 0;
-      LVBA_TRY(ex.fetch(&np, P->prun.run_ptr.p + P->prun.n_runs, 1));
-      P->n_pairs = np;
-      P->launches += ex.launches;
-    }
+    CudaExec ex;                                               // the destination table covers the small landmarks only
+    ex.stream = s;
+    int64_t np = 0;
+    LVBA_TRY(visual_tables(ex, P->table_in(), Tv_small, L.n_ordered, L.trk_ptr[Tv_small], P->prun, P->drun, &np));
+    P->launches += ex.launches;
+    P->n_pairs = np + L.big_pairs;
     if (P->n_big > 0) {
-      // pair items of the big landmarks (K (K - 1) each) and their camera-pair contributions: an unordered pair of observations
-      // of two distinct rows once, of one row in both orders, i.e. C(n, 2) + sum_row C(n_row, 2) over the n observations of
-      // non-constant cameras
-      std::vector<int64_t> bpp((size_t)P->n_big + 1, 0);
-      std::vector<int> rows;
-      for (int64_t b = 0; b < P->n_big; ++b) {
-        const int64_t i = mine[Tv_small + b], K = obs_ptr[i + 1] - obs_ptr[i];
-        bpp[b + 1] = bpp[b] + K * (K - 1);
-        rows.clear();
-        for (int64_t q_ = obs_ptr[i]; q_ < obs_ptr[i + 1]; ++q_) if (row_of_cam[obs_cam[q_]] >= 0) rows.push_back(row_of_cam[obs_cam[q_]]);
-        std::sort(rows.begin(), rows.end());
-        const long long n = (long long)rows.size();
-        long long contrib = n * (n - 1) / 2;
-        for (size_t a = 0; a < rows.size();) {
-          size_t e = a;
-          while (e < rows.size() && rows[e] == rows[a]) ++e;
-          contrib += (long long)(e - a) * (long long)(e - a - 1) / 2;
-          a = e;
-        }
-        P->n_pairs += contrib;
-      }
-      P->n_big_obs = nnz - trk_ptr[Tv_small];
-      P->n_big_pairs = bpp.back();
-      LVBA_TRY(P->big_pair_ptr.upload(bpp, s, &P->h2d));
+      P->n_big_obs = P->nnz - L.trk_ptr[Tv_small];
+      P->n_big_pairs = L.big_pair_ptr.back();
+      LVBA_TRY(P->big_pair_ptr.upload(L.big_pair_ptr, s, &P->h2d));
       LVBA_TRY(P->big_obs.alloc((size_t)P->n_big_obs * vbig::kObs));
       LVBA_TRY(P->big_params.alloc((size_t)P->n_big * kTrkParams));
     }
-  } else {
-    P->n_pairs = 0;
   }
   lap("device gather + destination table");
   if (P->n_rows > 0) LVBA_TRY(P->d_cam_of_row.upload(P->cam_of_row, s, &P->h2d));
@@ -368,36 +266,15 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   return LVBA_OK;
 }
 
-// Deterministic mode: the records of the build and their destinations.  Records of S: the tiles' pair runs, the tiles' row runs,
-// the big landmarks' observations, the big landmarks' ordered pairs; records of the camera rows: the tiles' row runs, the big
-// landmarks' observations.  Each set in its enumeration order, so that every destination's records come in ascending (tile, run)
-// order, then in item order.  Observations of constant cameras and pairs outside the lower envelope get a record without a
-// destination.
+// Deterministic mode: the records of the build and their destinations (visual_det_index), and the records of the column-norm pass
 inline int visual_det_setup(lvba_visual_problem* P) {
   if (P->det_ready) return LVBA_OK;
-  const int64_t npr = P->prun.n_runs, ndr = P->drun.n_runs;
-  const int64_t nS = npr + ndr + P->n_big_obs + P->n_big_pairs, nG = ndr + P->n_big_obs;
+  const int64_t nS = P->prun.n_runs + P->drun.n_runs + P->n_big_obs + P->n_big_pairs;
   if (nS >= (int64_t)1 << 32) return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode: %lld contributions to S (at most 2^32)", (long long)nS);
   CudaExec ex;
   ex.stream = P->stream;
-  LVBA_TRY(tiles::fixed_sum_alloc(P->det_S, nS, 36));
-  LVBA_TRY(tiles::fixed_sum_alloc(P->det_G, nG, 18));
-  LVBA_TRY(P->det_C.alloc((size_t)std::max<int64_t>(nG, 1) * 6));
-  if (P->n_tiles > 0) {
-    const tiles::VisTableIn tin{P->n_tiles, P->n_rows, P->env.nblocks, P->tile_trk.p, P->trk_ptr.p, P->obs_row.p, nullptr,
-                                P->env.d_first.p, P->env.d_row_start.p};
-    LVBA_TRY(ex.for_each(npr, tiles::VisPairRunDstF{tin, P->prun.tile_run.p, P->prun.run_ptr.p, P->prun.code.p, P->det_S.dst.p}));
-    LVBA_TRY(ex.for_each(ndr, tiles::ObsRunDstF{tin, P->drun.tile_run.p, P->drun.run_ptr.p, P->drun.code.p, P->det_S.dst.p + npr,
-                                                P->det_G.dst.p}));
-  }
-  if (P->n_big > 0) {
-    const VisualView vv = P->view();
-    const vbig::View bv = P->big_view();
-    LVBA_TRY(ex.for_each(P->n_big_obs, vbig::ObsDstF{vv, bv, P->env.nblocks, P->n_rows, P->det_S.dst.p + npr + ndr, P->det_G.dst.p + ndr}));
-    LVBA_TRY(ex.for_each(P->n_big_pairs, vbig::PairDstF{vv, bv, P->env.nblocks, P->det_S.dst.p + npr + ndr + P->n_big_obs}));
-  }
-  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_S, P->env.nblocks));
-  LVBA_TRY(tiles::fixed_sum_index(ex, P->det_G, P->n_rows));
+  LVBA_TRY(visual_det_index(ex, P->table_in(), P->prun, P->drun, P->view(), P->big_view(), P->n_big_obs, P->n_big_pairs, P->det_S, P->det_G));
+  LVBA_TRY(P->det_C.alloc((size_t)std::max<int64_t>(P->det_G.n_rec, 1) * 6));
   LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
   LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
   P->launches += ex.launches;
@@ -674,11 +551,9 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
                        const int64_t* obs_ptr, const int32_t* obs_cam, const float* obs_uv, const double intr[8],
-                       double sigma_px, double sigma_plane, int32_t fixed_cam, int32_t device, lvba_visual_problem** out) {
-  try { return lvba::visual_create_impl(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, device, out); }
-  catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
-  catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_visual_create"); }
-}
+                       double sigma_px, double sigma_plane, int32_t fixed_cam, int32_t device, lvba_visual_problem** out) LVBA_ABI_BEGIN {
+  return lvba::visual_create_impl(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, device, out);
+} LVBA_ABI_END("lvba_visual_create")
 
 int lvba_visual_destroy(lvba_visual_problem* p) LVBA_ABI_BEGIN {
   if (!p) return LVBA_OK;

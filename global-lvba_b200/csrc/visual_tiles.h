@@ -17,6 +17,7 @@ namespace tiles {
 
 constexpr int kVisTileSlots = 256;             // observations (threads) per tile CTA of the reduced camera system build
 constexpr int kMaxTrkPerTile = 128;            // landmarks per tile
+constexpr int kMaxTrkPerBatch = 128;           // landmarks per batch CTA (<= kSlots observations) of back-substitution and cost
 
 // 0..n-1 stably ordered by key[] in [0, n_keys)
 inline std::vector<int64_t> order_by_key(int n_keys, const int* key, int64_t n) {

@@ -177,9 +177,7 @@ int lvba_voxel_map_lookup(lvba_voxel_map* m, int64_t n, const double* X, double*
   auto& v = m->map;
   lvba::DevBuf<double> dX, dout;
   lvba::StreamDrain drain(v.ex.stream);
-  const bool tlog = getenv("LVBA_SETUP_TIMING") != nullptr;
-  double tprev = lvba::wall_ms();
-  auto lap = [&](const char* what) { if (tlog) { cudaStreamSynchronize(v.ex.stream); const double t = lvba::wall_ms(); fprintf(stderr, "[voxel lookup] %-18s %8.2f ms\n", what, t - tprev); tprev = t; } };
+  lvba::SetupLaps lap("voxel lookup", 18, v.ex.stream, lvba::wall_ms());
   LVBA_TRY(dX.upload(X, (size_t)n * 3, v.ex.stream));
   LVBA_TRY(dout.alloc((size_t)n * 4));
   lap("alloc + upload");
@@ -194,7 +192,7 @@ int lvba_voxel_map_lookup(lvba_voxel_map* m, int64_t n, const double* X, double*
 
 // tras_opt straight into path A: the map's plane voxels become a device-resident LiDAR problem.  Only the CSR index
 // arrays (12 B per cluster) visit the host, for the symbolic analysis; the 80-byte cluster records stay in HBM.
-int lvba_voxel_map_lidar_create(lvba_voxel_map* m, const double* poses, lvba_lidar_problem** out) {
+int lvba_voxel_map_lidar_create(lvba_voxel_map* m, const double* poses, lvba_lidar_problem** out) LVBA_ABI_BEGIN {
   if (!m || !poses || !out) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
   *out = nullptr;
   LVBA_CUDA(cudaSetDevice(m->device));
@@ -206,11 +204,8 @@ int lvba_voxel_map_lidar_create(lvba_voxel_map* m, const double* poses, lvba_lid
   LVBA_CUDA(cudaMemcpyAsync(vox_ptr.data(), v.vox_ptr.p, vox_ptr.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, v.ex.stream));
   if (v.nnz) LVBA_CUDA(cudaMemcpyAsync(pose_idx.data(), v.vox_pose.p, pose_idx.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, v.ex.stream));
   LVBA_CUDA(cudaStreamSynchronize(v.ex.stream));
-  try {
-    return lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, out, 0, nullptr,
-                                   v.vox_cluster.p);
-  } catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
-}
+  return lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, out, 0, nullptr, v.vox_cluster.p);
+} LVBA_ABI_END("lvba_voxel_map_lidar_create")
 
 // cut_voxel + recut (the map) -> tras_opt + BALM2::damping_iter (this call).  min_voxels_per_pose: the caller-side skip of
 // src/lvba_system.cpp:262-266 (`plvec_voxels.size() < 3 * x_win.size()`): LVBA_OK, LVBA_TERM_SKIPPED, poses untouched.
@@ -238,7 +233,7 @@ int lvba_voxel_map_lidar_lm(lvba_voxel_map* m, double* poses, int32_t min_voxels
 // The whole window stage of runWindowBA (src/lvba_system.cpp:232-266) from a windowed map: tras_opt + damping_iter of every
 // window in one batched solve (lvba_lidar_lm_batch), the clusters never leaving the device.
 int lvba_voxel_map_lidar_lm_batch(lvba_voxel_map* m, double* poses, int32_t min_voxels_per_pose, const lvba_lidar_opts* opts,
-                                  lvba_summary* summaries, lvba_summary* total) {
+                                  lvba_summary* summaries, lvba_summary* total) LVBA_ABI_BEGIN {
   if (!m || !poses) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
   if (min_voxels_per_pose < 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "min_voxels_per_pose must be >= 0");
   auto& v = m->map;
@@ -254,13 +249,9 @@ int lvba_voxel_map_lidar_lm_batch(lvba_voxel_map* m, double* poses, int32_t min_
   if (v.nnz) LVBA_CUDA(cudaMemcpyAsync(pose_idx.data(), v.vox_pose.p, pose_idx.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, v.ex.stream));
   LVBA_CUDA(cudaStreamSynchronize(v.ex.stream));
   lvba_lidar_problem* p = nullptr;
-  int rc;
-  try { rc = lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, &p, v.n_windows, m->win_ptr.data(), v.vox_cluster.p); }
-  catch (const std::bad_alloc&) { return lvba::fail(LVBA_ERR_NOMEM, "host allocation failed"); }
-  catch (...) { return lvba::fail(LVBA_ERR_INVALID_ARG, "unexpected exception in lvba_voxel_map_lidar_lm_batch"); }
-  if (rc != LVBA_OK) return rc;
+  LVBA_TRY(lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, &p, v.n_windows, m->win_ptr.data(), v.vox_cluster.p));
   return lvba::lidar_batch_one_shot(p, o, min_voxels_per_pose, poses, summaries, total, t0, "lvba_voxel_map_lidar_lm_batch");
-}
+} LVBA_ABI_END("lvba_voxel_map_lidar_lm_batch")
 
 int lvba_voxel_map_destroy(lvba_voxel_map* m) LVBA_ABI_BEGIN {
   if (!m) return LVBA_OK;

@@ -1,36 +1,32 @@
 // det_emu.cpp — TEST INFRASTRUCTURE: the fixed-order sums of the deterministic LiDAR build (lidar_tiles.h FixedSum / GatherF,
 // the record passes of lidar_big.h) run through the host policy, so that tests/test_deterministic_emu.py can check them without a
-// GPU.  The same set-up as lidar_create_impl + lidar_det_setup: voxels with more than kSmallMax slots go to the big-voxel passes,
-// the others into tiles; records of H = [pair runs][pose runs][big slots][big pairs], of g = [pose runs][big slots].  Never part
-// of the product.  emu_vdet_step does the same for the big-landmark passes of the visual build (visual_big.h).
+// GPU.  It calls the library's own set-up (global-lvba_b200/csrc/lidar_plan.h: lidar_layout, lidar_tables, lidar_det_index) and
+// does only the per-slot gathers of poses and cluster records itself, which the library does on the device: voxels with more than
+// kSlots slots go to the big-voxel passes, the others into tiles; records of H = [pair runs][pose runs][big slots][big pairs],
+// of g = [pose runs][big slots].  Never part of the product.  emu_vdet_step does the same for the big-landmark passes of the
+// visual build (visual_plan.h visual_det_index, visual_big.h).
 #include <cmath>
 #include <cstring>
 #include <vector>
 
-#include "../../global-lvba_b200/csrc/lidar_big.h"
-#include "../../global-lvba_b200/csrc/lidar_tiles.h"
-#include "../../global-lvba_b200/csrc/visual_big.h"
+#include "../../global-lvba_b200/csrc/lidar_plan.h"
+#include "../../global-lvba_b200/csrc/visual_plan.h"
 #include "host_exec.h"
 
 using namespace lvba;
-
-constexpr int kSmallMax = 128;     // kSlots of lidar.cuh
 
 struct DetOut {
   int W = 0;
   long long nblocks = 0;
   const int* first = nullptr;
   const long long* row_start = nullptr;
-  // tiles of the small voxels
-  std::vector<int> vox_ptr, pidx, tile_vox;
+  LidarLayout L;
+  std::vector<int> pidx;                 // pose of every local slot of the tiles
+  std::vector<double> big_cl;            // AoS records of the big voxels' slots
   tiles::Runs<HostExec> prun, drun;
-  // big voxels (caller order), AoS records
-  std::vector<int64_t> big_vox_ptr{0}, big_pair_ptr{0};
-  std::vector<int32_t> big_pose;
-  std::vector<double> big_cl;
   tiles::FixedSum<HostExec> H, g;
   big::View view() const {
-    return big::View{(int64_t)big_vox_ptr.size() - 1, big_vox_ptr.data(), big_pose.data(), big_cl.data(), big_pair_ptr.data(), first, row_start};
+    return big::View{(int64_t)L.big_vox.size(), L.big_vox_ptr.data(), L.big_pose.data(), big_cl.data(), L.big_pair_ptr.data(), first, row_start};
   }
 };
 
@@ -38,46 +34,16 @@ extern "C" void* emu_det_build(int W, int64_t V, const int64_t* vox_ptr, const i
                                const int* first, const long long* row_start, long long nblocks) {
   DetOut* o = new DetOut;
   o->W = W; o->nblocks = nblocks; o->first = first; o->row_start = row_start;
-  std::vector<int64_t> small;
-  for (int64_t a = 0; a < V; ++a) {
-    const int64_t K = vox_ptr[a + 1] - vox_ptr[a];
-    if (K <= kSmallMax) { small.push_back(a); continue; }
-    for (int64_t q = vox_ptr[a]; q < vox_ptr[a + 1]; ++q) {
-      o->big_pose.push_back(pose_idx[q]);
-      o->big_cl.insert(o->big_cl.end(), clusters + 10 * q, clusters + 10 * q + 10);
-    }
-    o->big_vox_ptr.push_back((int64_t)o->big_pose.size());
-    o->big_pair_ptr.push_back(o->big_pair_ptr.back() + K * (K - 1) / 2);
-  }
-  const int64_t Vl = (int64_t)small.size();
-  std::vector<int> slot0;
-  tiles::order_by_lowest_pose(W, small.data(), Vl, vox_ptr, pose_idx, slot0, o->vox_ptr);
-  for (int64_t i = 0; i < Vl; ++i)
-    for (int q = 0; q < o->vox_ptr[(size_t)i + 1] - o->vox_ptr[(size_t)i]; ++q) o->pidx.push_back(pose_idx[slot0[(size_t)i] + q]);
-  o->tile_vox = tiles::cut_ranges(Vl, o->vox_ptr.data(), nullptr, tiles::kTileSlots, tiles::kMaxVoxPerTile);
+  LidarLayout& L = o->L;
+  lidar_layout(W, V, vox_ptr, pose_idx, nullptr, 0, nullptr, L);
+  for (size_t i = 0; i + 1 < L.l_vox_ptr.size(); ++i)
+    for (int q = 0; q < L.l_vox_ptr[i + 1] - L.l_vox_ptr[i]; ++q) o->pidx.push_back(pose_idx[L.slot0[i] + q]);
+  for (int q : L.big_src) o->big_cl.insert(o->big_cl.end(), clusters + 10 * (int64_t)q, clusters + 10 * (int64_t)q + 10);
   HostExec ex;
-  const int64_t n_tiles = (int64_t)o->tile_vox.size() - 1;
-  std::vector<long long> cnt((size_t)Vl + 1), vox_pair((size_t)Vl + 1);
-  ex.for_each(Vl + 1, tiles::PairCountF{o->vox_ptr.data(), Vl, cnt.data()});
-  ex.exclusive_scan(cnt.data(), vox_pair.data(), Vl + 1);
-  const tiles::TableIn in{n_tiles, W, nblocks, o->tile_vox.data(), o->vox_ptr.data(), o->pidx.data(), vox_pair.data(), first, row_start};
-  if (n_tiles > 0 && (tiles::build_runs(ex, in, false, vox_pair[(size_t)Vl], o->prun) || tiles::build_runs(ex, in, true, o->vox_ptr[(size_t)Vl], o->drun))) {
-    delete o;
-    return nullptr;
-  }
-  // lidar_det_setup
-  const int64_t npr = o->prun.n_runs, ndr = o->drun.n_runs;
-  const int64_t nbs = (int64_t)o->big_pose.size(), nbp = o->big_pair_ptr.back();
-  tiles::fixed_sum_alloc(o->H, npr + ndr + nbs + nbp, 36);
-  tiles::fixed_sum_alloc(o->g, ndr + nbs, 6);
-  if (n_tiles > 0) {
-    ex.for_each(npr, tiles::PairRunDstF{in, o->prun.tile_run.p, o->prun.run_ptr.p, o->prun.code.p, o->H.dst.p});
-    ex.for_each(ndr, tiles::SlotRunDstF{in, o->drun.tile_run.p, o->drun.run_ptr.p, o->drun.code.p, o->H.dst.p + npr, o->g.dst.p});
-  }
-  const big::View bv = o->view();
-  ex.for_each(nbs, big::SlotDstF{bv, o->H.dst.p + npr + ndr, o->g.dst.p + ndr});
-  ex.for_each(nbp, big::PairDstF{bv, o->H.dst.p + npr + ndr + nbs});
-  if (tiles::fixed_sum_index(ex, o->H, nblocks) || tiles::fixed_sum_index(ex, o->g, W)) {
+  const tiles::TableIn in{(int64_t)L.tile_vox.size() - 1, W, nblocks, L.tile_vox.data(), L.l_vox_ptr.data(), o->pidx.data(), nullptr,
+                          first, row_start};
+  if (lidar_tables(ex, in, (int64_t)L.slot0.size(), L.n_pairs, L.nnz, o->prun, o->drun) ||
+      lidar_det_index(ex, in, o->prun, o->drun, o->view(), (int64_t)L.big_src.size(), L.big_pair_ptr.back(), o->H, o->g)) {
     delete o;
     return nullptr;
   }
@@ -94,18 +60,18 @@ extern "C" int64_t emu_det_get(void* h, int which, void* dst) {
     return (int64_t)n;
   };
   switch (which) {
-    case 0: return out(o->vox_ptr.data(), o->vox_ptr.size());
+    case 0: return out(o->L.l_vox_ptr.data(), o->L.l_vox_ptr.size());
     case 1: return out(o->pidx.data(), o->pidx.size());
-    case 2: return out(o->tile_vox.data(), o->tile_vox.size());
+    case 2: return out(o->L.tile_vox.data(), o->L.tile_vox.size());
     case 3: return out(o->prun.code.p, o->prun.code.n);
     case 4: return out(o->drun.code.p, o->drun.code.n);
     case 5: return out(o->prun.run_ptr.p, o->prun.run_ptr.n);
     case 6: return out(o->prun.tile_run.p, o->prun.tile_run.n);
     case 7: return out(o->drun.run_ptr.p, o->drun.run_ptr.n);
     case 8: return out(o->drun.tile_run.p, o->drun.tile_run.n);
-    case 9: return out(o->big_vox_ptr.data(), o->big_vox_ptr.size());
-    case 10: return out(o->big_pair_ptr.data(), o->big_pair_ptr.size());
-    case 11: return out(o->big_pose.data(), o->big_pose.size());
+    case 9: return out(o->L.big_vox_ptr.data(), o->L.big_vox_ptr.size());
+    case 10: return out(o->L.big_pair_ptr.data(), o->L.big_pair_ptr.size());
+    case 11: return out(o->L.big_pose.data(), o->L.big_pose.size());
     case 12: return out(o->H.dst.p, (size_t)o->H.n_rec);
     case 13: return out(o->H.by_dst.code.p, (size_t)o->H.n_rec);
     case 14: return out(o->H.by_dst.run_ptr.p, (size_t)o->H.by_dst.n_runs + 1);
@@ -125,7 +91,7 @@ extern "C" void emu_det_run(void* h, const double* tile_H, const double* tile_g,
   HostExec ex;
   const big::View bv = o->view();
   const int64_t npr = o->prun.n_runs, ndr = o->drun.n_runs;
-  const int64_t nb = bv.n_vox, nbs = (int64_t)o->big_pose.size(), nbp = o->big_pair_ptr.back();
+  const int64_t nb = bv.n_vox, nbs = (int64_t)o->L.big_pose.size(), nbp = o->L.big_pair_ptr.back();
   std::vector<double> params((size_t)nb * big::kParams), res((size_t)nb), feat((size_t)nbs * big::kFeat);
   std::memset(H, 0, (size_t)o->nblocks * 36 * sizeof(double));
   std::memset(g, 0, (size_t)o->W * 6 * sizeof(double));
@@ -175,13 +141,10 @@ extern "C" void emu_vdet_step(int n_rows, int64_t Tv, const int* trk_ptr, const 
   obs.alloc((size_t)nnz * vbig::kObs); params.alloc((size_t)Tv * kTrkParams); cost.alloc((size_t)Tv); gmax.alloc((size_t)Tv);
   tiles::FixedSum<HostExec> fS, fG;
   if (det) {                                                   // visual_det_setup without tiles
-    tiles::fixed_sum_alloc(fS, nnz + np, 36);
-    tiles::fixed_sum_alloc(fG, nnz, 18);
+    const tiles::VisTableIn no_tiles{0, n_rows, nblocks, nullptr, trk_ptr, obs_row, nullptr, first, row_start};
+    const tiles::Runs<HostExec> no_runs;
+    visual_det_index(ex, no_tiles, no_runs, no_runs, vv, bv, nnz, np, fS, fG);
     C.alloc((size_t)std::max<int64_t>(nnz, 1) * 6);
-    ex.for_each(nnz, vbig::ObsDstF{vv, bv, nblocks, n_rows, fS.dst.p, fG.dst.p});
-    ex.for_each(np, vbig::PairDstF{vv, bv, nblocks, fS.dst.p + nnz});
-    tiles::fixed_sum_index(ex, fS, nblocks);
-    tiles::fixed_sum_index(ex, fG, n_rows);
   }
   for (double* a : {cam_colsq0, rhs, cam_colsq, cam_grad}) std::memset(a, 0, (size_t)n_rows * 6 * sizeof(double));
   std::memset(S, 0, (size_t)nblocks * 36 * sizeof(double));

@@ -51,9 +51,12 @@ FIELDS = [("order", np.int64), ("vox_ptr", np.int32), ("pidx", np.int32), ("tile
 def run(emu, vox_ptr, pose_idx, W, pose_grp=None, max_slots=0, max_vox=0):
     vp = np.ascontiguousarray(vox_ptr, np.int64); pi = np.ascontiguousarray(pose_idx, np.int32)
     first, row_start = envelope_of(vp, pi, W)
-    grp = None if pose_grp is None else np.ascontiguousarray(pose_grp, np.int32)
+    n_grp = 0 if pose_grp is None else int(np.max(pose_grp)) + 1                 # pose_grp: consecutive windows 0, 1, ...
+    grp_ptr = np.zeros(n_grp + 1, np.int32)
+    if n_grp:
+        grp_ptr[1:] = np.cumsum(np.bincount(pose_grp, minlength=n_grp))
     h = emu.emu_tiles_build(ctypes.c_int(W), ctypes.c_int64(len(vp) - 1), vp.ctypes.data_as(P(ctypes.c_int64)), pi.ctypes.data_as(P(ctypes.c_int32)),
-                            None if grp is None else grp.ctypes.data_as(P(ctypes.c_int32)), first.ctypes.data_as(P(ctypes.c_int)),
+                            ctypes.c_int(n_grp), grp_ptr.ctypes.data_as(P(ctypes.c_int32)), first.ctypes.data_as(P(ctypes.c_int)),
                             row_start.ctypes.data_as(P(ctypes.c_longlong)), ctypes.c_longlong(int(row_start[-1])), ctypes.c_int(max_slots), ctypes.c_int(max_vox))
     assert h
     out = {}

@@ -34,14 +34,14 @@ def emu(tmp_path_factory):
 
 
 def rows_of(obs_cam, M, fixed_cam):
-    """System row of every observation: the active cameras in index order, -1 for the fixed camera."""
+    """System row of every camera: the active cameras in index order, -1 for the fixed camera."""
     used = np.zeros(M, bool)
     used[obs_cam] = True
     if 0 <= fixed_cam < M:
         used[fixed_cam] = False
     row_of_cam = np.full(M, -1, np.int64)
     row_of_cam[used] = np.arange(used.sum())
-    return row_of_cam[obs_cam].astype(np.int32), int(used.sum())
+    return row_of_cam.astype(np.int32), int(used.sum())
 
 
 def envelope_of(obs_ptr, row, n):
@@ -62,11 +62,11 @@ FIELDS = [("order", np.int64), ("trk_ptr", np.int32), ("row", np.int32), ("tile_
           ("prun", np.int64), ("ptile", np.int64), ("dcode", np.uint32), ("drun", np.int64), ("dtile", np.int64)]
 
 
-def run(emu, obs_ptr, row, n_rows, max_slots=0, max_trk=0):
-    op = np.ascontiguousarray(obs_ptr, np.int64); rw = np.ascontiguousarray(row, np.int32)
-    first, row_start = envelope_of(op, rw, n_rows)
+def run(emu, obs_ptr, cam, row_of_cam, n_rows, max_slots=0, max_trk=0):
+    op = np.ascontiguousarray(obs_ptr, np.int64); cm = np.ascontiguousarray(cam, np.int32); rc = np.ascontiguousarray(row_of_cam, np.int32)
+    first, row_start = envelope_of(op, rc[cm], n_rows)
     h = emu.emu_vis_tiles_build(ctypes.c_int(n_rows), ctypes.c_int64(len(op) - 1), op.ctypes.data_as(P(ctypes.c_int64)),
-                                rw.ctypes.data_as(P(ctypes.c_int32)), first.ctypes.data_as(P(ctypes.c_int)),
+                                cm.ctypes.data_as(P(ctypes.c_int32)), rc.ctypes.data_as(P(ctypes.c_int32)), first.ctypes.data_as(P(ctypes.c_int)),
                                 row_start.ctypes.data_as(P(ctypes.c_longlong)), ctypes.c_longlong(int(row_start[-1])),
                                 ctypes.c_int(max_slots), ctypes.c_int(max_trk))
     assert h
@@ -79,11 +79,11 @@ def run(emu, obs_ptr, row, n_rows, max_slots=0, max_trk=0):
     return out, first
 
 
-def check(emu, obs_ptr, row, n_rows, max_slots=0, max_trk=0):
+def check(emu, obs_ptr, cam, row_of_cam, n_rows, max_slots=0, max_trk=0):
     S = max_slots or emu.emu_vis_tile_slots()
     NT = max_trk or emu.emu_vis_max_trk_per_tile()
-    t, first = run(emu, obs_ptr, row, n_rows, max_slots, max_trk)
-    obs_ptr = np.asarray(obs_ptr, np.int64); row = np.asarray(row)
+    t, first = run(emu, obs_ptr, cam, row_of_cam, n_rows, max_slots, max_trk)
+    obs_ptr = np.asarray(obs_ptr, np.int64); row = np.asarray(row_of_cam)[np.asarray(cam, np.int64)]
     T = len(obs_ptr) - 1
     # ---- landmark order: a stable sort by the lowest row >= 0 (0 when there is none); the local CSR follows it
     low = np.array([min([r for r in row[obs_ptr[a]:obs_ptr[a + 1]] if r >= 0], default=0) for a in range(T)])
@@ -164,17 +164,17 @@ def problem(seed, M=40, T=None, fixed_cam=0, shuffle=True):
         K = np.diff(op)[perm]
         cam = np.concatenate([rng.permutation(cam[op[a]:op[a + 1]]) for a in perm])
         op = np.zeros(len(perm) + 1, np.int64); op[1:] = np.cumsum(K)
-    row, n_rows = rows_of(cam, M, fixed_cam)
-    return op, row, n_rows
+    row_of_cam, n_rows = rows_of(cam, M, fixed_cam)
+    return op, cam, row_of_cam, n_rows
 
 
 @pytest.mark.parametrize("fixed_cam", [0, -1])
 def test_table_of_synthetic_problems(emu, fixed_cam):
-    op, row, n = problem(31, fixed_cam=fixed_cam)
-    check(emu, op, row, n)                                   # the library's tile size
-    check(emu, op, row, n, max_slots=32, max_trk=4)          # many small tiles
-    op, row, n = problem(32, fixed_cam=fixed_cam, shuffle=False)
-    check(emu, op, row, n, max_slots=96, max_trk=48)
+    op, cam, rc, n = problem(31, fixed_cam=fixed_cam)
+    check(emu, op, cam, rc, n)                               # the library's tile size
+    check(emu, op, cam, rc, n, max_slots=32, max_trk=4)      # many small tiles
+    op, cam, rc, n = problem(32, fixed_cam=fixed_cam, shuffle=False)
+    check(emu, op, cam, rc, n, max_slots=96, max_trk=48)
 
 
 def test_camera_seen_twice_long_and_constant_landmarks(emu):
@@ -185,9 +185,9 @@ def test_camera_seen_twice_long_and_constant_landmarks(emu):
     tracks = [[5, 5, 9], [0, 0], [0], [3], list(rng.choice(M, 128)), [7, 0, 2, 7, 7], list(rng.choice(M, 40, replace=False)), [], [11, 4]]
     op = np.zeros(len(tracks) + 1, np.int64); op[1:] = np.cumsum([len(t) for t in tracks])
     cam = np.array([c for t in tracks for c in t], np.int64)
-    row, n = rows_of(cam, M, 0)
+    rc, n = rows_of(cam, M, 0)
     for S, NT in ((0, 0), (128, 64), (130, 2)):
-        t = check(emu, op, row, n, max_slots=S, max_trk=NT)
+        t = check(emu, op, cam, rc, n, max_slots=S, max_trk=NT)
         assert len(t["tile_trk"]) >= 2
 
 
