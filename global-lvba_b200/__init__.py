@@ -68,7 +68,8 @@ class VisualOpts(C.Structure):
                 ("jacobi_scaling", C.c_int32), ("device", C.c_int32), ("verbose", C.c_int32),
                 ("deterministic", C.c_int32),
                 ("reproj_loss", C.c_int32), ("reproj_loss_scale", C.c_double),
-                ("plane_loss", C.c_int32), ("plane_loss_scale", C.c_double)]
+                ("plane_loss", C.c_int32), ("plane_loss_scale", C.c_double),
+                ("cam_fixed", C.POINTER(C.c_uint8))]
 
 
 # lvba_loss_kind: the robust loss of the reprojection / plane residual blocks (VisualOpts.reproj_loss / plane_loss)
@@ -338,17 +339,33 @@ def env_blocks_to_dense(br, bc, blocks, n):
 
 
 # ------------------------------------------------------------------ B2: visual
-def visual_lm(q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam=0, opts=None):
-    """One-shot drop-in for the Ceres block of optimizeCameraPoses (lvba_system.cpp:1571-1656)."""
+def _with_cam_fixed(opts, cam_fixed, M):
+    """opts (None: the defaults) with cam_fixed set from a boolean mask of M cameras; returns (opts, the mask array the
+    pointer refers to, which the caller keeps alive for the call).  cam_fixed None leaves opts as they are."""
+    if cam_fixed is None:
+        return opts, None
+    m = np.ascontiguousarray(np.asarray(cam_fixed, bool), np.uint8)
+    if m.shape != (M,):
+        raise ValueError(f"cam_fixed has shape {m.shape}, expected ({M},)")
+    o = visual_default_opts() if opts is None else VisualOpts.from_buffer_copy(opts)
+    o.cam_fixed = _p(m, C.c_uint8)
+    return o, m
+
+
+def visual_lm(q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam=0, opts=None, cam_fixed=None):
+    """One-shot drop-in for the Ceres block of optimizeCameraPoses (lvba_system.cpp:1571-1656).  cam_fixed: boolean mask
+    [M] of further constant cameras (lvba_visual_opts::cam_fixed), or None."""
     lib = load_library()
     q = _f64(q).copy(); t = _f64(t).copy(); X = _f64(X).copy(); pl = _f64(plane_nd)
     op = np.ascontiguousarray(obs_ptr, np.int64); oc = np.ascontiguousarray(obs_cam, np.int32)
     uv = np.ascontiguousarray(obs_uv, np.float32); it = _f64(intr)
+    opts, mask = _with_cam_fixed(opts, cam_fixed, q.shape[0])
     s = Summary()
     _chk(lib.lvba_visual_lm(C.c_int32(q.shape[0]), C.c_int64(X.shape[0]), _p(q, C.c_double), _p(t, C.c_double),
                             _p(X, C.c_double), _p(pl, C.c_double), _p(op, C.c_int64), _p(oc, C.c_int32),
                             _p(uv, C.c_float), _p(it, C.c_double), C.c_double(sigma_px), C.c_double(sigma_plane),
                             C.c_int32(fixed_cam), C.byref(opts) if opts is not None else None, C.byref(s)))
+    del mask
     return q, t, X, s.as_dict()
 
 
@@ -409,8 +426,12 @@ class VisualProblem:
         _chk(self._lib.lvba_visual_get_system(self._h, _p(rhs, C.c_double), _p(blocks, C.c_double)))
         return cam, rhs, br, bc, blocks
 
-    def reset_lm(self, opts=None):
+    def reset_lm(self, opts=None, cam_fixed=None):
+        """lvba_visual_reset_lm; cam_fixed: boolean mask [M] of further constant cameras (a mask that differs from the
+        handle's re-plans it), or None for what opts.cam_fixed says."""
+        opts, mask = _with_cam_fixed(opts, cam_fixed, self.M)
         _chk(self._lib.lvba_visual_reset_lm(self._h, C.byref(opts) if opts is not None else None))
+        del mask
 
     def reset_state(self):
         _chk(self._lib.lvba_visual_reset_state(self._h))

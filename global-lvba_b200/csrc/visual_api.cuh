@@ -30,6 +30,9 @@ struct lvba_visual_problem {
   long long T = 0, Tv = 0, nnz = 0, n_pairs = 0;
   int n_rows = 0, n_batches = 0, n_tiles = 0, device = 0, fixed_cam = 0;
   std::vector<int> cam_of_row;
+  std::vector<uint8_t> cam_fixed;                   // constant cameras of the plan besides fixed_cam (lvba_visual_opts::cam_fixed,
+                                                    // one 0 / 1 per camera); empty: none
+  bool unusable = false;                            // a re-plan failed and so did restoring the previous one (visual_replan)
   cudaStream_t stream = nullptr;
   double intr[8];
   double sigma_px = 1, sigma_pl = 1;
@@ -116,10 +119,131 @@ __global__ void visual_gather_kernel(long long Tv, const int* __restrict__ trk_i
   }
 }
 
+// The constant cameras of lvba_visual_opts::cam_fixed as the handle keeps them: one 0 / 1 per camera, empty when no entry is
+// nonzero (an all-zero mask is no mask)
+inline std::vector<uint8_t> visual_mask(int M, const uint8_t* cam_fixed) {
+  std::vector<uint8_t> m;
+  if (!cam_fixed) return m;
+  bool any = false;
+  for (int c = 0; c < M && !any; ++c) any = cam_fixed[c] != 0;
+  if (!any) return m;
+  m.resize((size_t)M);
+  for (int c = 0; c < M; ++c) m[c] = cam_fixed[c] ? 1 : 0;
+  return m;
+}
+
+// The device arrays visual_plan gathers the per-observation arrays from, indexed by source landmark
+struct VisualSrc {
+  const long long* obs_ptr = nullptr;
+  const int* cam = nullptr;
+  const float2* uv = nullptr;
+  const double* plane = nullptr;
+};
+
+// Everything the handle derives from its system rows (row_of_cam and P->cam_of_row): the envelope and the solver path, the
+// shard, the landmark layout with its batches and tiles, the per-observation arrays, the destination table, the buffers of the
+// big landmarks and the row-sized buffers.  valid: the source landmarks with a usable plane, in ascending order of the caller's
+// landmark; obs_ptr / obs_cam: the host CSR of the source landmarks; src_id: the caller's landmark of every source landmark
+// (null: the source landmarks are the caller's).  get_src(VisualSrc&) provides the device arrays once there are landmarks to
+// gather.  visual_create_impl plans from the caller's arrays, visual_replan from the handle's own.
+template <class GetSrc>
+inline int visual_plan(lvba_visual_problem* P, const std::vector<int64_t>& valid, const int64_t* obs_ptr, const int32_t* obs_cam,
+                       const std::vector<int>& row_of_cam, const int* src_id, const GetSrc& get_src, SetupLaps& lap) {
+  cudaStream_t s = P->stream;
+  P->n_rows = (int)P->cam_of_row.size();
+  const int64_t Tv_all = (int64_t)valid.size();
+  DevBuf<int> d_row_of_cam, d_src_trk;
+
+  // ---- envelope of the reduced camera system over ALL valid landmarks
+  std::vector<int> min_row, min_sys_row;     // shard key: lowest camera; row-owned reduced system: lowest row of the clique
+  std::vector<int> first_raw = visual_first_rows(P->n_rows, valid.data(), Tv_all, obs_ptr, obs_cam, row_of_cam.data(), min_row, min_sys_row);
+  if (P->n_rows > 0) {
+    first_raw.resize(P->n_rows);
+    LVBA_TRY(P->env.build(first_raw, s, &P->h2d));
+    LVBA_TRY(P->solver.prepare(P->env, s));
+  } else {                                   // every camera constant (or unseen): no reduced system
+    Envelope& e = P->env;
+    e.n = 0; e.nblocks = 0; e.max_col = 0;
+    e.first.clear(); e.last.clear(); e.row_start.clear();
+    e.d_first.release(); e.d_last.release(); e.d_row_start.release();
+  }
+
+  lap("envelope + solver prepare");
+  // ---- shard (SURVEY.md §8e): landmark -> owner of its lowest camera index
+  Comm& cm = comm();
+  std::vector<int64_t> own;                                    // indices into valid
+  if (cm.active())
+    for (int64_t k = 0; k < Tv_all; ++k)
+      if ((P->solver.dist() ? P->solver.dist_owner(min_sys_row[k]) : shard_owner(min_row[k], P->M, cm.n_ranks)) == cm.rank) own.push_back(k);
+  VisualLayout L;                                              // landmark order and list, batches and tiles
+  visual_layout(P->n_rows, valid.data(), Tv_all, cm.active() ? &own : nullptr, min_sys_row.data(), obs_ptr, obs_cam, row_of_cam.data(), L);
+  const int64_t Tv = L.Tv, Tv_small = L.Tv_small;
+  P->Tv = Tv;
+  P->Tv_small = Tv_small;
+  P->n_big = Tv - Tv_small;
+  P->nnz = L.nnz;
+  lap("landmark list");
+  P->n_batches = (int)L.batch_trk.size() - 1;
+  P->n_tiles = (int)L.tile_trk.size() - 1;
+  lap("batches + tiles");
+
+  // ---- gather the per-observation arrays and build the destination table on the device
+  LVBA_TRY(P->trk_ptr.upload(L.trk_ptr, s, &P->h2d));
+  LVBA_TRY(P->batch_trk.upload(L.batch_trk, s, &P->h2d));
+  LVBA_TRY(P->tile_trk.upload(L.tile_trk, s, &P->h2d));
+  P->n_pairs = 0;
+  if (Tv > 0) {
+    VisualSrc src;
+    LVBA_TRY(get_src(src));
+    LVBA_TRY(d_row_of_cam.upload(row_of_cam, s, &P->h2d));
+    if (src_id) {                                              // the kernels index the state by the caller's landmark
+      std::vector<int> id(L.trk_id.size());
+      for (size_t k = 0; k < id.size(); ++k) id[k] = src_id[L.trk_id[k]];
+      LVBA_TRY(d_src_trk.upload(L.trk_id, s, &P->h2d));
+      LVBA_TRY(P->trk_id.upload(id, s, &P->h2d));
+    } else {
+      LVBA_TRY(P->trk_id.upload(L.trk_id, s, &P->h2d));
+    }
+    LVBA_TRY(P->obs_cam.alloc((size_t)P->nnz)); LVBA_TRY(P->obs_row.alloc((size_t)P->nnz)); LVBA_TRY(P->obs_uv.alloc((size_t)P->nnz));
+    LVBA_TRY(P->plane.alloc((size_t)Tv * 4));
+    visual_gather_kernel<<<(unsigned)((Tv + 127) / 128), 128, 0, s>>>(Tv, src_id ? d_src_trk.p : P->trk_id.p, P->trk_ptr.p, src.obs_ptr, src.cam,
+                                                                     src.uv, src.plane, d_row_of_cam.p, P->obs_cam.p, P->obs_row.p, P->obs_uv.p,
+                                                                     P->plane.p);
+    LVBA_CUDA(cudaGetLastError());
+    ++P->launches;
+    CudaExec ex;                                               // the destination table covers the small landmarks only
+    ex.stream = s;
+    int64_t np = 0;
+    LVBA_TRY(visual_tables(ex, P->table_in(), Tv_small, L.n_ordered, L.trk_ptr[Tv_small], P->prun, P->drun, &np));
+    P->launches += ex.launches;
+    P->n_pairs = np + L.big_pairs;
+    if (P->n_big > 0) {
+      P->n_big_obs = P->nnz - L.trk_ptr[Tv_small];
+      P->n_big_pairs = L.big_pair_ptr.back();
+      LVBA_TRY(P->big_pair_ptr.upload(L.big_pair_ptr, s, &P->h2d));
+      LVBA_TRY(P->big_obs.alloc((size_t)P->n_big_obs * vbig::kObs));
+      LVBA_TRY(P->big_params.alloc((size_t)P->n_big * kTrkParams));
+    }
+  }
+  lap("device gather + destination table");
+  if (P->n_rows > 0) LVBA_TRY(P->d_cam_of_row.upload(P->cam_of_row, s, &P->h2d));
+  const size_t n6 = (size_t)std::max(P->n_rows, 1) * 6;
+  LVBA_TRY(P->S.alloc((size_t)std::max<long long>(P->env.nblocks, 1) * 36));
+  LVBA_TRY(P->rhs.alloc(n6)); LVBA_TRY(P->y.alloc(n6)); LVBA_TRY(P->dadd.alloc(n6));
+  LVBA_TRY(P->cam_colsq.alloc(n6)); LVBA_TRY(P->cam_grad.alloc(n6)); LVBA_TRY(P->s_cam.alloc(n6));
+  LVBA_TRY(P->s_pt.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
+  LVBA_TRY(P->pt_colsq.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
+  const size_t nb = (size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1);   // partial slots, big landmarks last
+  LVBA_TRY(P->batch_cost.alloc(nb)); LVBA_TRY(P->batch_gmax.alloc(nb)); LVBA_TRY(P->batch_out.alloc(nb * 4));
+  LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
+  LVBA_CUDA(cudaStreamSynchronize(s));                         // the temporaries above are idle before they are parked
+  return LVBA_OK;
+}
+
 inline int visual_create_impl(int32_t M, int64_t T, const double* q, const double* t, const double* X,
                               const double* plane_nd, const int64_t* obs_ptr, const int32_t* obs_cam,
                               const float* obs_uv, const double intr[8], double sigma_px, double sigma_plane,
-                              int32_t fixed_cam, int32_t device, lvba_visual_problem** out) {
+                              int32_t fixed_cam, const uint8_t* cam_fixed, int32_t device, lvba_visual_problem** out) {
   if (!out) return fail(LVBA_ERR_INVALID_ARG, "out is null");
   *out = nullptr;
   if (M <= 0 || T < 0) return fail(LVBA_ERR_INVALID_ARG, "M=%d T=%lld", M, (long long)T);
@@ -147,6 +271,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   SetupLaps lap("visual setup", 26, nullptr, t_begin);
   std::unique_ptr<lvba_visual_problem> P(new lvba_visual_problem());
   P->M = M; P->T = T; P->fixed_cam = fixed_cam;
+  P->cam_fixed = visual_mask(M, cam_fixed);
   for (int i = 0; i < 8; ++i) P->intr[i] = intr[i];
   P->sigma_px = sigma_px; P->sigma_pl = sigma_plane;
   LVBA_CUDA(cudaGetDevice(&P->device));
@@ -158,79 +283,27 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   // ---- valid landmarks, active cameras (src/lvba_system.cpp:1582-1583, 1598-1603; SURVEY.md Q11)
   std::vector<int64_t> valid;
   std::vector<int> row_of_cam;
-  visual_rows(M, T, plane_nd, obs_ptr, obs_cam, fixed_cam, valid, row_of_cam, P->cam_of_row);
-  P->n_rows = (int)P->cam_of_row.size();
-  const int64_t Tv_all = (int64_t)valid.size();
-
+  visual_rows(M, T, plane_nd, obs_ptr, obs_cam, fixed_cam, P->cam_fixed.empty() ? nullptr : P->cam_fixed.data(), valid, row_of_cam,
+              P->cam_of_row);
   lap("valid landmarks / rows");
-  // ---- envelope of the reduced camera system over ALL valid landmarks
-  std::vector<int> min_row, min_sys_row;     // shard key: lowest camera; row-owned reduced system: lowest row of the clique
-  std::vector<int> first_raw = visual_first_rows(P->n_rows, valid.data(), Tv_all, obs_ptr, obs_cam, row_of_cam.data(), min_row, min_sys_row);
-  if (P->n_rows > 0) {
-    first_raw.resize(P->n_rows);
-    LVBA_TRY(P->env.build(first_raw, s, &P->h2d));
-    LVBA_TRY(P->solver.prepare(P->env, s));
-  }
 
-  lap("envelope + solver prepare");
-  // ---- shard (SURVEY.md §8e): landmark -> owner of its lowest camera index
-  Comm& cm = comm();
-  std::vector<int64_t> own;                                    // indices into valid
-  if (cm.active())
-    for (int64_t k = 0; k < Tv_all; ++k)
-      if ((P->solver.dist() ? P->solver.dist_owner(min_sys_row[k]) : shard_owner(min_row[k], M, cm.n_ranks)) == cm.rank) own.push_back(k);
-  VisualLayout L;                                              // landmark order and list, batches and tiles
-  visual_layout(P->n_rows, valid.data(), Tv_all, cm.active() ? &own : nullptr, min_sys_row.data(), obs_ptr, obs_cam, row_of_cam.data(), L);
-  const int64_t Tv = L.Tv, Tv_small = L.Tv_small;
-  P->Tv = Tv;
-  P->Tv_small = Tv_small;
-  P->n_big = Tv - Tv_small;
-  P->nnz = L.nnz;
-  lap("landmark list");
-  P->n_batches = (int)L.batch_trk.size() - 1;
-  P->n_tiles = (int)L.tile_trk.size() - 1;
-  lap("batches + tiles");
-
-  // ---- upload the caller's arrays as they are; gather the per-observation arrays and build the destination table on the device
-  LVBA_TRY(P->trk_ptr.upload(L.trk_ptr, s, &P->h2d));
-  LVBA_TRY(P->batch_trk.upload(L.batch_trk, s, &P->h2d));
-  LVBA_TRY(P->tile_trk.upload(L.tile_trk, s, &P->h2d));
-  P->n_pairs = 0;
-  if (Tv > 0) {
+  // ---- the caller's arrays go up as they are (one DMA each from the caller's, ideally pinned, memory); the plan gathers the
+  // per-observation arrays from them on the device
+  DevBuf<long long> d_obs_ptr;
+  DevBuf<int> d_raw_cam;
+  DevBuf<float2> d_raw_uv;
+  DevBuf<double> d_raw_plane;
+  auto upload_raw = [&](VisualSrc& src) -> int {
     const int64_t nnz_all = obs_ptr[T];
-    DevBuf<long long> d_obs_ptr;
-    DevBuf<int> d_raw_cam, d_row_of_cam;
-    DevBuf<float2> d_raw_uv;
-    DevBuf<double> d_raw_plane;
     static_assert(sizeof(long long) == sizeof(int64_t), "obs_ptr is uploaded as it is");
     LVBA_TRY(d_obs_ptr.upload(reinterpret_cast<const long long*>(obs_ptr), (size_t)T + 1, s, &P->h2d));
     LVBA_TRY(d_raw_cam.upload(obs_cam, (size_t)nnz_all, s, &P->h2d));
     LVBA_TRY(d_raw_uv.upload(reinterpret_cast<const float2*>(obs_uv), (size_t)nnz_all, s, &P->h2d));
     LVBA_TRY(d_raw_plane.upload(plane_nd, (size_t)T * 4, s, &P->h2d));
-    LVBA_TRY(d_row_of_cam.upload(row_of_cam, s, &P->h2d));
-    LVBA_TRY(P->trk_id.upload(L.trk_id, s, &P->h2d));
-    LVBA_TRY(P->obs_cam.alloc((size_t)P->nnz)); LVBA_TRY(P->obs_row.alloc((size_t)P->nnz)); LVBA_TRY(P->obs_uv.alloc((size_t)P->nnz));
-    LVBA_TRY(P->plane.alloc((size_t)Tv * 4));
-    visual_gather_kernel<<<(unsigned)((Tv + 127) / 128), 128, 0, s>>>(Tv, P->trk_id.p, P->trk_ptr.p, d_obs_ptr.p, d_raw_cam.p, d_raw_uv.p,
-                                                                     d_raw_plane.p, d_row_of_cam.p, P->obs_cam.p, P->obs_row.p, P->obs_uv.p, P->plane.p);
-    LVBA_CUDA(cudaGetLastError());
-    ++P->launches;
-    CudaExec ex;                                               // the destination table covers the small landmarks only
-    ex.stream = s;
-    int64_t np = 0;
-    LVBA_TRY(visual_tables(ex, P->table_in(), Tv_small, L.n_ordered, L.trk_ptr[Tv_small], P->prun, P->drun, &np));
-    P->launches += ex.launches;
-    P->n_pairs = np + L.big_pairs;
-    if (P->n_big > 0) {
-      P->n_big_obs = P->nnz - L.trk_ptr[Tv_small];
-      P->n_big_pairs = L.big_pair_ptr.back();
-      LVBA_TRY(P->big_pair_ptr.upload(L.big_pair_ptr, s, &P->h2d));
-      LVBA_TRY(P->big_obs.alloc((size_t)P->n_big_obs * vbig::kObs));
-      LVBA_TRY(P->big_params.alloc((size_t)P->n_big * kTrkParams));
-    }
-  }
-  lap("device gather + destination table");
-  if (P->n_rows > 0) LVBA_TRY(P->d_cam_of_row.upload(P->cam_of_row, s, &P->h2d));
+    src = VisualSrc{d_obs_ptr.p, d_raw_cam.p, d_raw_uv.p, d_raw_plane.p};
+    return LVBA_OK;
+  };
+  LVBA_TRY(visual_plan(P.get(), valid, obs_ptr, obs_cam, row_of_cam, nullptr, upload_raw, lap));
   LVBA_TRY(P->q.upload(q, (size_t)M * 4, s, &P->h2d));
   LVBA_TRY(P->t.upload(t, (size_t)M * 3, s, &P->h2d));
   LVBA_TRY(P->X.upload(X, (size_t)T * 3, s, &P->h2d));
@@ -243,15 +316,6 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
     LVBA_TRY(dup(P->q0, P->q, (size_t)M * 4)); LVBA_TRY(dup(P->t0, P->t, (size_t)M * 3)); LVBA_TRY(dup(P->X0, P->X, (size_t)T * 3));
     LVBA_TRY(dup(P->qc, P->q, (size_t)M * 4)); LVBA_TRY(dup(P->tc, P->t, (size_t)M * 3)); LVBA_TRY(dup(P->Xc, P->X, (size_t)T * 3));
   }
-  const size_t n6 = (size_t)std::max(P->n_rows, 1) * 6;
-  LVBA_TRY(P->S.alloc((size_t)std::max<long long>(P->env.nblocks, 1) * 36));
-  LVBA_TRY(P->rhs.alloc(n6)); LVBA_TRY(P->y.alloc(n6)); LVBA_TRY(P->dadd.alloc(n6));
-  LVBA_TRY(P->cam_colsq.alloc(n6)); LVBA_TRY(P->cam_grad.alloc(n6)); LVBA_TRY(P->s_cam.alloc(n6));
-  LVBA_TRY(P->s_pt.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
-  LVBA_TRY(P->pt_colsq.alloc((size_t)std::max<int64_t>(Tv, 1) * 3));
-  const size_t nb = (size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1);   // partial slots, big landmarks last
-  LVBA_TRY(P->batch_cost.alloc(nb)); LVBA_TRY(P->batch_gmax.alloc(nb)); LVBA_TRY(P->batch_out.alloc(nb * 4));
-  LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
   LVBA_TRY(P->scal.alloc(16)); LVBA_TRY(P->scal.zero(s));
   LVBA_TRY(P->cam_step.alloc((size_t)M * 6)); LVBA_TRY(P->pt_step.alloc((size_t)std::max<int64_t>(T, 1) * 3));
   LVBA_CUDA(cudaFuncSetAttribute(visual_build_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)visual_build_smem_bytes()));
@@ -263,6 +327,70 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   lvba_visual_default_opts(&P->opts);
   P->ms_setup = wall_ms() - t_begin;
   *out = P.release();
+  return LVBA_OK;
+}
+
+// A new set of constant cameras on a handle (lvba_visual_reset_lm): visual_plan again, from the handle's own arrays.  The
+// source landmarks are the local landmarks of the current plan, taken in the caller's order, so that the new plan is the one
+// lvba_visual_create would make with this mask; observations, planes and the state stay on the device.  One GPU only: the
+// local landmarks are then all valid ones (visual_set_mode refuses a mask under an active communicator).
+// A failure leaves the handle as it was (the previous plan is made again from the same source arrays) with deterministic mode
+// off; only if that fails too is the handle marked unusable, and then every call but destroy, get_state, set_state and
+// reset_state refuses it.
+inline int visual_replan(lvba_visual_problem* P, std::vector<uint8_t> mask) {
+  SetupLaps lap("visual re-plan", 26, P->stream, wall_ms());
+  cudaStream_t s = P->stream;
+  const int64_t Tv = P->Tv;
+  std::vector<int> trk_ptr((size_t)Tv + 1, 0), trk_id((size_t)Tv), cam((size_t)P->nnz);
+  if (Tv > 0) {
+    LVBA_CUDA(cudaMemcpyAsync(trk_ptr.data(), P->trk_ptr.p, trk_ptr.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    LVBA_CUDA(cudaMemcpyAsync(trk_id.data(), P->trk_id.p, trk_id.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (!cam.empty()) LVBA_CUDA(cudaMemcpyAsync(cam.data(), P->obs_cam.p, cam.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    P->d2h += (int64_t)(trk_ptr.size() + trk_id.size() + cam.size()) * (int64_t)sizeof(int);
+  }
+  std::vector<int64_t> valid((size_t)Tv), src_ptr(trk_ptr.begin(), trk_ptr.end());
+  for (int64_t k = 0; k < Tv; ++k) valid[k] = k;
+  std::sort(valid.begin(), valid.end(), [&](int64_t a, int64_t b) { return trk_id[a] < trk_id[b]; });
+  std::vector<char> used((size_t)P->M, 0);
+  for (int c : cam) used[c] = 1;
+  lap("rows");
+  // the records of deterministic mode follow the table: set up again when the mode is next asked for (visual_set_mode)
+  tiles::fixed_sum_release(P->det_S); tiles::fixed_sum_release(P->det_G); P->det_C.release();
+  P->det_ready = false;
+  P->det = false;
+  P->solver.set_deterministic(false);
+  DevBuf<long long> d_src_ptr;
+  DevBuf<int> old_cam;
+  DevBuf<float2> old_uv;
+  DevBuf<double> old_plane;
+  old_cam.swap(P->obs_cam); old_uv.swap(P->obs_uv); old_plane.swap(P->plane);
+  auto old_arrays = [&](VisualSrc& src) -> int {
+    LVBA_TRY(d_src_ptr.upload(reinterpret_cast<const long long*>(src_ptr.data()), src_ptr.size(), s, &P->h2d));
+    src = VisualSrc{d_src_ptr.p, old_cam.p, old_uv.p, old_plane.p};
+    return LVBA_OK;
+  };
+  auto plan_with = [&](const std::vector<uint8_t>& m) -> int {
+    std::vector<int> row_of_cam;
+    visual_row_map(P->M, used, P->fixed_cam, m.empty() ? nullptr : m.data(), row_of_cam, P->cam_of_row);
+    LVBA_TRY(visual_plan(P, valid, src_ptr.data(), cam.data(), row_of_cam, trk_id.data(), old_arrays, lap));
+    return P->scal.zero(s);                                    // no stale camera gradient when the new plan has no rows
+  };
+  int rc;
+  try { rc = plan_with(mask); } catch (const std::bad_alloc&) { rc = fail(LVBA_ERR_NOMEM, "host allocation failed"); }
+  if (rc != LVBA_OK) {
+    const std::string why = last_error_ref();
+    cudaStreamSynchronize(s);
+    cudaGetLastError();
+    int rc_back;
+    try { rc_back = plan_with(P->cam_fixed); } catch (const std::bad_alloc&) { rc_back = LVBA_ERR_NOMEM; }
+    if (rc_back != LVBA_OK) {
+      P->unusable = true;
+      return fail(rc, "re-plan for the new cam_fixed failed (%s), and so did restoring the previous plan: destroy the handle", why.c_str());
+    }
+    return fail(rc, "re-plan for the new cam_fixed failed (%s); the handle keeps its previous constant cameras", why.c_str());
+  }
+  P->cam_fixed = std::move(mask);
   return LVBA_OK;
 }
 
@@ -296,11 +424,31 @@ inline int visual_check_loss(const lvba_visual_opts& o) {
   return LVBA_OK;
 }
 
-// the LM mode of the handle (lvba_visual_reset_lm and the one-shot call): deterministic mode and the robust losses
+// a handle whose failed re-plan could not be undone (visual_replan) takes no further calls but destroy and the state copies
+inline int visual_check_usable(const lvba_visual_problem* P) {
+  if (P->unusable) return fail(LVBA_ERR_INVALID_ARG, "this handle lost its plan in a failed lvba_visual_reset_lm: destroy it");
+  return LVBA_OK;
+}
+
+// constant cameras beyond fixed_cam run on one GPU (the shard of a landmark follows its lowest camera, whatever is constant)
+inline int visual_check_mask(bool has_mask) {
+  if (has_mask && comm().active())
+    return fail(LVBA_ERR_UNSUPPORTED, "cam_fixed runs on one GPU: constant cameras are not supported with an active communicator");
+  return LVBA_OK;
+}
+
+// the LM mode of the handle (lvba_visual_reset_lm and the one-shot call): the constant cameras, deterministic mode and the
+// robust losses
 inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   LVBA_TRY(visual_check_loss(o));
   if (o.deterministic && comm().active())
     return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode runs on one GPU: the multi-GPU sums of NCCL have no fixed order");
+  std::vector<uint8_t> mask = visual_mask(P->M, o.cam_fixed);
+  LVBA_TRY(visual_check_mask(!mask.empty() || !P->cam_fixed.empty()));
+  if (mask != P->cam_fixed) {
+    LVBA_CUDA(cudaSetDevice(P->device));
+    LVBA_TRY(visual_replan(P, std::move(mask)));
+  }
   if (o.deterministic) {
     LVBA_CUDA(cudaSetDevice(P->device));
     const int rc = visual_det_setup(P);
@@ -466,8 +614,9 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   P->timers.end();
   LVBA_CUDA(cudaGetLastError());
   LVBA_CUDA(cudaMemcpyAsync(P->h_scal, P->scal.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  LVBA_CUDA(cudaMemcpyAsync(P->h_scal + 15, P->solver.status.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (P->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(P->h_scal + 15, P->solver.status.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   LVBA_CUDA(cudaStreamSynchronize(s));
+  if (P->n_rows == 0) *reinterpret_cast<int*>(P->h_scal + 15) = 0;   // every camera constant: nothing was factorised
   P->d2h += 16 * sizeof(double);
   return LVBA_OK;
 }
@@ -547,12 +696,13 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
   // no loss (src/lvba_system.cpp:1630, :1639); the scales of the reference's HuberLoss objects (:1585-1586)
   o->reproj_loss = LVBA_LOSS_NONE; o->reproj_loss_scale = 1.0;
   o->plane_loss = LVBA_LOSS_NONE; o->plane_loss_scale = 0.1;
+  o->cam_fixed = nullptr;
 }
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
                        const int64_t* obs_ptr, const int32_t* obs_cam, const float* obs_uv, const double intr[8],
                        double sigma_px, double sigma_plane, int32_t fixed_cam, int32_t device, lvba_visual_problem** out) LVBA_ABI_BEGIN {
-  return lvba::visual_create_impl(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, device, out);
+  return lvba::visual_create_impl(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, nullptr, device, out);
 } LVBA_ABI_END("lvba_visual_create")
 
 int lvba_visual_destroy(lvba_visual_problem* p) LVBA_ABI_BEGIN {
@@ -600,6 +750,7 @@ int lvba_visual_get_state(lvba_visual_problem* p, double* q, double* t, double* 
 
 int lvba_visual_cost(lvba_visual_problem* p, double* cost) LVBA_ABI_BEGIN {
   if (!p || !cost) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   cudaStream_t s = p->stream;
   if (p->robust()) lvba::visual_cost_t<true>(p, p->state(), p->scal.p + 8);
@@ -614,6 +765,7 @@ int lvba_visual_cost(lvba_visual_problem* p, double* cost) LVBA_ABI_BEGIN {
 int lvba_visual_step(lvba_visual_problem* p, double radius, int32_t jacobi_scaling, int32_t recompute_scale,
                      double* cam_step, double* pt_step, double* model_cost_change, double* cost) LVBA_ABI_BEGIN {
   if (!p || !(radius > 0)) return lvba::fail(LVBA_ERR_INVALID_ARG, "bad argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   if (recompute_scale || !p->lm.have_scale) LVBA_TRY(lvba::visual_compute_scale(p, jacobi_scaling));
   LVBA_CUDA(cudaMemsetAsync(p->cam_step.p, 0, (size_t)p->M * 6 * sizeof(double), p->stream));
@@ -629,6 +781,7 @@ int lvba_visual_step(lvba_visual_problem* p, double radius, int32_t jacobi_scali
 
 int lvba_visual_structure(lvba_visual_problem* p, int32_t* n_active, int32_t* cam_of_row, int64_t* nblocks, int32_t* brow, int32_t* bcol) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   if (n_active) *n_active = p->n_rows;
   if (cam_of_row) for (int r = 0; r < p->n_rows; ++r) cam_of_row[r] = p->cam_of_row[r];
   if (nblocks) *nblocks = p->env.nblocks;
@@ -643,6 +796,7 @@ int lvba_visual_structure(lvba_visual_problem* p, int32_t* n_active, int32_t* ca
 
 int lvba_visual_get_system(lvba_visual_problem* p, double* rhs, double* blocks) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   if (rhs && p->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(rhs, p->rhs.p, (size_t)p->n_rows * 6 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
   if (blocks && p->env.nblocks > 0) LVBA_CUDA(cudaMemcpyAsync(blocks, p->S.p, (size_t)p->env.nblocks * 36 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
@@ -652,6 +806,7 @@ int lvba_visual_get_system(lvba_visual_problem* p, double* rhs, double* blocks) 
 
 int lvba_visual_reset_lm(lvba_visual_problem* p, const lvba_visual_opts* opts) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   lvba_visual_opts o;
   if (opts) o = *opts; else lvba_visual_default_opts(&o);
   LVBA_TRY(lvba::visual_set_mode(p, o));
@@ -673,12 +828,14 @@ int lvba_visual_reset_state(lvba_visual_problem* p) LVBA_ABI_BEGIN {
 
 int lvba_visual_iterate(lvba_visual_problem* p, int32_t n_iter, lvba_summary* summary) LVBA_ABI_BEGIN {
   if (!p || n_iter < 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "bad argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   return lvba::visual_iterate_impl(p, n_iter, summary);
 } LVBA_ABI_END("lvba_visual_iterate")
 
 int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_valid_tracks, int64_t* n_blocks_env, int64_t* n_pairs) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   if (nnz_valid) *nnz_valid = p->nnz;
   if (n_valid_tracks) *n_valid_tracks = p->Tv;
   if (n_blocks_env) *n_blocks_env = p->env.nblocks;
@@ -688,6 +845,7 @@ int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_va
 
 int lvba_visual_big_counts(lvba_visual_problem* p, int64_t* n_big, int64_t* n_big_obs, int64_t* n_big_pairs) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
   if (n_big) *n_big = p->n_big;
   if (n_big_obs) *n_big_obs = p->n_big_obs;
   if (n_big_pairs) *n_big_pairs = p->n_big_pairs;
@@ -701,8 +859,11 @@ int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const 
   lvba_visual_opts o;
   if (opts) o = *opts; else lvba_visual_default_opts(&o);
   LVBA_TRY(lvba::visual_check_loss(o));                       // before any device work: the buffers stay untouched
+  LVBA_TRY(lvba::visual_check_mask(M > 0 && !lvba::visual_mask(M, o.cam_fixed).empty()));
   lvba_visual_problem* p = nullptr;
-  int rc = lvba_visual_create(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, o.device, &p);
+  // planned once, with the constant cameras: the reset below finds the handle's mask equal to the options'
+  int rc = lvba::visual_create_impl(M, T, q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam, o.cam_fixed,
+                                    o.device, &p);
   if (rc != LVBA_OK) return rc;
   return lvba::lm_one_shot(p, o, p->Tv > 0, lvba_visual_reset_lm, lvba_visual_iterate, lvba_visual_destroy,
                            [&] { return lvba_visual_get_state(p, q, t, X); }, t0, summary);   // write-back, src/lvba_system.cpp:1651-1665

@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <climits>
 #include <cmath>
+#include <utility>
 #include <vector>
 
 #include "setup_pool.h"
@@ -26,10 +27,23 @@ inline bool plane_valid(const double* p) {   // has_valid_plane, src/lvba_system
   return std::fabs(p[0]) > 1e-6 || std::fabs(p[1]) > 1e-6 || std::fabs(p[2]) > 1e-6;
 }
 
-// Valid landmarks (a usable plane) and active cameras (seen by one, not the fixed camera), src/lvba_system.cpp:1582-1583,
-// 1598-1603: valid in ascending order, row_of_cam[c] = system row of camera c (-1: constant), cam_of_row its inverse.
+// The system rows from the cameras seen by a valid landmark (cam_used [M]): one row per such camera that is not constant, in
+// ascending camera order.  Constant: fixed_cam and every c with cam_fixed[c] != 0 (cam_fixed may be null).
+// row_of_cam[c] = system row of camera c (-1: constant or unseen), cam_of_row its inverse.
+inline void visual_row_map(int M, std::vector<char> cam_used, int fixed_cam, const uint8_t* cam_fixed, std::vector<int>& row_of_cam,
+                           std::vector<int>& cam_of_row) {
+  if (fixed_cam >= 0 && fixed_cam < M) cam_used[fixed_cam] = 0;
+  if (cam_fixed)
+    for (int c = 0; c < M; ++c) if (cam_fixed[c]) cam_used[c] = 0;
+  row_of_cam.assign(M, -1);
+  cam_of_row.clear();
+  for (int c = 0; c < M; ++c) if (cam_used[c]) { row_of_cam[c] = (int)cam_of_row.size(); cam_of_row.push_back(c); }
+}
+
+// Valid landmarks (a usable plane) and active cameras (seen by one, not constant), src/lvba_system.cpp:1582-1583, 1598-1603:
+// valid in ascending order, the rows as visual_row_map.
 inline void visual_rows(int M, int64_t T, const double* plane_nd, const int64_t* obs_ptr, const int32_t* obs_cam, int fixed_cam,
-                        std::vector<int64_t>& valid, std::vector<int>& row_of_cam, std::vector<int>& cam_of_row) {
+                        const uint8_t* cam_fixed, std::vector<int64_t>& valid, std::vector<int>& row_of_cam, std::vector<int>& cam_of_row) {
   std::vector<char> cam_used(M, 0);
   {
     std::vector<char> is_valid((size_t)T, 0), used_w((size_t)kMaxSetupThreads * (size_t)M, 0);
@@ -45,9 +59,7 @@ inline void visual_rows(int M, int64_t T, const double* plane_nd, const int64_t*
       for (int c = 0; c < M; ++c) cam_used[c] |= used_w[(size_t)w * (size_t)M + c];
     for (int64_t i = 0; i < T; ++i) if (is_valid[(size_t)i]) valid.push_back(i);
   }
-  if (fixed_cam >= 0 && fixed_cam < M) cam_used[fixed_cam] = 0;
-  row_of_cam.assign(M, -1);
-  for (int c = 0; c < M; ++c) if (cam_used[c]) { row_of_cam[c] = (int)cam_of_row.size(); cam_of_row.push_back(c); }
+  visual_row_map(M, std::move(cam_used), fixed_cam, cam_fixed, row_of_cam, cam_of_row);
 }
 
 // The raw envelope of the reduced camera system over the landmarks valid[0..n): first[r] = the lowest row that shares a landmark

@@ -455,18 +455,27 @@ struct Observation { int cam; float u, v; };
 
 // opts: null = lvba_visual_default_opts, plain least squares as the reference's nullptr losses (:1630, :1639).  Its
 // loss_function_reproj / loss_function_plane (HuberLoss(1.0) / HuberLoss(0.1), :1585-1586) map to reproj_loss = plane_loss =
-// LVBA_LOSS_HUBER with the default scales 1.0 / 0.1 (INTEGRATION.md, B2).
+// LVBA_LOSS_HUBER with the default scales 1.0 / 0.1 (INTEGRATION.md, B2).  Camera 0 is constant, as in the reference
+// (:1582-1583); cam_fixed (null: none, else one entry per camera, nonzero = constant) holds further cameras constant and
+// overrides opts->cam_fixed.
 inline int solve_visual(std::vector<std::array<double, 4>>& qs, std::vector<std::array<double, 3>>& ts,
                         std::vector<std::array<double, 3>>& Xs, const std::vector<std::array<double, 3>>& plane_n,
                         const std::vector<double>& plane_d, const std::vector<std::vector<Observation>>& obs_of_point,
                         double fx, double fy, double cx, double cy, double k1, double k2, double p1, double p2,
                         double sigma_px = 0.5, double sigma_plane = 0.01, const lvba_visual_opts* opts = nullptr,
-                        lvba_summary* summary = nullptr) {
+                        lvba_summary* summary = nullptr, const std::vector<uint8_t>* cam_fixed = nullptr) {
   const int M = (int)qs.size();
   const int64_t T = (int64_t)Xs.size();
   if ((int)ts.size() != M) throw std::runtime_error("lvba_b200::solve_visual: qs/ts size mismatch");      // cf. :1427
   if ((int64_t)plane_n.size() != T || (int64_t)plane_d.size() != T || (int64_t)obs_of_point.size() != T)
     throw std::runtime_error("lvba_b200::solve_visual: per-point array size mismatch");
+  if (cam_fixed && (int)cam_fixed->size() != M) throw std::runtime_error("lvba_b200::solve_visual: cam_fixed needs one entry per camera");
+  lvba_visual_opts o;
+  if (cam_fixed) {
+    if (opts) o = *opts; else lvba_visual_default_opts(&o);
+    o.cam_fixed = cam_fixed->data();
+    opts = &o;
+  }
   std::vector<int64_t> obs_ptr(T + 1, 0);
   std::vector<int32_t> obs_cam;
   std::vector<float> obs_uv;

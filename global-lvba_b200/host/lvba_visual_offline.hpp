@@ -17,6 +17,7 @@
 #include <limits>
 #include <dlfcn.h>
 
+#include <algorithm>
 #include <array>
 #include <cmath>
 #include <cstdint>
@@ -88,6 +89,34 @@ inline bool parse_loss(const char* text, double default_scale, int32_t& kind, do
   }
   kind = k;
   scale = a;
+  return true;
+}
+
+// A list of index ranges `A:B,C,D:E` (each A:B inclusive, A <= B, a single index C for C:C, indices decimal and >= 0) as a
+// mask of n entries, 1 on every listed index.  Anything else, or an index >= n, is refused with a message in *err; mask is
+// then untouched.  n < 0 checks the syntax only and leaves mask untouched.
+inline bool parse_index_ranges(const char* text, int n, std::vector<uint8_t>& mask, std::string* err = nullptr) {
+  const std::string s = text ? text : "";
+  std::vector<uint8_t> m((size_t)std::max(n, 0), 0);
+  auto index = [](const std::string& t, long& v) {
+    if (t.empty() || t.size() > 9 || t.find_first_not_of("0123456789") != std::string::npos) return false;
+    v = std::strtol(t.c_str(), nullptr, 10);
+    return true;
+  };
+  size_t pos = 0;
+  do {
+    const size_t comma = s.find(',', pos);
+    const std::string item = s.substr(pos, comma == std::string::npos ? std::string::npos : comma - pos);
+    const size_t colon = item.find(':');
+    long a = 0, b = 0;
+    const bool ok = colon == std::string::npos ? index(item, a) && index(item, b)
+                                               : index(item.substr(0, colon), a) && index(item.substr(colon + 1), b);
+    if (!ok || a > b) { if (err) *err = "'" + s + "': '" + item + "' is not an index or a range A:B with A <= B"; return false; }
+    if (n >= 0 && b >= n) { if (err) *err = "'" + s + "': index " + std::to_string(b) + " is past the last of " + std::to_string(n); return false; }
+    if (n >= 0) for (long i = a; i <= b; ++i) m[(size_t)i] = 1;
+    pos = comma == std::string::npos ? std::string::npos : comma + 1;
+  } while (pos != std::string::npos);
+  if (n >= 0) mask.swap(m);
   return true;
 }
 

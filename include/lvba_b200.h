@@ -98,6 +98,21 @@ typedef struct lvba_visual_opts {
   double reproj_loss_scale;      /* 1.0 */
   int32_t plane_loss;            /* LVBA_LOSS_NONE (:1639) */
   double plane_loss_scale;       /* 0.1 */
+  /* Constant cameras (ceres::Problem::SetParameterBlockConstant, which the reference calls on camera 0 at
+   * src/lvba_system.cpp:1582-1583): NULL (the default) or M bytes, nonzero = camera held constant.  The constant cameras are
+   * fixed_cam and every camera c with cam_fixed[c] != 0; they get no row in the reduced camera system and come back
+   * bit-identical.  Their observations still enter their landmarks' blocks and every cost, which covers all residual blocks;
+   * Jacobi scaling, the LM diagonal and the gradient and parameter tolerances cover the free parameters only (Ceres).  With
+   * every camera constant only the landmarks move: lvba_visual_structure reports n_active = 0 and no blocks, lvba_visual_step
+   * writes cam_step as zeros and the landmark step of the eliminated point blocks alone.  Landmarks are never constant.
+   * As `deterministic`: the one-shot call plans its problem with the mask; a handle takes it from lvba_visual_reset_lm (a new
+   * handle has none), and a reset whose mask differs from the handle's current one re-plans the rows, the landmark layout
+   * and the build's tables before it returns (observations and state stay on the device).  If that re-plan fails, the reset
+   * returns the error and the handle keeps its previous constant cameras with deterministic mode off (reset again to turn it
+   * on); should restoring the previous plan fail as well, every later call on the handle but lvba_visual_destroy and the state
+   * copies returns LVBA_ERR_INVALID_ARG.  An all-zero mask is the same as
+   * NULL; any nonzero entry with an active communicator is LVBA_ERR_UNSUPPORTED.  The library keeps no copy of the pointer. */
+  const uint8_t* cam_fixed;
 } lvba_visual_opts;
 
 typedef enum lvba_termination {
@@ -214,7 +229,8 @@ int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env
  *   plane_nd    [T*4] (n, d); n == 0 marks "no valid plane" => landmark and its observations are skipped (:1598-1603)
  *   obs_ptr     [T+1] CSR; obs_cam [nnz] camera of each inlier observation; obs_uv [nnz*2] float pixel (:1624-1625).
  *               A landmark may have any number of observations, and may see one camera more than once.
- *   fixed_cam   camera held constant (0 in the reference, :1582-1583); -1 = none
+ *   fixed_cam   camera held constant (0 in the reference, :1582-1583); -1 = none.  lvba_visual_opts::cam_fixed adds any
+ *               set of further constant cameras.
  * ====================================================================================== */
 int lvba_visual_lm(int32_t M, int64_t T, double* q_wxyz, double* t, double* X,
                    const double* plane_nd, const int64_t* obs_ptr, const int32_t* obs_cam,

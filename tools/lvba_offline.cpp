@@ -34,6 +34,8 @@
 //                (HuberLoss, src/lvba_system.cpp:1585-1586).  The reference passes no loss (:1630, :1639): the default is none.
 //   --visual-problem F   write the visual stage's problem, its state before and after the solve, to F
 //                (lvba_visual_offline.hpp write_visual_problem), to re-run or inspect that solve elsewhere
+//   --fix-cameras LIST   hold these cameras of the visual stage constant besides camera 0 (lvba_visual_opts::cam_fixed); LIST is
+//                index ranges A:B (inclusive) or single indices, comma separated, e.g. 0:3,10; an index past the last image is an error
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -56,7 +58,7 @@ int main(int argc, char** argv) {
   int fuse_order = LVBA_FUSE_ORDER_LIBSTDCXX;         // the library's default: what a g++ build of the reference does
   int window = 0;
   double anchor_leaf = 0.1;
-  std::string db_path, sparse_dir, lidar_opt, visual_problem;
+  std::string db_path, sparse_dir, lidar_opt, visual_problem, fix_cameras;
   lvba_b200::offline::Config cfg;
   lvba_visual_opts visual_opts;
   lvba_visual_default_opts(&visual_opts);
@@ -83,6 +85,12 @@ int main(int argc, char** argv) {
     else if (a == "--lidar-opt") lidar_opt = next();
     else if (a == "--sparse-dir") sparse_dir = next();
     else if (a == "--visual-problem") visual_problem = next();
+    else if (a == "--fix-cameras") {
+      std::vector<uint8_t> unused;
+      std::string e;
+      fix_cameras = next();
+      if (!lvba_b200::offline::parse_index_ranges(fix_cameras.c_str(), -1, unused, &e)) { std::fprintf(stderr, "--fix-cameras: %s\n", e.c_str()); return 64; }
+    }
     else if (a == "--reproj-loss" || a == "--plane-loss") {
       const bool reproj = a == "--reproj-loss";
       std::string e;
@@ -229,6 +237,11 @@ int main(int argc, char** argv) {
     std::printf("{\"images\": %zu, \"first_image\": %.6f, \"width\": %d, \"height\": %d, \"fx\": %.9f, \"keypoints\": %lld, \"kp_sum\": %.6f, \"matches\": %lld, \"match_sum\": %lld, \"cam_sum\": %.9f}\n",
                 images_ids.size(), images_ids[0], cfg.width, cfg.height, cfg.fx, n_kp, kp_sum, n_match, match_sum, cam_sum);
     return 0;
+  }
+  std::vector<uint8_t> cam_fixed;                                             // one entry per image: the cameras of --fix-cameras
+  if (!fix_cameras.empty()) {
+    if (!off::parse_index_ranges(fix_cameras.c_str(), (int)images_ids.size(), cam_fixed, &err)) { std::fprintf(stderr, "--fix-cameras: %s\n", err.c_str()); return 64; }
+    visual_opts.cam_fixed = cam_fixed.data();
   }
   const float default_eigen[4] = {0.3f, 0.1f, 0.06f, 0.03f};                  // bavoxel.hpp:17 when set_eigen_ratio_array never ran
   off::VisualResult vr;
