@@ -30,7 +30,7 @@ EXPORTS = [
     "lvba_lidar_lm", "lvba_lidar_lm_batch", "lvba_lidar_create", "lvba_lidar_destroy", "lvba_lidar_set_poses",
     "lvba_lidar_get_poses", "lvba_lidar_build", "lvba_lidar_residual", "lvba_lidar_solve",
     "lvba_lidar_structure", "lvba_lidar_get_system", "lvba_lidar_reset_lm", "lvba_lidar_reset_state", "lvba_lidar_iterate",
-    "lvba_lidar_counts",
+    "lvba_lidar_counts", "lvba_lidar_rows",
     "lvba_visual_lm", "lvba_visual_create", "lvba_visual_destroy", "lvba_visual_set_state",
     "lvba_visual_get_state", "lvba_visual_cost", "lvba_visual_step", "lvba_visual_structure",
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
@@ -57,7 +57,8 @@ class LvbaError(RuntimeError):
 
 class LidarOpts(C.Structure):
     _fields_ = [("u0", C.c_double), ("v0", C.c_double), ("max_iter", C.c_int32), ("rel_tol", C.c_double),
-                ("device", C.c_int32), ("verbose", C.c_int32), ("deterministic", C.c_int32)]
+                ("device", C.c_int32), ("verbose", C.c_int32), ("deterministic", C.c_int32),
+                ("pose_fixed", C.POINTER(C.c_uint8))]
 
 
 class VisualOpts(C.Structure):
@@ -188,11 +189,26 @@ def visual_default_opts(reproj_loss=None, plane_loss=None):
 
 
 # ------------------------------------------------------------------ B1: LiDAR
-def lidar_lm(vox_ptr, pose_idx, clusters, poses, opts=None):
-    """One-shot drop-in for BALM2::damping_iter (bavoxel.hpp:662).  Returns (poses, summary dict)."""
+def _with_pose_fixed(opts, pose_fixed, W):
+    """opts (None: the defaults) with pose_fixed set from a boolean mask of W poses; returns (opts, the mask array the
+    pointer refers to, which the caller keeps alive for the call).  pose_fixed None leaves opts as they are."""
+    if pose_fixed is None:
+        return opts, None
+    m = np.ascontiguousarray(np.asarray(pose_fixed, bool), np.uint8)
+    if m.shape != (W,):
+        raise ValueError(f"pose_fixed has shape {m.shape}, expected ({W},)")
+    o = lidar_default_opts() if opts is None else LidarOpts.from_buffer_copy(opts)
+    o.pose_fixed = _p(m, C.c_uint8)
+    return o, m
+
+
+def lidar_lm(vox_ptr, pose_idx, clusters, poses, opts=None, pose_fixed=None):
+    """One-shot drop-in for BALM2::damping_iter (bavoxel.hpp:662).  pose_fixed: boolean mask [W] of constant poses
+    (lvba_lidar_opts::pose_fixed), or None.  Returns (poses, summary dict)."""
     lib = load_library()
     vp = np.ascontiguousarray(vox_ptr, np.int64); pi = np.ascontiguousarray(pose_idx, np.int32)
     cl = _f64(clusters); ps = _f64(poses).copy()
+    opts, mask = _with_pose_fixed(opts, pose_fixed, ps.shape[0])
     s = Summary()
     _chk(lib.lvba_lidar_lm(C.c_int32(ps.shape[0]), C.c_int64(len(vp) - 1), _p(vp, C.c_int64), _p(pi, C.c_int32),
                            _p(cl, C.c_double), _p(ps, C.c_double), C.byref(opts) if opts is not None else None,
@@ -200,13 +216,14 @@ def lidar_lm(vox_ptr, pose_idx, clusters, poses, opts=None):
     return ps, s.as_dict()
 
 
-def lidar_lm_batch(win_ptr, vox_ptr, pose_idx, clusters, poses, min_voxels_per_pose=3, opts=None):
-    """Every window of LvbaSystem::runWindowBA (src/lvba_system.cpp:232-302) in one call.
-    Returns (poses, [per-window summary dict], total summary dict)."""
+def lidar_lm_batch(win_ptr, vox_ptr, pose_idx, clusters, poses, min_voxels_per_pose=3, opts=None, pose_fixed=None):
+    """Every window of LvbaSystem::runWindowBA (src/lvba_system.cpp:232-302) in one call.  pose_fixed: boolean mask over
+    the concatenated poses, or None.  Returns (poses, [per-window summary dict], total summary dict)."""
     lib = load_library()
     wp = np.ascontiguousarray(win_ptr, np.int32)
     vp = np.ascontiguousarray(vox_ptr, np.int64); pi = np.ascontiguousarray(pose_idx, np.int32)
     cl = _f64(clusters); ps = _f64(poses).copy()
+    opts, mask = _with_pose_fixed(opts, pose_fixed, ps.shape[0])
     nw = len(wp) - 1
     sums = (Summary * max(nw, 1))()
     tot = Summary()
@@ -267,6 +284,13 @@ class LidarProblem:
     def solve(self, u):
         dx = np.empty(self.W * 6); _chk(self._lib.lvba_lidar_solve(self._h, C.c_double(u), _p(dx, C.c_double))); return dx
 
+    def rows(self):
+        """pose_of_row [n_rows] (lvba_lidar_rows): the free poses, one row of the pose system each, ascending."""
+        n = C.c_int32(); _chk(self._lib.lvba_lidar_rows(self._h, C.byref(n), None))
+        out = np.empty(n.value, np.int32)
+        _chk(self._lib.lvba_lidar_rows(self._h, C.byref(n), _p(out, C.c_int32)))
+        return out
+
     def structure(self):
         nb = C.c_int64(); _chk(self._lib.lvba_lidar_structure(self._h, C.byref(nb), None, None))
         br = np.empty(nb.value, np.int32); bc = np.empty(nb.value, np.int32)
@@ -274,12 +298,16 @@ class LidarProblem:
         return br, bc
 
     def get_system(self):
+        """(g [n_rows, 6], brow, bcol, blocks): the system over the rows (rows())."""
         br, bc = self.structure()
-        g = np.empty((self.W, 6)); blocks = np.empty((len(br), 6, 6))
+        g = np.empty((len(self.rows()), 6)); blocks = np.empty((len(br), 6, 6))
         _chk(self._lib.lvba_lidar_get_system(self._h, _p(g, C.c_double), _p(blocks, C.c_double)))
         return g, br, bc, blocks
 
-    def reset_lm(self, opts=None):
+    def reset_lm(self, opts=None, pose_fixed=None):
+        """lvba_lidar_reset_lm; pose_fixed: boolean mask [W] of constant poses (a mask that differs from the handle's
+        re-plans it), or None for what opts.pose_fixed says."""
+        opts, mask = _with_pose_fixed(opts, pose_fixed, self.W)
         _chk(self._lib.lvba_lidar_reset_lm(self._h, C.byref(opts) if opts is not None else None))
 
     def reset_state(self):
@@ -522,10 +550,11 @@ class VoxelMap:
                                              _p(o["eigenvalues"], C.c_double)))
         return o
 
-    def lidar_lm(self, poses, min_voxels_per_pose=0, opts=None):
-        """tras_opt + BALM2::damping_iter on the map's voxels without the clusters leaving the device.
-        Returns (poses, summary dict)."""
+    def lidar_lm(self, poses, min_voxels_per_pose=0, opts=None, pose_fixed=None):
+        """tras_opt + BALM2::damping_iter on the map's voxels without the clusters leaving the device.  pose_fixed: boolean
+        mask [W] of constant poses, or None.  Returns (poses, summary dict)."""
         ps = _f64(poses).copy()
+        opts, mask = _with_pose_fixed(opts, pose_fixed, ps.shape[0])
         s = Summary()
         _chk(self._lib.lvba_voxel_map_lidar_lm(self._h, _p(ps, C.c_double), C.c_int32(min_voxels_per_pose),
                                                C.byref(opts) if opts is not None else None, C.byref(s)))
@@ -538,9 +567,11 @@ class VoxelMap:
         _chk(self._lib.lvba_voxel_map_windows(self._h, C.byref(n), _p(w, C.c_int32)))
         return w
 
-    def lidar_lm_batch(self, poses, min_voxels_per_pose=3, opts=None):
-        """runWindowBA's window stage from a windowed map.  Returns (poses, [per-window summary], total)."""
+    def lidar_lm_batch(self, poses, min_voxels_per_pose=3, opts=None, pose_fixed=None):
+        """runWindowBA's window stage from a windowed map.  pose_fixed: boolean mask over the concatenated poses, or None.
+        Returns (poses, [per-window summary], total)."""
         ps = _f64(poses).copy()
+        opts, mask = _with_pose_fixed(opts, pose_fixed, ps.shape[0])
         nw = len(self.win_ptr) - 1
         sums = (Summary * max(nw, 1))()
         tot = Summary()

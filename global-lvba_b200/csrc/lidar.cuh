@@ -54,7 +54,11 @@ struct LidarView {
   const unsigned* pairs;    // li | lj << 16, li < lj slots local to the tile
   const int64_t* tile_drun; // [n_tiles+1] pose runs of every tile
   const int64_t* drun_ptr;  // run r = dslot[drun_ptr[r] .. drun_ptr[r+1]): the slots of one pose
-  const unsigned* dslot;    // slots local to the tile; a tile's items are dslot[s0 .. s0 + ns)
+  const unsigned* dslot;    // slots local to the tile; a tile's items are dslot[s0 .. s0 + ns) (constant poses: see row_of)
+  // constant poses (lvba_lidar_opts::pose_fixed, read by lidar_build_kernel<*, true>): row_of[pose] = its row of the pose
+  // system, -1 for a constant pose.  Slots of constant poses have no pose run, so a tile's slot items are then
+  // dslot[drun_ptr[tile_drun[b]] .. drun_ptr[tile_drun[b + 1]]).
+  const int* row_of;
 };
 
 struct SlotData {
@@ -172,7 +176,10 @@ lidar_residual_kernel(LidarView lv, const double* __restrict__ poses, double* __
 // kDet = false: every run's sum goes into H and g by RED.  kDet = true (deterministic mode): H and g are the records of
 // tiles::FixedSum (lidar_tiles.h) and every run's sum is stored into its own: the pair runs' blocks at H[r], the pose runs'
 // diagonal blocks at H[n_pair_runs + r] and their gradient rows at g[r]; tiles::GatherF adds them up in a fixed order.
-template <bool kDet>
+// kFixed = true (constant poses): phase 1 addresses the envelope and g through lv.row_of.  A slot of a constant pose still
+// enters its voxel's plane and lambda_0; the destination table gives it no pose run and its pairs no pair run, so phases 3-4
+// write nothing for it.  sPose then holds the slot's row (-1: constant).
+template <bool kDet, bool kFixed>
 __global__ void __launch_bounds__(kTileSlots, 512 / kTileSlots)
 lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, double* __restrict__ H,
                    double* __restrict__ g, double* __restrict__ batch_res) {
@@ -196,6 +203,7 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
   const int s0 = lv.vox_ptr[v0], ns = lv.vox_ptr[v1] - s0;
   const int64_t d0 = lv.tile_drun[b];
   const int nd = (int)(lv.tile_drun[b + 1] - d0);
+  const int dbase = kFixed ? (int)lv.drun_ptr[d0] : s0;    // the tile's slot items: dslot[dbase ..)
 
   // ---- phase 1: load + transform
   SlotData s;
@@ -207,14 +215,29 @@ lidar_build_kernel(LidarView lv, EnvView env, const double* __restrict__ poses, 
     transform_cluster(s, out);
 #pragma unroll
     for (int q = 0; q < 10; ++q) stage[tid * kLStage + q] = out[q];
-    sPose[tid] = pose;
-    const long long rs = env.row_start[pose];
-    const int fr = env.first[pose];
-    sRowRS[tid] = rs; sRowFirst[tid] = fr;
-    sDiag[tid] = (rs + (pose - fr)) * 36;
-    sDSlot[tid] = (unsigned short)lv.dslot[s0 + tid];   // the tile's slot items are dslot[s0 .. s0 + ns), grouped by pose
+    if constexpr (kFixed) {
+      const int row = lv.row_of[pose];
+      sPose[tid] = row;
+      if (row >= 0) {
+        const long long rs = env.row_start[row];
+        const int fr = env.first[row];
+        sRowRS[tid] = rs; sRowFirst[tid] = fr;
+        sDiag[tid] = (rs + (row - fr)) * 36;
+      }
+    } else {
+      sPose[tid] = pose;
+      const long long rs = env.row_start[pose];
+      const int fr = env.first[pose];
+      sRowRS[tid] = rs; sRowFirst[tid] = fr;
+      sDiag[tid] = (rs + (pose - fr)) * 36;
+      sDSlot[tid] = (unsigned short)lv.dslot[s0 + tid];   // the tile's slot items are dslot[s0 .. s0 + ns), grouped by pose
+    }
   }
-  for (int r = tid; r <= nd; r += S) sDRun[r] = (unsigned short)(lv.drun_ptr[d0 + r] - s0);
+  if constexpr (kFixed) {                               // the slots with a row, grouped by row
+    const int nds = (int)(lv.drun_ptr[d0 + nd] - dbase);
+    if (tid < nds) sDSlot[tid] = (unsigned short)lv.dslot[dbase + tid];
+  }
+  for (int r = tid; r <= nd; r += S) sDRun[r] = (unsigned short)(lv.drun_ptr[d0 + r] - dbase);
   __syncthreads();
 
   // ---- phase 2: per voxel merge + eigen solve (bavoxel.hpp:97-110)
@@ -437,6 +460,31 @@ __global__ void lidar_retract_kernel(int W, const double* __restrict__ poses, co
   so3_exp(d, E);
   mat3_mul(R, E, Rn);
   double* o = trial + 12 * j;
+#pragma unroll
+  for (int q = 0; q < 9; ++q) o[q] = Rn[q];
+  o[9] = p[9] + d[3]; o[10] = p[10] + d[4]; o[11] = p[11] + d[5];
+}
+
+// the same with constant poses: dx holds the rows of the free poses (row_of[j] = row of pose j, -1: constant), and a constant
+// pose is copied as it is, so that it comes back bit-identical
+__global__ void lidar_retract_rows_kernel(int W, const double* __restrict__ poses, const double* __restrict__ dx,
+                                          const int* __restrict__ row_of, double* __restrict__ trial) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= W) return;
+  const double* p = poses + 12 * j;
+  double* o = trial + 12 * j;
+  const int r = row_of[j];
+  if (r < 0) {
+#pragma unroll
+    for (int q = 0; q < 12; ++q) o[q] = p[q];
+    return;
+  }
+  const double* d = dx + 6 * r;
+  double E[9], R[9], Rn[9];
+#pragma unroll
+  for (int q = 0; q < 9; ++q) R[q] = p[q];
+  so3_exp(d, E);
+  mat3_mul(R, E, Rn);
 #pragma unroll
   for (int q = 0; q < 9; ++q) o[q] = Rn[q];
   o[9] = p[9] + d[3]; o[10] = p[10] + d[4]; o[11] = p[11] + d[5];

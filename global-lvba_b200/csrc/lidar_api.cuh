@@ -132,13 +132,23 @@ struct lvba_lidar_problem {
   // which they are summed, set up when a reset first asks for the mode (lidar_det_setup)
   bool det = false, det_ready = false;
   lvba::tiles::FixedSum<lvba::CudaExec> det_H, det_g;
+  // ---- the rows of the pose system (lvba_lidar_opts::pose_fixed): the free poses in ascending order.  Without a mask every
+  // pose is its own row (n_rows = W; row_of, pose_of_row and d_row_of empty)
+  int n_rows = 0;
+  std::vector<uint8_t> pose_fixed;                 // the handle's constant poses (empty: none)
+  std::vector<int> row_of, pose_of_row;
+  lvba::DevBuf<int> d_row_of;
+  std::vector<int> grp_row_ptr;                    // batched window BA: [G+1] row offsets of the windows
+  lvba::DevBuf<int> d_grp_row_ptr, d_row_grp;      // the same on the device, and the window of every row
+  bool unusable = false;                           // a re-plan failed and so did restoring the previous one (lidar_replan)
   lvba::big::View big_view() const {
-    return lvba::big::View{(int64_t)n_big, big_vox_ptr.p, big_pose.p, big_cl.p, big_pair_ptr.p, env.d_first.p, env.d_row_start.p};
+    return lvba::big::View{(int64_t)n_big, big_vox_ptr.p, big_pose.p, big_cl.p, big_pair_ptr.p, env.d_first.p, env.d_row_start.p,
+                           d_row_of.p, (int64_t)env.nblocks, W};
   }
 
   // the tiles' CSR for the passes of lidar_tiles.h (vox_pair: set by lidar_tables)
   lvba::tiles::TableIn table_in() const {
-    return lvba::tiles::TableIn{n_tiles, W, env.nblocks, tile_vox.p, vox_ptr.p, pidx.p, nullptr, env.d_first.p, env.d_row_start.p};
+    return lvba::tiles::TableIn{n_tiles, W, env.nblocks, tile_vox.p, vox_ptr.p, pidx.p, nullptr, env.d_first.p, env.d_row_start.p, d_row_of.p};
   }
   lvba::LidarView view() const {
     lvba::LidarView v_;
@@ -148,6 +158,7 @@ struct lvba_lidar_problem {
     v_.n_tiles = n_tiles; v_.tile_vox = tile_vox.p;
     v_.tile_prun = prun.tile_run.p; v_.prun_ptr = prun.run_ptr.p; v_.pairs = prun.code.p;
     v_.tile_drun = drun.tile_run.p; v_.drun_ptr = drun.run_ptr.p; v_.dslot = drun.code.p;
+    v_.row_of = d_row_of.p;
     return v_;
   }
   ~lvba_lidar_problem() {
@@ -194,10 +205,93 @@ inline int lidar_validate(int32_t W, int64_t V, const int64_t* vox_ptr, const in
   return LVBA_OK;
 }
 
+// lvba_lidar_opts::pose_fixed as the handle keeps it: W bytes with a nonzero entry, or empty (NULL and all-zero masks)
+inline std::vector<uint8_t> lidar_mask(int W, const uint8_t* pose_fixed) {
+  if (!pose_fixed || std::none_of(pose_fixed, pose_fixed + W, [](uint8_t b) { return b != 0; })) return {};
+  std::vector<uint8_t> m(pose_fixed, pose_fixed + W);
+  for (uint8_t& b : m) b = b != 0;
+  return m;
+}
+
+// constant poses run on one GPU (a voxel's shard follows its lowest pose, whatever is constant; a sharded handle is not re-planned)
+inline int lidar_check_mask(bool has_mask) {
+  if (has_mask && comm().active())
+    return fail(LVBA_ERR_UNSUPPORTED, "pose_fixed runs on one GPU: constant poses are not supported with an active communicator");
+  return LVBA_OK;
+}
+
+// a handle whose failed re-plan could not be undone (lidar_replan) takes no further calls but destroy and the pose copies
+inline int lidar_check_usable(const lvba_lidar_problem* P) {
+  if (P->unusable) return fail(LVBA_ERR_INVALID_ARG, "this handle lost its plan in a failed lvba_lidar_reset_lm: destroy it");
+  return LVBA_OK;
+}
+
+// The rows of the pose system for the constant poses `mask` (empty: none), their envelope over the caller's CSR and, for the
+// single solve, the solver path.  A voxel without a free slot couples no rows; one row system per handle.
+inline int lidar_plan_rows(lvba_lidar_problem* P, const std::vector<uint8_t>& mask, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx) {
+  cudaStream_t s = P->stream;
+  if (mask.empty()) {
+    P->n_rows = P->W;
+    P->row_of.clear(); P->pose_of_row.clear();
+    P->d_row_of.release();
+  } else {
+    P->n_rows = lidar_row_map(P->W, mask.data(), P->row_of, P->pose_of_row);
+    LVBA_TRY(P->d_row_of.upload(P->row_of, s, &P->h2d));
+  }
+  if (P->n_rows > 0) {
+    LVBA_TRY(P->env.build(lidar_first_rows(P->W, V, vox_ptr, pose_idx, mask.empty() ? nullptr : P->row_of.data(), P->n_rows), s, &P->h2d));
+    if (P->n_groups == 0) LVBA_TRY(P->solver.prepare(P->env, s));
+  } else {                                   // every pose constant: no pose system
+    Envelope& e = P->env;
+    e.n = 0; e.nblocks = 0; e.max_col = 0;
+    e.first.clear(); e.last.clear(); e.row_start.clear();
+    e.d_first.release(); e.d_last.release(); e.d_row_start.release();
+  }
+  return LVBA_OK;
+}
+
+// The rest of the plan that follows the rows, once the voxel layout is on the device: the windows' rows and the block-diagonal
+// solver of a batch (a window without a free pose is an empty group), the build's destination table and the row-sized buffers.
+inline int lidar_plan_tables(lvba_lidar_problem* P) {
+  cudaStream_t s = P->stream;
+  if (P->n_groups > 0) {
+    const int G = P->n_groups;
+    for (int g = 0; g < G; ++g)                                // counted in poses, constant ones included
+      if (P->grp_ptr[g + 1] - P->grp_ptr[g] > 31)
+        return fail(LVBA_ERR_UNSUPPORTED, "window %d has %d poses; the batched solve handles <= 31 per window", g, P->grp_ptr[g + 1] - P->grp_ptr[g]);
+    P->grp_row_ptr.assign((size_t)G + 1, 0);
+    std::vector<int> row_grp;
+    row_grp.reserve((size_t)P->n_rows);
+    for (int g = 0; g < G; ++g) {
+      for (int p = P->grp_ptr[g]; p < P->grp_ptr[g + 1]; ++p)
+        if (P->row_of.empty() || P->row_of[p] >= 0) row_grp.push_back(g);
+      P->grp_row_ptr[g + 1] = (int)row_grp.size();
+    }
+    if (P->n_rows > 0) LVBA_TRY(P->solver.prepare(P->env, s, LVBA_SOLVE_AUTO, 0, P->grp_row_ptr));
+    LVBA_TRY(P->d_grp_row_ptr.upload(P->grp_row_ptr, s, &P->h2d));
+    LVBA_TRY(P->d_row_grp.upload(row_grp, s, &P->h2d));
+    LVBA_CUDA(cudaStreamSynchronize(s));                       // row_grp is uploaded
+  }
+  {                                                            // destination table of the build, on the device from the local CSR
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(lidar_tables(ex, P->table_in(), P->V_local, P->n_pairs, P->nnz_local, P->prun, P->drun));
+    P->launches += ex.launches;
+  }
+  LVBA_TRY(P->H.alloc((size_t)P->env.nblocks * 36));
+  LVBA_TRY(P->g.alloc((size_t)P->n_rows * 6));
+  LVBA_TRY(P->diag.alloc((size_t)P->n_rows * 6));
+  LVBA_TRY(P->dadd.alloc((size_t)P->n_rows * 6));
+  LVBA_TRY(P->dx.alloc((size_t)P->n_rows * 6));
+  return LVBA_OK;
+}
+
+// pose_fixed: the constant poses to plan with (null: none; lidar_mask'ed by the caller's opts); the one-shot calls plan once
+// with their mask, a handle starts with none.
 inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
                              const double* clusters, const double* poses, int32_t device,
                              lvba_lidar_problem** out, int32_t n_groups = 0, const int32_t* grp_ptr = nullptr,
-                             const double* d_clusters = nullptr, bool keep_structure = true) {
+                             const double* d_clusters = nullptr, bool keep_structure = true, const uint8_t* pose_fixed = nullptr) {
   // keep_structure: copy the caller's CSR for lvba_lidar_counts (a handle may outlive the caller's arrays); the one-shot calls,
   // whose handle dies before they return, skip the 7 MB of copies
   // d_clusters: the same AoS records already resident on the selected device (a voxel map's export buffer); when set,
@@ -206,6 +300,8 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   *out = nullptr;
   const double t_val0 = wall_ms();
   LVBA_TRY(lidar_validate(W, V, vox_ptr, pose_idx, d_clusters ? d_clusters : clusters, poses));
+  std::vector<uint8_t> mask = lidar_mask(W, pose_fixed);
+  LVBA_TRY(lidar_check_mask(!mask.empty()));
   LVBA_TRY(select_device(device));
   const double t0 = wall_ms();
   SetupLaps lap("lidar setup", 22, nullptr, t_val0);
@@ -244,8 +340,6 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   P->have_structure = keep_structure;
   lap("host copies");
 
-  // ---- envelope structure over ALL voxels (identical on every rank)
-  LVBA_TRY(P->env.build(lidar_first_rows(W, V, vox_ptr, pose_idx), s, &P->h2d));
   Comm& cm = comm();
   const bool sharded = cm.active();
   if (n_groups > 0) {
@@ -253,9 +347,11 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
     P->n_groups = n_groups;
     P->grp_ptr.assign(grp_ptr, grp_ptr + n_groups + 1);
   }
-  // a rank holds the voxels of its poses, cut by the solver's row split: the solver is prepared first.  The batched solve (one
-  // GPU) is prepared after the layout, which checks that no voxel spans two windows.
-  if (n_groups == 0) LVBA_TRY(P->solver.prepare(P->env, s));
+  // ---- rows and their envelope over ALL voxels (identical on every rank).  A rank holds the voxels of its poses, cut by the
+  // solver's row split: the solver is prepared first.  The batched solve (one GPU) is prepared after the layout, which checks
+  // that no voxel spans two windows (lidar_plan_tables).
+  P->pose_fixed = std::move(mask);
+  LVBA_TRY(lidar_plan_rows(P.get(), P->pose_fixed, V, vox_ptr, pose_idx));
   lap("envelope+solver alloc");
 
   // ---- shard: voxel -> owner of its lowest pose index (SURVEY.md §8e)
@@ -279,7 +375,6 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   P->n_batches = (int)L.batch_vox.size() - 1;
   P->n_tiles = (int)L.tile_vox.size() - 1;
   if (n_groups > 0) {
-    LVBA_TRY(P->solver.prepare(P->env, s, LVBA_SOLVE_AUTO, 0, P->grp_ptr));
     P->grp_V = L.grp_V;
     LVBA_TRY(P->d_grp_batch.upload(L.grp_batch, s, &P->h2d));
     LVBA_TRY(P->d_grp_tile.upload(L.grp_tile, s, &P->h2d));
@@ -341,25 +436,16 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
   if (L.identity) LVBA_TRY(P->pidx.upload(reinterpret_cast<const int*>(pose_idx), (size_t)nnz, s, &P->h2d));
   LVBA_TRY(P->batch_vox.upload(L.batch_vox, s, &P->h2d));
   LVBA_TRY(P->tile_vox.upload(L.tile_vox, s, &P->h2d));
-  {                                                            // destination table of the build, on the device from the CSR just uploaded
-    CudaExec ex;
-    ex.stream = s;
-    LVBA_TRY(lidar_tables(ex, P->table_in(), Vl, L.n_pairs, nnz, P->prun, P->drun));
-    P->launches += ex.launches;
-  }
+  LVBA_TRY(lidar_plan_tables(P.get()));                       // destination table from the CSR just uploaded, row buffers
   lap("destination table");
   LVBA_TRY(P->poses.upload(poses, (size_t)W * 12, s, &P->h2d));
   LVBA_TRY(P->poses0.upload(poses, (size_t)W * 12, s));
   LVBA_TRY(P->trial.alloc((size_t)W * 12));
-  LVBA_TRY(P->H.alloc((size_t)P->env.nblocks * 36));
-  LVBA_TRY(P->g.alloc((size_t)W * 6));
-  LVBA_TRY(P->diag.alloc((size_t)W * 6));
-  LVBA_TRY(P->dadd.alloc((size_t)W * 6));
-  LVBA_TRY(P->dx.alloc((size_t)W * 6));
   LVBA_TRY(P->batch_res.alloc((size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1)));
   LVBA_TRY(P->scal.alloc(8));
   LVBA_TRY(P->scal.zero(s));
-  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
   LVBA_CUDA(cudaStreamSynchronize(s));
   aos.release();                                               // the caller's records were consumed by the kernels above
   lap("index upload+allocs");
@@ -377,16 +463,63 @@ inline int lidar_det_setup(lvba_lidar_problem* P) {
   CudaExec ex;
   ex.stream = P->stream;
   LVBA_TRY(lidar_det_index(ex, P->table_in(), P->prun, P->drun, P->big_view(), P->n_big_slots, P->n_big_pairs, P->det_H, P->det_g));
-  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
+  LVBA_CUDA(cudaFuncSetAttribute(lidar_build_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)lidar_build_smem_bytes()));
   P->launches += ex.launches;
   P->det_ready = true;
   return LVBA_OK;
 }
 
-// the LM mode of the handle (lvba_lidar_reset_lm and the one-shot calls)
+// A new set of constant poses on a handle (lvba_lidar_reset_lm): the rows, the envelope, the solver, the build's tables and the
+// row-sized buffers again, from the handle's host copy of the caller's CSR.  The voxel layout does not depend on the rows
+// (voxels stay in the order of their lowest pose), so the clusters, batches and tiles stay as they are on the device.  The
+// result equals a fresh one-shot call with that mask, bit for bit in deterministic mode.  One GPU only (lidar_check_mask).
+// A failure leaves the handle as it was (the previous plan is made again) with deterministic mode off; only if that fails too
+// is the handle marked unusable, and then every call but destroy and the pose copies refuses it.
+inline int lidar_replan(lvba_lidar_problem* P, std::vector<uint8_t> mask) {
+  if (!P->have_structure) return fail(LVBA_ERR_UNSUPPORTED, "this problem was created without its host-side structure copy: it cannot be re-planned");
+  cudaStream_t s = P->stream;
+  LVBA_CUDA(cudaStreamSynchronize(s));                         // nothing in flight reads the buffers re-planned below
+  // the records of deterministic mode follow the table: set up again when the mode is next asked for (lidar_set_mode)
+  tiles::fixed_sum_release(P->det_H); tiles::fixed_sum_release(P->det_g);
+  P->det_ready = false;
+  P->det = false;
+  P->solver.set_deterministic(false);
+  static_assert(sizeof(long long) == sizeof(int64_t), "the host copy of vox_ptr is read as it is");
+  auto plan_with = [&](const std::vector<uint8_t>& m) -> int {
+    LVBA_TRY(lidar_plan_rows(P, m, P->V_total, reinterpret_cast<const int64_t*>(P->h_vox_ptr_all.data()), P->h_pose_idx_all.data()));
+    LVBA_TRY(lidar_plan_tables(P));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    return LVBA_OK;
+  };
+  int rc;
+  try { rc = plan_with(mask); } catch (const std::bad_alloc&) { rc = fail(LVBA_ERR_NOMEM, "host allocation failed"); }
+  if (rc != LVBA_OK) {
+    const std::string why = last_error_ref();
+    cudaStreamSynchronize(s);
+    cudaGetLastError();
+    int rc_back;
+    try { rc_back = plan_with(P->pose_fixed); } catch (const std::bad_alloc&) { rc_back = LVBA_ERR_NOMEM; }
+    if (rc_back != LVBA_OK) {
+      P->unusable = true;
+      return fail(rc, "re-plan for the new pose_fixed failed (%s), and so did restoring the previous plan: destroy the handle", why.c_str());
+    }
+    return fail(rc, "re-plan for the new pose_fixed failed (%s); the handle keeps its previous constant poses", why.c_str());
+  }
+  P->pose_fixed = std::move(mask);
+  return LVBA_OK;
+}
+
+// the LM mode of the handle (lvba_lidar_reset_lm and the one-shot calls): the constant poses and deterministic mode
 inline int lidar_set_mode(lvba_lidar_problem* P, const lvba_lidar_opts& o) {
   if (o.deterministic && comm().active())
     return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode runs on one GPU: the multi-GPU sums of NCCL have no fixed order");
+  std::vector<uint8_t> mask = lidar_mask(P->W, o.pose_fixed);
+  LVBA_TRY(lidar_check_mask(!mask.empty() || !P->pose_fixed.empty()));
+  if (mask != P->pose_fixed) {
+    LVBA_CUDA(cudaSetDevice(P->device));
+    LVBA_TRY(lidar_replan(P, std::move(mask)));
+  }
   if (o.deterministic) {
     LVBA_CUDA(cudaSetDevice(P->device));
     const int rc = lidar_det_setup(P);
@@ -426,12 +559,14 @@ inline int lidar_build_hg(lvba_lidar_problem* P, const double* d_poses) {
   LVBA_TRY(P->H.zero(s));
   LVBA_TRY(P->g.zero(s));
   if (P->n_tiles > 0) {
-    if (P->det)
-      lidar_build_kernel<true><<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->det_H.rec.p,
-                                                                                         P->det_g.rec.p, P->batch_res.p);
-    else
-      lidar_build_kernel<false><<<P->n_tiles, kTileSlots, lidar_build_smem_bytes(), s>>>(P->view(), P->env.view(), d_poses, P->H.p, P->g.p,
-                                                                                          P->batch_res.p);
+    const bool fixed = !P->pose_fixed.empty();
+    double* H = P->det ? P->det_H.rec.p : P->H.p;
+    double* g = P->det ? P->det_g.rec.p : P->g.p;
+    const unsigned smem = (unsigned)lidar_build_smem_bytes();
+    if (P->det && fixed) lidar_build_kernel<true, true><<<P->n_tiles, kTileSlots, smem, s>>>(P->view(), P->env.view(), d_poses, H, g, P->batch_res.p);
+    else if (P->det) lidar_build_kernel<true, false><<<P->n_tiles, kTileSlots, smem, s>>>(P->view(), P->env.view(), d_poses, H, g, P->batch_res.p);
+    else if (fixed) lidar_build_kernel<false, true><<<P->n_tiles, kTileSlots, smem, s>>>(P->view(), P->env.view(), d_poses, H, g, P->batch_res.p);
+    else lidar_build_kernel<false, false><<<P->n_tiles, kTileSlots, smem, s>>>(P->view(), P->env.view(), d_poses, H, g, P->batch_res.p);
     ++P->launches;
   }
   if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/false, P->n_tiles));
@@ -480,10 +615,14 @@ inline int lidar_residual_dev(lvba_lidar_problem* P, const double* d_poses, int 
   return LVBA_OK;
 }
 
-// (H + u diag(H)) dx = -g ; q1 ; leaves dx on the device.  scal[1] = q1, scal[2] = non-finite flag
+// (H + u diag(H)) dx = -g over the rows ; q1 ; leaves dx on the device.  scal[1] = q1, scal[2] = non-finite flag
 inline int lidar_solve_dev(lvba_lidar_problem* P, double u) {
   cudaStream_t s = P->stream;
-  const int n6 = 6 * P->W;
+  if (P->n_rows == 0) {                                      // every pose constant: nothing to solve, q1 = 0
+    LVBA_CUDA(cudaMemsetAsync(P->scal.p + 1, 0, 2 * sizeof(double), s));
+    return LVBA_OK;
+  }
+  const int n6 = 6 * P->n_rows;
   const EnvView ev = P->env.view();
   env_get_diag_kernel<<<(n6 + 255) / 256, 256, 0, s>>>(ev, P->H.p, P->diag.p);
   if (P->solver.dist()) {                                    // a rank holds the rows it owns: the diagonal of the others arrives by all-reduce
@@ -502,10 +641,20 @@ inline int lidar_solve_dev(lvba_lidar_problem* P, double u) {
 
 inline int lidar_fetch_scal(lvba_lidar_problem* P) {
   LVBA_CUDA(cudaMemcpyAsync(P->h_scal, P->scal.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, P->stream));
-  LVBA_CUDA(cudaMemcpyAsync(P->h_scal + 7, P->solver.status.p, sizeof(int), cudaMemcpyDeviceToHost, P->stream));
+  if (P->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(P->h_scal + 7, P->solver.status.p, sizeof(int), cudaMemcpyDeviceToHost, P->stream));
+  else memset(P->h_scal + 7, 0, sizeof(int));                // no solver ran: a status of 0
   LVBA_CUDA(cudaStreamSynchronize(P->stream));
   P->d2h += 8 * sizeof(double) + sizeof(int);
   return LVBA_OK;
+}
+
+// trial = poses (+) dx, constant poses copied as they are
+inline void lidar_retract(lvba_lidar_problem* P) {
+  if (P->pose_fixed.empty())
+    lidar_retract_kernel<<<(P->W + 127) / 128, 128, 0, P->stream>>>(P->W, P->poses.p, P->dx.p, P->trial.p);
+  else
+    lidar_retract_rows_kernel<<<(P->W + 127) / 128, 128, 0, P->stream>>>(P->W, P->poses.p, P->dx.p, P->d_row_of.p, P->trial.p);
+  ++P->launches;
 }
 
 // n passes of the damping_iter loop body (bavoxel.hpp:686-766)
@@ -515,6 +664,15 @@ inline int lidar_iterate_impl(lvba_lidar_problem* P, int n_iter, lvba_summary* s
   const double V = (double)P->V_total;
   BalmState& lm = P->lm;
   const int iters0 = lm.iters, acc0 = lm.accepted, builds0 = P->builds;
+  if (P->n_rows == 0 && n_iter > 0 && !lm.converged) {       // every pose constant: the residual once, nothing to solve (Ceres:
+    P->timers.begin(PH_RESID);                               // no free parameter block, function tolerance)
+    LVBA_TRY(lidar_residual_dev(P, P->poses.p, 3));
+    P->timers.end();
+    LVBA_TRY(lidar_fetch_scal(P));
+    lm.cost_first = lm.cost_last = lm.residual1 = P->h_scal[3] / V;
+    lm.have_first = lm.converged = true;
+    lm.term = LVBA_TERM_FUNCTION_TOL;
+  }
   for (int it = 0; it < n_iter && !lm.converged; ++it) {
     if (P->is_calc_hess) {                                   // divide_thread, :688-689
       P->timers.begin(PH_BUILD);
@@ -526,8 +684,7 @@ inline int lidar_iterate_impl(lvba_lidar_problem* P, int n_iter, lvba_summary* s
     LVBA_TRY(lidar_solve_dev(P, lm.u));                      // :692-710, :729
     P->timers.end();
     P->timers.begin(PH_RESID);
-    lidar_retract_kernel<<<(P->W + 127) / 128, 128, 0, P->stream>>>(P->W, P->poses.p, P->dx.p, P->trial.p);   // :722-727
-    ++P->launches;
+    lidar_retract(P);                                        // :722-727
     LVBA_TRY(lidar_residual_dev(P, P->trial.p, 3));          // only_residual, :731
     P->timers.end();
     LVBA_TRY(lidar_fetch_scal(P));
@@ -559,16 +716,38 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
   std::vector<double> u_host((size_t)G);
   std::vector<int> acc_host((size_t)G);
   int n_active = 0;
+  bool any_constant = false;
   for (int g = 0; g < G; ++g) {
-    const int Wg = P->grp_ptr[g + 1] - P->grp_ptr[g];
+    const int Wg = P->grp_ptr[g + 1] - P->grp_ptr[g];       // the skip rule counts every pose of the window, constant ones included
     WinState& w = ws[g];
     w.reset(P->opts);
     w.skipped = Wg <= 0 || P->grp_V[g] == 0 || P->grp_V[g] < (long long)min_voxels_per_pose * Wg;   // src/lvba_system.cpp:262-266
-    w.active = !w.skipped;
+    w.active = !w.skipped && P->grp_row_ptr[g + 1] > P->grp_row_ptr[g];
     if (w.skipped) w.term = LVBA_TERM_SKIPPED;
+    any_constant = any_constant || (!w.skipped && !w.active);
     n_active += w.active;
   }
-  const int n6 = 6 * P->W;
+  if (any_constant) {                                          // windows whose poses are all constant: their residual once
+    P->timers.begin(PH_RESID);
+    if (P->n_batches > 0) {
+      lidar_residual_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->poses.p, P->batch_res.p);
+      ++P->launches;
+    }
+    lidar_group_sum_kernel<<<G, 128, 0, s>>>(P->batch_res.p, P->d_grp_batch.p, P->d_grp_scal.p, 3);
+    ++P->launches;
+    P->timers.end();
+    LVBA_CUDA(cudaMemcpyAsync(P->h_grp_scal, P->d_grp_scal.p, (size_t)4 * G * sizeof(double), cudaMemcpyDeviceToHost, s));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    P->d2h += (int64_t)G * 32;
+    for (int g = 0; g < G; ++g) {
+      WinState& w = ws[g];
+      if (w.skipped || w.active) continue;
+      w.cost_first = w.cost_last = w.residual1 = P->h_grp_scal[4 * g + 3] / (double)P->grp_V[g];
+      w.have_first = w.converged = true;
+      w.term = LVBA_TERM_FUNCTION_TOL;
+    }
+  }
+  const int n6 = 6 * P->n_rows;
   const EnvView ev = P->env.view();
   int passes = 0;
   for (int it = 0; it < P->opts.max_iter && n_active > 0; ++it, ++passes) {
@@ -585,16 +764,15 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
     // ---- (H + u_w diag(H)) dx = -g, q1 per window
     P->timers.begin(PH_SOLVE);
     env_get_diag_kernel<<<(n6 + 255) / 256, 256, 0, s>>>(ev, P->H.p, P->diag.p);
-    lidar_rhs_grouped_kernel<<<(n6 + 255) / 256, 256, 0, s>>>(n6, P->g.p, P->diag.p, P->d_u_grp.p, P->d_pose_grp.p, P->solver.z.p, P->dadd.p);
+    lidar_rhs_grouped_kernel<<<(n6 + 255) / 256, 256, 0, s>>>(n6, P->g.p, P->diag.p, P->d_u_grp.p, P->d_row_grp.p, P->solver.z.p, P->dadd.p);
     P->launches += 2;
     LVBA_TRY(P->solver.solve(P->env, P->H.p, P->dadd.p, P->dx.p, s, &P->launches));
-    lidar_q1_grouped_kernel<<<G, 128, 0, s>>>(P->d_grp_ptr.p, P->dx.p, P->diag.p, P->g.p, P->d_u_grp.p, P->solver.status.p, P->d_grp_scal.p);
+    lidar_q1_grouped_kernel<<<G, 128, 0, s>>>(P->d_grp_row_ptr.p, P->dx.p, P->diag.p, P->g.p, P->d_u_grp.p, P->solver.status.p, P->d_grp_scal.p);
     ++P->launches;
     P->timers.end();
     // ---- trial state and its residual per window
     P->timers.begin(PH_RESID);
-    lidar_retract_kernel<<<(P->W + 127) / 128, 128, 0, s>>>(P->W, P->poses.p, P->dx.p, P->trial.p);
-    ++P->launches;
+    lidar_retract(P);
     if (P->n_batches > 0) {
       lidar_residual_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->trial.p, P->batch_res.p);
       ++P->launches;
@@ -663,6 +841,7 @@ extern "C" {
 void lvba_lidar_default_opts(lvba_lidar_opts* o) {
   if (!o) return;
   o->u0 = 0.01; o->v0 = 2.0; o->max_iter = 10; o->rel_tol = 1e-6; o->device = -1; o->verbose = 0; o->deterministic = 0;
+  o->pose_fixed = nullptr;
 }
 
 int lvba_lidar_create(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
@@ -696,6 +875,7 @@ int lvba_lidar_get_poses(lvba_lidar_problem* p, double* poses) LVBA_ABI_BEGIN {
 
 int lvba_lidar_build(lvba_lidar_problem* p, double* residual_sum) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   LVBA_TRY(lvba::lidar_build_dev(p, p->poses.p, 0));
   LVBA_TRY(lvba::lidar_fetch_scal(p));
@@ -705,6 +885,7 @@ int lvba_lidar_build(lvba_lidar_problem* p, double* residual_sum) LVBA_ABI_BEGIN
 
 int lvba_lidar_residual(lvba_lidar_problem* p, const double* poses, double* residual_sum) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   const double* dp = p->poses.p;
   if (poses) {
@@ -719,16 +900,35 @@ int lvba_lidar_residual(lvba_lidar_problem* p, const double* poses, double* resi
 
 int lvba_lidar_solve(lvba_lidar_problem* p, double u, double* dx) LVBA_ABI_BEGIN {
   if (!p || !dx) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   LVBA_TRY(lvba::lidar_solve_dev(p, u));
-  LVBA_CUDA(cudaMemcpyAsync(dx, p->dx.p, (size_t)p->W * 6 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
-  LVBA_TRY(lvba::lidar_fetch_scal(p));
-  p->d2h += (int64_t)p->W * 48;
+  if (p->pose_fixed.empty()) {
+    LVBA_CUDA(cudaMemcpyAsync(dx, p->dx.p, (size_t)p->W * 6 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    LVBA_TRY(lvba::lidar_fetch_scal(p));
+  } else {                                                    // the rows' steps, zeros for the constant poses
+    std::vector<double> dr((size_t)p->n_rows * 6);
+    if (p->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(dr.data(), p->dx.p, dr.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+    LVBA_TRY(lvba::lidar_fetch_scal(p));
+    std::fill(dx, dx + (size_t)p->W * 6, 0.0);
+    for (int r = 0; r < p->n_rows; ++r) std::copy(dr.begin() + 6 * r, dr.begin() + 6 * r + 6, dx + 6 * (size_t)p->pose_of_row[r]);
+  }
+  p->d2h += (int64_t)p->n_rows * 48;
   return LVBA_OK;
 } LVBA_ABI_END("lvba_lidar_solve")
 
+int lvba_lidar_rows(lvba_lidar_problem* p, int32_t* n_rows, int32_t* pose_of_row) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
+  if (n_rows) *n_rows = p->n_rows;
+  if (pose_of_row)
+    for (int r = 0; r < p->n_rows; ++r) pose_of_row[r] = p->pose_fixed.empty() ? r : p->pose_of_row[r];
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_lidar_rows")
+
 int lvba_lidar_structure(lvba_lidar_problem* p, int64_t* nblocks, int32_t* brow, int32_t* bcol) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   if (nblocks) *nblocks = p->env.nblocks;
   if (brow && bcol) {
     for (int r = 0; r < p->env.n; ++r)
@@ -742,15 +942,17 @@ int lvba_lidar_structure(lvba_lidar_problem* p, int64_t* nblocks, int32_t* brow,
 
 int lvba_lidar_get_system(lvba_lidar_problem* p, double* g, double* blocks) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
-  if (g) LVBA_CUDA(cudaMemcpyAsync(g, p->g.p, (size_t)p->W * 6 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
-  if (blocks) LVBA_CUDA(cudaMemcpyAsync(blocks, p->H.p, (size_t)p->env.nblocks * 36 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  if (g && p->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(g, p->g.p, (size_t)p->n_rows * 6 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  if (blocks && p->env.nblocks > 0) LVBA_CUDA(cudaMemcpyAsync(blocks, p->H.p, (size_t)p->env.nblocks * 36 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
   LVBA_CUDA(cudaStreamSynchronize(p->stream));
   return LVBA_OK;
 } LVBA_ABI_END("lvba_lidar_get_system")
 
 int lvba_lidar_reset_lm(lvba_lidar_problem* p, const lvba_lidar_opts* opts) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   lvba_lidar_opts o;
   if (opts) o = *opts; else lvba_lidar_default_opts(&o);
   LVBA_TRY(lvba::lidar_set_mode(p, o));
@@ -770,25 +972,41 @@ int lvba_lidar_reset_state(lvba_lidar_problem* p) LVBA_ABI_BEGIN {
 
 int lvba_lidar_iterate(lvba_lidar_problem* p, int32_t n_iter, lvba_summary* summary) LVBA_ABI_BEGIN {
   if (!p || n_iter < 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "bad argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
   return lvba::lidar_iterate_impl(p, n_iter, summary);
 } LVBA_ABI_END("lvba_lidar_iterate")
 
 int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env, int64_t* n_blocks_nonzero, int64_t* n_pairs) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_usable(p));
   if (!p->have_structure) return lvba::fail(LVBA_ERR_UNSUPPORTED, "this problem was created without its host-side structure copy");
   if (nnz) *nnz = (int64_t)p->h_pose_idx_all.size();
   if (n_blocks_env) *n_blocks_env = p->env.nblocks;
   int64_t np = 0;
   std::unordered_set<uint64_t> seen;
   const bool want_nz = n_blocks_nonzero != nullptr;
-  for (int64_t a = 0; a < p->V_total; ++a) {
-    const int64_t lo = p->h_vox_ptr_all[a], hi = p->h_vox_ptr_all[a + 1];
-    np += (hi - lo) * (hi - lo - 1) / 2;
-    if (want_nz)
-      for (int64_t x = lo; x < hi; ++x)
-        for (int64_t y = x; y < hi; ++y)
-          seen.insert(((uint64_t)p->h_pose_idx_all[x] << 32) | (uint32_t)p->h_pose_idx_all[y]);
+  if (p->pose_fixed.empty()) {
+    for (int64_t a = 0; a < p->V_total; ++a) {
+      const int64_t lo = p->h_vox_ptr_all[a], hi = p->h_vox_ptr_all[a + 1];
+      np += (hi - lo) * (hi - lo - 1) / 2;
+      if (want_nz)
+        for (int64_t x = lo; x < hi; ++x)
+          for (int64_t y = x; y < hi; ++y)
+            seen.insert(((uint64_t)p->h_pose_idx_all[x] << 32) | (uint32_t)p->h_pose_idx_all[y]);
+    }
+  } else {                                                    // the row system: pairs and blocks of free poses only
+    std::vector<int> rows;
+    for (int64_t a = 0; a < p->V_total; ++a) {
+      rows.clear();
+      for (int64_t x = p->h_vox_ptr_all[a]; x < p->h_vox_ptr_all[a + 1]; ++x)
+        if (p->row_of[p->h_pose_idx_all[x]] >= 0) rows.push_back(p->row_of[p->h_pose_idx_all[x]]);
+      const int64_t k = (int64_t)rows.size();
+      np += k * (k - 1) / 2;
+      if (want_nz)
+        for (int64_t x = 0; x < k; ++x)
+          for (int64_t y = x; y < k; ++y) seen.insert(((uint64_t)rows[x] << 32) | (uint32_t)rows[y]);
+    }
   }
   if (n_pairs) *n_pairs = np;
   if (want_nz) *n_blocks_nonzero = (int64_t)seen.size();
@@ -801,7 +1019,8 @@ int lvba_lidar_lm(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* p
   lvba_lidar_opts o;
   if (opts) o = *opts; else lvba_lidar_default_opts(&o);
   lvba_lidar_problem* p = nullptr;
-  LVBA_TRY(lvba::lidar_create_impl(W, V, vox_ptr, pose_idx, clusters, poses, o.device, &p, 0, nullptr, nullptr, /*keep_structure=*/false));
+  LVBA_TRY(lvba::lidar_create_impl(W, V, vox_ptr, pose_idx, clusters, poses, o.device, &p, 0, nullptr, nullptr, /*keep_structure=*/false,
+                                    o.pose_fixed));
   return lvba::lm_one_shot(p, o, V > 0, lvba_lidar_reset_lm, lvba_lidar_iterate, lvba_lidar_destroy,
                            [&] { return lvba_lidar_get_poses(p, poses); }, t0, summary);     // x_stats written back only on success
 } LVBA_ABI_END("lvba_lidar_lm")
@@ -818,7 +1037,8 @@ int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, co
   lvba_lidar_opts o;
   if (opts) o = *opts; else lvba_lidar_default_opts(&o);
   lvba_lidar_problem* p = nullptr;
-  LVBA_TRY(lvba::lidar_create_impl(win_ptr[n_windows], V, vox_ptr, pose_idx, clusters, poses, o.device, &p, n_windows, win_ptr));
+  LVBA_TRY(lvba::lidar_create_impl(win_ptr[n_windows], V, vox_ptr, pose_idx, clusters, poses, o.device, &p, n_windows, win_ptr, nullptr, true,
+                                    o.pose_fixed));
   return lvba::lidar_batch_one_shot(p, o, min_voxels_per_pose, poses, summaries, total, t0, "lvba_lidar_lm_batch");
 } LVBA_ABI_END("lvba_lidar_lm_batch")
 

@@ -45,7 +45,15 @@ struct View {
   // envelope of the pose system
   const int* first;
   const long long* row_start;
+  // constant poses (lvba_lidar_opts::pose_fixed): row_of[pose] = its row, -1 for a constant pose; null: every pose is its own
+  // row.  A slot or pair of a constant pose adds nothing to H and g; its deterministic record gets no destination (nblocks
+  // for H, W for g: the destination counts of tiles::FixedSum in lidar_det_index).
+  const int* row_of = nullptr;
+  int64_t nblocks = 0;
+  int W = 0;
 };
+
+LVBA_BHD int row_of_pose(const View& bv, int pose) { return bv.row_of ? bv.row_of[pose] : pose; }
 
 LVBA_BHD void mat3_mul(const double* A, const double* B, double* C) {
   for (int i = 0; i < 3; ++i)
@@ -194,9 +202,11 @@ struct SlotsPass {             // one item per slot of the big voxels
       for (int i = 0; i < 36; ++i) H[36 * s + i] = Hd[i];
       for (int j = 0; j < 6; ++j) g[6 * s + j] = jjt[j];
     } else {
-      double* Hb = H + (bv.row_start[pose] + (pose - bv.first[pose])) * 36;
+      const int row = row_of_pose(bv, pose);
+      if (row < 0) return;
+      double* Hb = H + (bv.row_start[row] + (row - bv.first[row])) * 36;
       for (int i = 0; i < 36; ++i) atomic_add_f64(Hb + i, Hd[i]);
-      for (int j = 0; j < 6; ++j) atomic_add_f64(g + 6 * (int64_t)pose + j, jjt[j]);
+      for (int j = 0; j < 6; ++j) atomic_add_f64(g + 6 * (int64_t)row + j, jjt[j]);
     }
   }
 };
@@ -243,7 +253,8 @@ struct PairsPass {             // one item per slot pair (i < j) of the big voxe
       for (int r = 0; r < 6; ++r)
         for (int c = 0; c < 6; ++c) H[36 * p + 6 * c + r] = Hb[6 * r + c];
     } else {
-      const int pi = bv.pose_idx[si], pj = bv.pose_idx[sj];           // ascending inside a voxel: pi < pj
+      const int pi = row_of_pose(bv, bv.pose_idx[si]), pj = row_of_pose(bv, bv.pose_idx[sj]);   // ascending inside a voxel: pi < pj
+      if (pi < 0 || pj < 0) return;
       double* B = H + (bv.row_start[pj] + (pi - bv.first[pj])) * 36;  // lower block (pj, pi) = Hb^T   (:171-173)
       for (int r = 0; r < 6; ++r)
         for (int c = 0; c < 6; ++c) atomic_add_f64(B + 6 * c + r, Hb[6 * r + c]);
@@ -261,9 +272,9 @@ using PairsDetF = PairsPass<true>;
 struct SlotDstF {
   View bv; int64_t* dst_H; int64_t* dst_g;
   LVBA_BHD void operator()(int64_t s) const {
-    const int pose = bv.pose_idx[s];
-    dst_H[s] = bv.row_start[pose] + (pose - bv.first[pose]);
-    dst_g[s] = pose;
+    const int row = row_of_pose(bv, bv.pose_idx[s]);
+    dst_H[s] = row < 0 ? bv.nblocks : bv.row_start[row] + (row - bv.first[row]);
+    dst_g[s] = row < 0 ? bv.W : row;
   }
 };
 struct PairDstF {
@@ -271,8 +282,8 @@ struct PairDstF {
   LVBA_BHD void operator()(int64_t p) const {
     int64_t lo, si, sj;
     pair_slots(bv, p, lo, si, sj);
-    const int pi = bv.pose_idx[si], pj = bv.pose_idx[sj];
-    dst_H[p] = bv.row_start[pj] + (pi - bv.first[pj]);
+    const int pi = row_of_pose(bv, bv.pose_idx[si]), pj = row_of_pose(bv, bv.pose_idx[sj]);
+    dst_H[p] = (pi < 0 || pj < 0) ? bv.nblocks : bv.row_start[pj] + (pi - bv.first[pj]);
   }
 };
 

@@ -18,22 +18,40 @@
 
 namespace lvba {
 
-// The raw envelope of the pose system: first[r] = the lowest pose that shares a voxel with pose r (r when there is none).
-// Clique minima over the caller's CSR in parallel chunks, one row array per worker.
-inline std::vector<int> lidar_first_rows(int W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx) {
-  std::vector<int> first(W);
-  for (int r = 0; r < W; ++r) first[r] = r;
-  std::vector<int> first_w((size_t)kMaxSetupThreads * (size_t)W);
-  for (int w = 0; w < kMaxSetupThreads; ++w) std::copy(first.begin(), first.end(), first_w.begin() + (size_t)w * (size_t)W);
+// The rows of the pose system under constant poses (lvba_lidar_opts::pose_fixed, mask: W bytes or null): the free poses in
+// ascending order.  row_of[pose] = its row, -1 for a constant pose; pose_of_row its inverse.  Returns the number of rows.
+inline int lidar_row_map(int W, const uint8_t* mask, std::vector<int>& row_of, std::vector<int>& pose_of_row) {
+  row_of.assign((size_t)W, -1);
+  pose_of_row.clear();
+  for (int p = 0; p < W; ++p)
+    if (!mask || !mask[p]) { row_of[p] = (int)pose_of_row.size(); pose_of_row.push_back(p); }
+  return (int)pose_of_row.size();
+}
+
+// The raw envelope of the pose system: first[r] = the lowest row that shares a voxel with row r (r when there is none).
+// Clique minima over the caller's CSR in parallel chunks, one row array per worker.  row_of (lidar_row_map, n_rows rows): the
+// rows of the free poses, a voxel's constant slots couple nothing; null: every pose is its own row (n_rows = W).
+inline std::vector<int> lidar_first_rows(int W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx, const int* row_of = nullptr,
+                                         int n_rows = -1) {
+  const int n = row_of ? n_rows : W;
+  auto row = [&](int64_t q) { return row_of ? row_of[pose_idx[q]] : pose_idx[q]; };
+  std::vector<int> first(n);
+  for (int r = 0; r < n; ++r) first[r] = r;
+  std::vector<int> first_w((size_t)kMaxSetupThreads * (size_t)n);
+  for (int w = 0; w < kMaxSetupThreads; ++w) std::copy(first.begin(), first.end(), first_w.begin() + (size_t)w * (size_t)n);
   parallel_chunks(V, 1 << 14, [&](int64_t a0, int64_t a1, int w) {
-    int* fr = first_w.data() + (size_t)w * (size_t)W;
+    int* fr = first_w.data() + (size_t)w * (size_t)n;
     for (int64_t a = a0; a < a1; ++a) {
-      const int m = pose_idx[vox_ptr[a]];
-      for (int64_t q = vox_ptr[a]; q < vox_ptr[a + 1]; ++q) fr[pose_idx[q]] = std::min(fr[pose_idx[q]], m);
+      int64_t q0 = vox_ptr[a];                                 // the voxel's lowest free row (ascending poses: ascending rows)
+      while (q0 < vox_ptr[a + 1] && row(q0) < 0) ++q0;
+      if (q0 == vox_ptr[a + 1]) continue;
+      const int m = row(q0);
+      for (int64_t q = q0; q < vox_ptr[a + 1]; ++q)
+        if (row(q) >= 0) fr[row(q)] = std::min(fr[row(q)], m);
     }
   });
   for (int w = 0; w < kMaxSetupThreads; ++w)
-    for (int r = 0; r < W; ++r) first[r] = std::min(first[r], first_w[(size_t)w * (size_t)W + r]);
+    for (int r = 0; r < n; ++r) first[r] = std::min(first[r], first_w[(size_t)w * (size_t)n + r]);
   return first;
 }
 

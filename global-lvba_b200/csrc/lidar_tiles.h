@@ -71,9 +71,14 @@ struct TableIn {
   const int* vox_ptr;           // [V + 1] slot offsets (the tiles' voxel order)
   const int* pidx;              // [nnz] pose of every slot
   const long long* vox_pair;    // [V + 1] prefix sums of K (K - 1) / 2
-  const int* first;             // envelope first[] per pose row
-  const long long* row_start;   // envelope row_start[] per pose row
+  const int* first;             // envelope first[] per row
+  const long long* row_start;   // envelope row_start[] per row
+  // constant poses (lvba_lidar_opts::pose_fixed): row_of[pose] = its row of the pose system, -1 for a constant pose; null: every
+  // pose is its own row.  A pair or slot of a constant pose has no destination.
+  const int* row_of = nullptr;
 };
+
+LVBA_THD int row_of_pose(const TableIn& q, int pose) { return q.row_of ? q.row_of[pose] : pose; }
 
 // items 0..V: cnt[i] = pose pairs of local voxel i (0 for i = V); its exclusive scan is TableIn::vox_pair
 struct PairCountF {
@@ -102,20 +107,21 @@ struct PairKeyF {
     const int64_t i = r - j * (j - 1) / 2;
     const int s0 = q.vox_ptr[q.tile_vox[t]];
     const int si = q.vox_ptr[a] + (int)i, sj = q.vox_ptr[a] + (int)j;
-    const int pi = q.pidx[si], pj = q.pidx[sj];               // ascending inside a voxel: pi < pj
-    key[p] = (uint64_t)t * (uint64_t)q.nblocks + (uint64_t)(q.row_start[pj] + (pi - q.first[pj]));
+    const int pi = row_of_pose(q, q.pidx[si]), pj = row_of_pose(q, q.pidx[sj]);   // ascending inside a voxel: pi < pj
+    key[p] = (pi < 0 || pj < 0) ? (uint64_t)q.n_tiles * (uint64_t)q.nblocks
+                                : (uint64_t)t * (uint64_t)q.nblocks + (uint64_t)(q.row_start[pj] + (pi - q.first[pj]));
     code[p] = (uint32_t)(si - s0) | ((uint32_t)(sj - s0) << 16);
   }
 };
 
-// one item per slot: key = (tile, pose), code = slot local to the tile
+// one item per slot: key = (tile, pose), code = slot local to the tile (a slot of a constant pose: no destination)
 struct SlotKeyF {
   TableIn in; uint64_t* key = nullptr; uint32_t* code = nullptr;
   LVBA_THD void operator()(int64_t s) const {
     const TableIn& q = in;
     int64_t t = 0, hi = q.n_tiles;
     while (hi - t > 1) { const int64_t m = (t + hi) >> 1; if (q.vox_ptr[q.tile_vox[m]] <= s) t = m; else hi = m; }
-    key[s] = (uint64_t)t * (uint64_t)q.W + (uint64_t)q.pidx[s];
+    key[s] = row_of_pose(q, q.pidx[s]) < 0 ? (uint64_t)q.n_tiles * (uint64_t)q.W : (uint64_t)t * (uint64_t)q.W + (uint64_t)q.pidx[s];
     code[s] = (uint32_t)(s - q.vox_ptr[q.tile_vox[t]]);
   }
 };
@@ -258,8 +264,9 @@ GatherF gather_part(const FixedSum<Ex>& f, const double* rec, int width, int el0
   return GatherF{f.by_dst.run_ptr.p, f.by_dst.code.p, f.dst.p, rec, width, el0, n_el, out};
 }
 
-// Destinations of the records of the LiDAR build (lidar_build_kernel<true>): one item per pair run (the lower H block of its
-// pose pair), one per pose run (the diagonal H block and the gradient row of its pose).  tile_run / run_ptr / code: a Runs.
+// Destinations of the records of the LiDAR build (lidar_build_kernel<true, *>): one item per pair run (the lower H block of its
+// pose pair), one per pose run (the diagonal H block and the gradient row of its pose), addressed by row.  The runs hold only
+// pairs and slots with rows.  tile_run / run_ptr / code: a Runs.
 LVBA_THD int64_t tile_of_run(const int64_t* tile_run, int64_t n_tiles, int64_t r) {
   int64_t t = 0, hi = n_tiles;                                 // the last tile whose runs start at or before r
   while (hi - t > 1) { const int64_t m = (t + hi) >> 1; if (tile_run[m] <= r) t = m; else hi = m; }
@@ -270,7 +277,7 @@ struct PairRunDstF {
   LVBA_THD void operator()(int64_t r) const {
     const int s0 = in.vox_ptr[in.tile_vox[tile_of_run(tile_run, in.n_tiles, r)]];
     const uint32_t c = code[run_ptr[r]];
-    const int pi = in.pidx[s0 + (int)(c & 0xffff)], pj = in.pidx[s0 + (int)(c >> 16)];
+    const int pi = row_of_pose(in, in.pidx[s0 + (int)(c & 0xffff)]), pj = row_of_pose(in, in.pidx[s0 + (int)(c >> 16)]);
     dst_H[r] = in.row_start[pj] + (pi - in.first[pj]);
   }
 };
@@ -278,9 +285,9 @@ struct SlotRunDstF {
   TableIn in; const int64_t* tile_run; const int64_t* run_ptr; const uint32_t* code; int64_t* dst_H; int64_t* dst_g;
   LVBA_THD void operator()(int64_t r) const {
     const int s0 = in.vox_ptr[in.tile_vox[tile_of_run(tile_run, in.n_tiles, r)]];
-    const int pose = in.pidx[s0 + (int)code[run_ptr[r]]];
-    dst_H[r] = in.row_start[pose] + (pose - in.first[pose]);
-    dst_g[r] = pose;
+    const int row = row_of_pose(in, in.pidx[s0 + (int)code[run_ptr[r]]]);
+    dst_H[r] = in.row_start[row] + (row - in.first[row]);
+    dst_g[r] = row;
   }
 };
 

@@ -439,7 +439,8 @@ struct EnvSolver {
   const double* jobs_x = nullptr;
   // ---- batched mode (window BA): the system is block diagonal; every group is factorised by its own CTA
   int n_groups = 0;
-  std::vector<int> grp_ptr;     // [n_groups+1] row offsets
+  std::vector<int> grp_ptr;     // [n_groups+1] row offsets; an empty group (a window whose poses are all constant) has no job
+  int n_group_jobs = 0;         // the groups with rows
   DevBuf<int> first_rel;        // first[r] relative to the first row of r's group
   // window sizes P the register-window kernel is built for (P - 1 = widest column it holds): the work per pivot column
   // grows with P^2, so a system is factorised with the smallest P that fits its envelope
@@ -637,6 +638,7 @@ struct EnvSolver {
     if (path == kSolveBatch) {
       for (int g = 0; g < n_groups; ++g) {
         const int r0 = grp_ptr[g], ng = grp_ptr[g + 1] - r0;
+        if (ng == 0) continue;                                      // nothing to factorise; its status stays 0
         EnvView vg{ng, first_rel.p + r0, env.d_row_start.p + r0, env.d_last.p + r0, env.nblocks};
         fj.push_back(FactorJob{vg, L.p, dinv.p + 36 * (size_t)r0, z.p + 6 * (size_t)r0, ng, nullptr, nullptr, status.p + g});
         bj.push_back(BacksolveJob{vg, L.p, x + 6 * (size_t)r0, ng});
@@ -654,6 +656,7 @@ struct EnvSolver {
       fj.push_back(FactorJob{v, L.p, dinv.p, z.p, env.n, nullptr, nullptr, status.p});
       bj.push_back(BacksolveJob{v, L.p, x, env.n});
     }
+    if (path == kSolveBatch) n_group_jobs = (int)fj.size();
     LVBA_TRY(d_fjobs.upload(fj, s));
     LVBA_TRY(d_bjobs.upload(bj, s));
     LVBA_CUDA(cudaStreamSynchronize(s));               // local vectors
@@ -748,9 +751,9 @@ struct EnvSolver {
     }
     if (path != LVBA_SOLVE_SHARED_WINDOW) LVBA_TRY(build_jobs(env, x, s));
     if (path == kSolveBatch) {
-      LVBA_TRY(launch_factor(pid(mc), n_groups, d_fjobs.p, s, launches));
+      if (n_group_jobs > 0) LVBA_TRY(launch_factor(pid(mc), n_group_jobs, d_fjobs.p, s, launches));
       launch_apply(env.n, dinv.p, z.p, x, s);
-      launch_backsolve(n_groups, d_bjobs.p, s);
+      if (n_group_jobs > 0) launch_backsolve(n_group_jobs, d_bjobs.p, s);
       *launches += 2;
     } else if (path == LVBA_SOLVE_TWISTED) {
       // ---------------- twisted: two half factorisations on two SMs, joined at the separator

@@ -105,6 +105,22 @@ inline int voxel_map_create_impl(int32_t W, const int64_t* scan_ptr, const float
   return LVBA_OK;
 }
 
+// lvba_voxel_map_lidar_create, planned with the constant poses pose_fixed (null: none; the one-shot call plans once with its mask)
+inline int voxel_map_lidar_create_impl(lvba_voxel_map* m, const double* poses, lvba_lidar_problem** out, const uint8_t* pose_fixed) {
+  if (!m || !poses || !out) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  *out = nullptr;
+  LVBA_CUDA(cudaSetDevice(m->device));
+  auto& v = m->map;
+  if (v.W <= 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "the map has no scans");
+  if (v.n_windows > 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "windowed map: use lvba_voxel_map_lidar_lm_batch");
+  std::vector<int64_t> vox_ptr((size_t)v.V + 1);
+  std::vector<int32_t> pose_idx((size_t)v.nnz);
+  LVBA_CUDA(cudaMemcpyAsync(vox_ptr.data(), v.vox_ptr.p, vox_ptr.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, v.ex.stream));
+  if (v.nnz) LVBA_CUDA(cudaMemcpyAsync(pose_idx.data(), v.vox_pose.p, pose_idx.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, v.ex.stream));
+  LVBA_CUDA(cudaStreamSynchronize(v.ex.stream));
+  return lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, out, 0, nullptr, v.vox_cluster.p,
+                                 true, pose_fixed);
+}
 }  // namespace lvba
 
 extern "C" {
@@ -193,18 +209,7 @@ int lvba_voxel_map_lookup(lvba_voxel_map* m, int64_t n, const double* X, double*
 // tras_opt straight into path A: the map's plane voxels become a device-resident LiDAR problem.  Only the CSR index
 // arrays (12 B per cluster) visit the host, for the symbolic analysis; the 80-byte cluster records stay in HBM.
 int lvba_voxel_map_lidar_create(lvba_voxel_map* m, const double* poses, lvba_lidar_problem** out) LVBA_ABI_BEGIN {
-  if (!m || !poses || !out) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
-  *out = nullptr;
-  LVBA_CUDA(cudaSetDevice(m->device));
-  auto& v = m->map;
-  if (v.W <= 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "the map has no scans");
-  if (v.n_windows > 0) return lvba::fail(LVBA_ERR_INVALID_ARG, "windowed map: use lvba_voxel_map_lidar_lm_batch");
-  std::vector<int64_t> vox_ptr((size_t)v.V + 1);
-  std::vector<int32_t> pose_idx((size_t)v.nnz);
-  LVBA_CUDA(cudaMemcpyAsync(vox_ptr.data(), v.vox_ptr.p, vox_ptr.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, v.ex.stream));
-  if (v.nnz) LVBA_CUDA(cudaMemcpyAsync(pose_idx.data(), v.vox_pose.p, pose_idx.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, v.ex.stream));
-  LVBA_CUDA(cudaStreamSynchronize(v.ex.stream));
-  return lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, out, 0, nullptr, v.vox_cluster.p);
+  return lvba::voxel_map_lidar_create_impl(m, poses, out, nullptr);
 } LVBA_ABI_END("lvba_voxel_map_lidar_create")
 
 // cut_voxel + recut (the map) -> tras_opt + BALM2::damping_iter (this call).  min_voxels_per_pose: the caller-side skip of
@@ -224,7 +229,7 @@ int lvba_voxel_map_lidar_lm(lvba_voxel_map* m, double* poses, int32_t min_voxels
     return LVBA_OK;
   }
   lvba_lidar_problem* p = nullptr;
-  int rc = lvba_voxel_map_lidar_create(m, poses, &p);
+  int rc = lvba::voxel_map_lidar_create_impl(m, poses, &p, o.pose_fixed);
   if (rc != LVBA_OK) return rc;
   return lvba::lm_one_shot(p, o, /*solve=*/true, lvba_lidar_reset_lm, lvba_lidar_iterate, lvba_lidar_destroy,
                            [&] { return lvba_lidar_get_poses(p, poses); }, t0, summary);
@@ -249,7 +254,8 @@ int lvba_voxel_map_lidar_lm_batch(lvba_voxel_map* m, double* poses, int32_t min_
   if (v.nnz) LVBA_CUDA(cudaMemcpyAsync(pose_idx.data(), v.vox_pose.p, pose_idx.size() * sizeof(int32_t), cudaMemcpyDeviceToHost, v.ex.stream));
   LVBA_CUDA(cudaStreamSynchronize(v.ex.stream));
   lvba_lidar_problem* p = nullptr;
-  LVBA_TRY(lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, &p, v.n_windows, m->win_ptr.data(), v.vox_cluster.p));
+  LVBA_TRY(lvba::lidar_create_impl(v.W, v.V, vox_ptr.data(), pose_idx.data(), nullptr, poses, m->device, &p, v.n_windows, m->win_ptr.data(), v.vox_cluster.p,
+                                    true, o.pose_fixed));
   return lvba::lidar_batch_one_shot(p, o, min_voxels_per_pose, poses, summaries, total, t0, "lvba_voxel_map_lidar_lm_batch");
 } LVBA_ABI_END("lvba_voxel_map_lidar_lm_batch")
 

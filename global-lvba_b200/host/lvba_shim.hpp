@@ -37,13 +37,26 @@
 
 namespace lvba_b200 {
 
+// opts with the constant poses pose_fixed (null: opts as they are; else one entry per pose, nonzero = constant, which
+// overrides opts->pose_fixed); `o` holds the copy when one is needed
+inline const lvba_lidar_opts* with_pose_fixed(const lvba_lidar_opts* opts, const std::vector<uint8_t>* pose_fixed, int W,
+                                              lvba_lidar_opts& o, const char* who) {
+  if (!pose_fixed) return opts;
+  if ((int)pose_fixed->size() != W) throw std::runtime_error(std::string("lvba_b200::") + who + ": pose_fixed needs one entry per pose");
+  if (opts) o = *opts; else lvba_lidar_default_opts(&o);
+  o.pose_fixed = pose_fixed->data();
+  return &o;
+}
+
 // ---- B1: x_stats[i].R (3x3), x_stats[i].p (3) ; voxhess.plvec_voxels[a] -> const vector<PointCluster>* with
-//      (*ptr)[i].P (3x3), .v (3), .N ; voxhess.win_size
+//      (*ptr)[i].P (3x3), .v (3), .N ; voxhess.win_size.  pose_fixed (null: none) holds poses constant (lvba_lidar_opts::pose_fixed).
 template <class PoseVec, class VoxHess>
 inline int damping_iter(PoseVec& x_stats, VoxHess& voxhess, const lvba_lidar_opts* opts = nullptr,
-                        lvba_summary* summary = nullptr) {
+                        lvba_summary* summary = nullptr, const std::vector<uint8_t>* pose_fixed = nullptr) {
   const int W = voxhess.win_size;
   if ((int)x_stats.size() < W) throw std::runtime_error("lvba_b200::damping_iter: x_stats smaller than win_size");
+  lvba_lidar_opts o;
+  opts = with_pose_fixed(opts, pose_fixed, W, o, "damping_iter");
   const int64_t V = (int64_t)voxhess.plvec_voxels.size();
   std::vector<int64_t> vox_ptr(V + 1, 0);
   std::vector<int32_t> pose_idx;
@@ -179,10 +192,13 @@ class SurfMap {
 
   // tras_opt(voxhess) + BALM2::damping_iter(x_stats, voxhess) on the map's plane voxels.  min_voxels_per_pose mirrors the
   // caller's `plvec_voxels.size() < 3 * x_win.size()` skip (src/lvba_system.cpp:262-266): returns LVBA_OK with
-  // summary->termination = LVBA_TERM_SKIPPED and x_stats untouched when there are too few voxels.
-  int damping_iter(PoseVec& x_stats, int min_voxels_per_pose = 0, const lvba_lidar_opts* opts = nullptr, lvba_summary* summary = nullptr) {
+  // summary->termination = LVBA_TERM_SKIPPED and x_stats untouched when there are too few voxels.  pose_fixed: as damping_iter.
+  int damping_iter(PoseVec& x_stats, int min_voxels_per_pose = 0, const lvba_lidar_opts* opts = nullptr, lvba_summary* summary = nullptr,
+                   const std::vector<uint8_t>* pose_fixed = nullptr) {
     if (!map_) throw std::runtime_error("lvba_b200::SurfMap::damping_iter: map not built");
     if ((int)x_stats.size() < win_size_) throw std::runtime_error("lvba_b200::SurfMap::damping_iter: x_stats smaller than win_size");
+    lvba_lidar_opts o;
+    opts = with_pose_fixed(opts, pose_fixed, win_size_, o, "SurfMap::damping_iter");
     std::vector<double> poses((size_t)win_size_ * 12);
     for (int i = 0; i < win_size_; ++i) {
       for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) poses[12 * i + 3 * r + c] = x_stats[i].R(r, c);
@@ -226,12 +242,17 @@ class SurfMap {
 //      are dataset_io_->pl_fulls_ / x_buf_; windows are the consecutive `window_size` slices of the loop at :232-233.  On return
 //      x_wins[w] holds the optimised x_win of window w (the odometry poses when the window was skipped by the
 //      `plvec_voxels.size() < 3 * x_win.size()` rule, :259-263, which summaries[w].termination == LVBA_TERM_SKIPPED reports).
+//      pose_fixed (null: none): one entry per frame of the concatenated windows, nonzero = held constant (a window whose frames
+//      are all constant reports LVBA_TERM_FUNCTION_TOL with no iteration).
 template <class CloudPtrVec, class PoseVec>
 inline int run_window_stage(const CloudPtrVec& pl_fulls, const PoseVec& x_buf_full, int window_size, double root_voxel_size,
                             const float eigen_ratio_array[4], std::vector<PoseVec>& x_wins, std::vector<lvba_summary>* summaries = nullptr,
-                            lvba_summary* total = nullptr, const lvba_lidar_opts* opts = nullptr) {
+                            lvba_summary* total = nullptr, const lvba_lidar_opts* opts = nullptr,
+                            const std::vector<uint8_t>* pose_fixed = nullptr) {
   if (window_size <= 0) throw std::runtime_error("lvba_b200::run_window_stage: window_size must be positive");
   const int total_size = (int)std::min(pl_fulls.size(), x_buf_full.size());
+  lvba_lidar_opts lo;
+  opts = with_pose_fixed(opts, pose_fixed, total_size, lo, "run_window_stage");
   std::vector<int32_t> win_ptr{0};
   for (int start = 0; start < total_size; start += window_size) win_ptr.push_back(std::min(start + window_size, total_size));
   const int n_windows = (int)win_ptr.size() - 1;
@@ -291,9 +312,10 @@ struct WindowBAResult {
 template <class CloudPtrVec, class PoseVec>
 inline int run_window_ba(const CloudPtrVec& pl_fulls, const PoseVec& x_buf_full, int window_size, double root_voxel_size,
                          const float eigen_ratio_array[4], double anchor_leaf, bool use_window_ba_rel, WindowBAResult<PoseVec>& res,
-                         const lvba_lidar_opts* opts = nullptr) {
+                         const lvba_lidar_opts* opts = nullptr, const std::vector<uint8_t>* pose_fixed = nullptr) {
   std::vector<PoseVec> x_wins;
-  int rc = run_window_stage(pl_fulls, x_buf_full, window_size, root_voxel_size, eigen_ratio_array, x_wins, &res.summaries, nullptr, opts);
+  int rc = run_window_stage(pl_fulls, x_buf_full, window_size, root_voxel_size, eigen_ratio_array, x_wins, &res.summaries, nullptr, opts,
+                            pose_fixed);
   if (rc != LVBA_OK) return rc;
   const int total_size = (int)std::min(pl_fulls.size(), x_buf_full.size());
   res.anchor_poses.clear(); res.anchor_clouds.clear();

@@ -53,6 +53,22 @@ typedef struct lvba_lidar_opts {
                           * Costs device memory for one record per summed contribution (allocated when a call or
                           * lvba_lidar_reset_lm first asks for the mode) and build / solve time.  One GPU only: with an
                           * active communicator (lvba_comm_init) the call returns LVBA_ERR_UNSUPPORTED. */
+  /* Constant poses (ceres::Problem::SetParameterBlockConstant applied to damping_iter, e.g. the first scan as the gauge, or
+   * the scans of a map already optimised): NULL (the default) or W bytes, nonzero = pose held constant; for the batched
+   * calls W covers the concatenated poses.  A constant pose gets no row in the pose system (the free poses get rows in
+   * ascending pose order, see lvba_lidar_rows) and comes back bit-identical.  Every voxel still enters the cost through all
+   * of its slots, constant ones included, and the AVG_THR divisor stays V.  D = diag(H) of the free rows.  With no free
+   * pose (in a batch: no free pose in a window) there is nothing to solve: the residual is evaluated once, the summary has
+   * 0 iterations, 0 builds, cost_first = cost_last and LVBA_TERM_FUNCTION_TOL (a window that min_voxels_per_pose skips is
+   * still LVBA_TERM_SKIPPED).  Read by lvba_lidar_lm, lvba_lidar_lm_batch, lvba_voxel_map_lidar_lm and
+   * lvba_voxel_map_lidar_lm_batch, which plan their problem with it, and by lvba_lidar_reset_lm (a new handle has none):
+   * a reset whose mask differs from the handle's current one re-plans the rows, the envelope, the solver and the build's
+   * tables before it returns (the clusters stay on the device).  If that re-plan fails, the reset returns the error and
+   * the handle keeps its previous constant poses with deterministic mode off (reset again to turn it on); should restoring
+   * the previous plan fail as well, every later call on the handle but lvba_lidar_destroy and the pose copies returns
+   * LVBA_ERR_INVALID_ARG.  An all-zero mask is the same as NULL; any nonzero entry with an active communicator is
+   * LVBA_ERR_UNSUPPORTED.  The library keeps no copy of the pointer. */
+  const uint8_t* pose_fixed;
 } lvba_lidar_opts;
 
 /* ---- path B robust losses: the ceres::LossFunction of a residual block (src/lvba_system.cpp:1585-1586, :1630, :1639).
@@ -201,19 +217,24 @@ int lvba_lidar_build(lvba_lidar_problem* p, double* residual_sum);
 /* VOX_HESS::evaluate_only_residual (bavoxel.hpp:176-203) at `poses` (host, W*12) or at the
  * current device poses when poses == NULL. */
 int lvba_lidar_residual(lvba_lidar_problem* p, const double* poses, double* residual_sum);
-/* (H + u*diag(H)) dx = -g  (bavoxel.hpp:692-710); dx [W*6] to host. */
+/* (H + u*diag(H)) dx = -g  (bavoxel.hpp:692-710) over the free rows; dx [W*6] to host, zeros for constant poses. */
 int lvba_lidar_solve(lvba_lidar_problem* p, double u, double* dx);
-/* Block structure of the lower-triangular envelope that stores H: nblocks and per block (row, col). */
+/* The rows of the pose system: n_rows free poses (W without lvba_lidar_opts::pose_fixed) and pose_of_row [n_rows], the
+ * pose of every row, ascending (the identity without a mask).  Either pointer may be NULL. */
+int lvba_lidar_rows(lvba_lidar_problem* p, int32_t* n_rows, int32_t* pose_of_row);
+/* Block structure of the lower-triangular envelope that stores H over the rows: nblocks and per block (row, col). */
 int lvba_lidar_structure(lvba_lidar_problem* p, int64_t* nblocks, int32_t* brow, int32_t* bcol);
-/* Copy out g [W*6] and the envelope blocks [nblocks*36, row-major 6x6, block (r,c) = H[6r.., 6c..]]. */
+/* Copy out g [n_rows*6] and the envelope blocks [nblocks*36, row-major 6x6, block (r,c) = H[6r.., 6c..]], by rows. */
 int lvba_lidar_get_system(lvba_lidar_problem* p, double* g, double* blocks);
 /* n LM passes of damping_iter starting from the handle's state (u, v, poses carried in the
- * handle; call lvba_lidar_reset_lm to restart).  Device-resident: no problem data crosses PCIe. */
+ * handle; call lvba_lidar_reset_lm to restart).  Device-resident: no problem data crosses PCIe.  The reset also takes the
+ * handle's constant poses (lvba_lidar_opts::pose_fixed), which build, solve, iterate and get_system then follow. */
 int lvba_lidar_reset_lm(lvba_lidar_problem* p, const lvba_lidar_opts* opts);
 /* restore the poses passed to lvba_lidar_create (device-to-device; nothing crosses PCIe) */
 int lvba_lidar_reset_state(lvba_lidar_problem* p);
 int lvba_lidar_iterate(lvba_lidar_problem* p, int32_t n_iter, lvba_summary* summary);
-/* exact algorithmic byte / flop counters of SURVEY.md §8(d) for this problem instance */
+/* exact algorithmic byte / flop counters of SURVEY.md §8(d) for this problem instance (nnz: every slot; the blocks and
+ * pose pairs: those of the row system) */
 int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env,
                       int64_t* n_blocks_nonzero, int64_t* n_pairs);
 

@@ -36,6 +36,10 @@
 //                (lvba_visual_offline.hpp write_visual_problem), to re-run or inspect that solve elsewhere
 //   --fix-cameras LIST   hold these cameras of the visual stage constant besides camera 0 (lvba_visual_opts::cam_fixed); LIST is
 //                index ranges A:B (inclusive) or single indices, comma separated, e.g. 0:3,10; an index past the last image is an error
+//   --fix-scans LIST   hold these input scans constant in the LiDAR LM (lvba_lidar_opts::pose_fixed), LIST as for --fix-cameras
+//                (an index past the last scan is an error, --check included): e.g. the first scan as the gauge, or the scans of a
+//                session optimised earlier.  Without --window both global stages hold them; with --window the window stage holds
+//                the listed frames and a global stage holds an anchor when every frame of its window is listed.
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -58,7 +62,7 @@ int main(int argc, char** argv) {
   int fuse_order = LVBA_FUSE_ORDER_LIBSTDCXX;         // the library's default: what a g++ build of the reference does
   int window = 0;
   double anchor_leaf = 0.1;
-  std::string db_path, sparse_dir, lidar_opt, visual_problem, fix_cameras;
+  std::string db_path, sparse_dir, lidar_opt, visual_problem, fix_cameras, fix_scans;
   lvba_b200::offline::Config cfg;
   lvba_visual_opts visual_opts;
   lvba_visual_default_opts(&visual_opts);
@@ -90,6 +94,12 @@ int main(int argc, char** argv) {
       std::string e;
       fix_cameras = next();
       if (!lvba_b200::offline::parse_index_ranges(fix_cameras.c_str(), -1, unused, &e)) { std::fprintf(stderr, "--fix-cameras: %s\n", e.c_str()); return 64; }
+    }
+    else if (a == "--fix-scans") {
+      std::vector<uint8_t> unused;
+      std::string e;
+      fix_scans = next();
+      if (!lvba_b200::offline::parse_index_ranges(fix_scans.c_str(), -1, unused, &e)) { std::fprintf(stderr, "--fix-scans: %s\n", e.c_str()); return 64; }
     }
     else if (a == "--reproj-loss" || a == "--plane-loss") {
       const bool reproj = a == "--reproj-loss";
@@ -130,6 +140,11 @@ int main(int argc, char** argv) {
   for (size_t i = 0; i < n; ++i) { for (int k = 0; k < 9; ++k) pose_sum += (k + 1) * ds.x_buf[i].R.m[k]; for (int k = 0; k < 3; ++k) pose_sum += (k + 10) * ds.x_buf[i].p.v[k]; }
   std::printf("{\"scans\": %zu, \"poses\": %zu, \"points\": %zu, \"coordinate_sum\": %.6f, \"pose_sum\": %.9f, \"first_ts\": %.6f, \"last_ts\": %.6f}\n",
               ds.clouds.size(), ds.x_buf.size(), points, sum, pose_sum, n ? ds.x_buf[0].t : 0.0, n ? ds.x_buf[n - 1].t : 0.0);
+  std::vector<uint8_t> scan_fixed;                                          // one entry per scan: the scans of --fix-scans
+  if (!fix_scans.empty() && !lvba_b200::offline::parse_index_ranges(fix_scans.c_str(), (int)n, scan_fixed, &err)) {
+    std::fprintf(stderr, "--fix-scans: %s\n", err.c_str());
+    return 64;
+  }
   if (check && !visual) return 0;
   std::vector<Pose> frames(ds.x_buf.begin(), ds.x_buf.begin() + (long)n);              // x_buf_full
   const std::vector<Pose> frames_before = frames;                                      // x_buf_before_
@@ -145,7 +160,8 @@ int main(int argc, char** argv) {
   std::vector<lvba_b200::AnchorCloud*> anchor_clouds;
   const bool windows = lidar && window > 0;
   if (windows) {                                                             // runWindowBA (:205-316)
-    const int rc = lvba_b200::run_window_ba(frame_clouds, frames, window, voxel[0], eigen[0], anchor_leaf, window_rel, wba, &lidar_opts);
+    const int rc = lvba_b200::run_window_ba(frame_clouds, frames, window, voxel[0], eigen[0], anchor_leaf, window_rel, wba, &lidar_opts,
+                                            scan_fixed.empty() ? nullptr : &scan_fixed);
     if (rc != LVBA_OK) { std::fprintf(stderr, "window BA failed (%d): %s\n", rc, lvba_last_error()); return rc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
     size_t pts = 0;
     for (auto& c : wba.anchor_clouds) { anchor_clouds.push_back(&c); pts += c.points.size(); }
@@ -153,6 +169,12 @@ int main(int argc, char** argv) {
                 wba.win_total, wba.win_skipped, wba.anchor_poses.size(), pts);
   }
   std::vector<Pose>& poses = windows ? wba.anchor_poses : frames;            // anchor_poses / anchor_clouds of runLidarBA (:329-334)
+  std::vector<uint8_t> pose_fixed = scan_fixed;                              // the global stages' constant poses
+  if (windows && !scan_fixed.empty()) {                                      // an anchor is constant when all frames of its window are
+    pose_fixed.assign(wba.anchor_poses.size(), 1);
+    for (size_t i = 0; i < n; ++i)
+      if (wba.anchor_index_per_frame[i] >= 0 && !scan_fixed[i]) pose_fixed[(size_t)wba.anchor_index_per_frame[i]] = 0;
+  }
   for (int idx = stage1 ? 0 : 1; lidar && idx < 2 && !poses.empty(); ++idx) { // the two passes (:358-389)
     lvba_voxel_summary vs{};
     lvba_summary s{};
@@ -160,7 +182,7 @@ int main(int argc, char** argv) {
     lvba_b200::SurfMap<std::vector<Pose>> surf;
     rc = windows ? surf.build(anchor_clouds, poses, voxel[idx], eigen[idx], &vs) : surf.build(frame_clouds, poses, voxel[idx], eigen[idx], &vs);
     if (rc != LVBA_OK) { std::fprintf(stderr, "stage %d voxel map failed (%d): %s\n", idx + 1, rc, lvba_last_error()); return rc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
-    rc = surf.damping_iter(poses, 0, &lidar_opts, &s);
+    rc = surf.damping_iter(poses, 0, &lidar_opts, &s, pose_fixed.empty() ? nullptr : &pose_fixed);
     if (rc != LVBA_OK) { std::fprintf(stderr, "stage %d LM failed (%d): %s\n", idx + 1, rc, lvba_last_error()); return 1; }
     std::printf("{\"stage\": %d, \"voxels\": %lld, \"clusters\": %lld, \"map_ms\": %.3f, \"iterations\": %d, \"accepted\": %d, \"cost_first\": %.9e, \"cost_last\": %.9e, \"lm_ms\": %.3f}\n",
                 idx + 1, (long long)vs.n_voxels, (long long)vs.nnz, vs.ms_total, s.iterations, s.accepted, s.cost_first, s.cost_last, s.ms_total);
