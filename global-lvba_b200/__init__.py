@@ -31,6 +31,7 @@ EXPORTS = [
     "lvba_lidar_get_poses", "lvba_lidar_build", "lvba_lidar_residual", "lvba_lidar_solve",
     "lvba_lidar_structure", "lvba_lidar_get_system", "lvba_lidar_reset_lm", "lvba_lidar_reset_state", "lvba_lidar_iterate",
     "lvba_lidar_counts", "lvba_lidar_rows",
+    "lvba_lidar_voxel_residuals", "lvba_lidar_remove_voxels", "lvba_lidar_remove_outliers",
     "lvba_visual_lm", "lvba_visual_create", "lvba_visual_destroy", "lvba_visual_set_state",
     "lvba_visual_get_state", "lvba_visual_cost", "lvba_visual_step", "lvba_visual_structure",
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
@@ -326,6 +327,33 @@ class LidarProblem:
         a, b, c, d = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int64()
         _chk(self._lib.lvba_lidar_counts(self._h, C.byref(a), C.byref(b), C.byref(c) if nonzero else None, C.byref(d)))
         return dict(nnz=a.value, n_blocks_env=b.value, n_blocks_nonzero=c.value if nonzero else None, n_pairs=d.value)
+
+    def voxel_residuals(self, poses=None):
+        """lambda0 [V] of every voxel (lvba_lidar_voxel_residuals, VOX_HESS::evaluate_residual) at `poses`, or at the
+        handle's poses when None; in the handle's voxel order (the caller's, minus the voxels removed so far)."""
+        out = np.empty(self.V)
+        ps = None if poses is None else _f64(poses)
+        _chk(self._lib.lvba_lidar_voxel_residuals(self._h, None if ps is None else _p(ps, C.c_double), _p(out, C.c_double)))
+        return out
+
+    def remove_voxels(self, mask):
+        """Erase the voxels where mask [V] is true (lvba_lidar_remove_voxels); returns the number of voxels left."""
+        m = np.ascontiguousarray(np.asarray(mask, bool), np.uint8)
+        if m.shape != (self.V,):
+            raise ValueError(f"mask has shape {m.shape}, expected ({self.V},)")
+        n = C.c_int64()
+        _chk(self._lib.lvba_lidar_remove_voxels(self._h, _p(m, C.c_uint8), C.byref(n)))
+        self.V = n.value
+        return self.V
+
+    def remove_outliers(self, ratio):
+        """BALM2::remove_outlier at the handle's poses (lvba_lidar_remove_outliers); returns the boolean mask [V before the
+        call] of the removed voxels."""
+        out = np.zeros(self.V, np.uint8)
+        n = C.c_int64()
+        _chk(self._lib.lvba_lidar_remove_outliers(self._h, C.c_double(ratio), _p(out, C.c_uint8), C.byref(n)))
+        self.V -= n.value
+        return out.astype(bool)
 
 
 SOLVE_AUTO, SOLVE_ONE_CTA, SOLVE_TWISTED, SOLVE_CHUNKED, SOLVE_SHARED_WINDOW, SOLVE_ANY_WIDTH = range(6)

@@ -122,12 +122,15 @@ LVBA_DEV void voxel_cov(const double* stage, int s_lo, int s_hi, double cov[6], 
 
 // ------------------------------------------------------------------------------------------------
 // residual-only pass: sum_v lambda0 (per-batch partial written to batch_res[blockIdx.x]).
+// kPerVoxel = true (lvba_lidar_voxel_residuals): every voxel's lambda0 is stored instead, at out[vox_id[v]] for local voxel v
+// (out[v] when vox_id is null: the local order is the handle's), and nothing is summed.
 // The four warps of a batch CTA work on their own quarter of the batch's voxels — whose slots are contiguous — without a
 // block barrier in between: lane = slot (load, transform, stage), then lane = voxel (merge, smallest eigenvalue).  With one barrier
 // between "all slots" and "all voxels" three warps of four would wait for the one that holds the ~18 voxels; this way a warp
 // only ever waits for its own loads.
+template <bool kPerVoxel>
 __global__ void __launch_bounds__(kSlots)
-lidar_residual_kernel(LidarView lv, const double* __restrict__ poses, double* __restrict__ batch_res) {
+lidar_residual_kernel(LidarView lv, const double* __restrict__ poses, double* __restrict__ batch_res, const int* __restrict__ vox_id) {
   constexpr int kS = 11;                      // 10 doubles per slot + 1 pad (odd stride)
   constexpr int kWarps = kSlots / 32;
   __shared__ double stage[kSlots * kS];
@@ -157,9 +160,12 @@ lidar_residual_kernel(LidarView lv, const double* __restrict__ poses, double* __
       for (int q = 0; q < 10; ++q) acc[q] += stage[sl * kS + q];
     const double inv = 1.0 / acc[9];
     const double m0 = acc[6] * inv, m1 = acc[7] * inv, m2 = acc[8] * inv;
-    lam0 += sym3_smallest_eigenvalue(acc[0] * inv - m0 * m0, acc[1] * inv - m0 * m1, acc[2] * inv - m0 * m2,
-                                     acc[3] * inv - m1 * m1, acc[4] * inv - m1 * m2, acc[5] * inv - m2 * m2);
+    const double lam = sym3_smallest_eigenvalue(acc[0] * inv - m0 * m0, acc[1] * inv - m0 * m1, acc[2] * inv - m0 * m2,
+                                                acc[3] * inv - m1 * m1, acc[4] * inv - m1 * m2, acc[5] * inv - m2 * m2);
+    if constexpr (kPerVoxel) batch_res[vox_id ? vox_id[v] : v] = lam;
+    else lam0 += lam;
   }
+  if constexpr (kPerVoxel) return;
   lam0 = warp_sum(lam0);
   if (lane == 0) red[warp] = lam0;
   __syncthreads();

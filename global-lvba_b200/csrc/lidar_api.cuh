@@ -8,6 +8,7 @@
 #include "balm_rule.h"
 #include "exec.cuh"
 #include "lidar.cuh"
+#include "lidar_outliers.h"
 #include "lidar_plan.h"
 
 namespace lvba {
@@ -141,6 +142,13 @@ struct lvba_lidar_problem {
   std::vector<int> grp_row_ptr;                    // batched window BA: [G+1] row offsets of the windows
   lvba::DevBuf<int> d_grp_row_ptr, d_row_grp;      // the same on the device, and the window of every row
   bool unusable = false;                           // a re-plan failed and so did restoring the previous one (lidar_replan)
+  // ---- voxel outlier removal (lidar_outliers.h; one GPU, a handle with its host structure): where every voxel's records are,
+  // and on the device, uploaded at the first per-voxel residual of a plan, the handle voxel of every local voxel (none when the
+  // layout is the identity) and of every big voxel
+  bool have_home = false, vox_id_ready = false;
+  lvba::outliers::VoxelHome home;
+  lvba::DevBuf<int> d_vox_id, d_big_id;
+  lvba::DevBuf<double> d_vox_res;                  // [V_total] lambda_0 of every voxel, handle order
   lvba::big::View big_view() const {
     return lvba::big::View{(int64_t)n_big, big_vox_ptr.p, big_pose.p, big_cl.p, big_pair_ptr.p, env.d_first.p, env.d_row_start.p,
                            d_row_of.p, (int64_t)env.nblocks, W};
@@ -272,6 +280,9 @@ inline int lidar_plan_tables(lvba_lidar_problem* P) {
     LVBA_TRY(P->d_row_grp.upload(row_grp, s, &P->h2d));
     LVBA_CUDA(cudaStreamSynchronize(s));                       // row_grp is uploaded
   }
+  if (P->n_tiles <= 0) {                                       // no tiles (a removal left only big voxels): no runs from a previous plan
+    for (tiles::Runs<CudaExec>* r : {&P->prun, &P->drun}) { r->code.release(); r->run_ptr.release(); r->tile_run.release(); r->n_runs = 0; }
+  }
   {                                                            // destination table of the build, on the device from the local CSR
     CudaExec ex;
     ex.stream = s;
@@ -368,6 +379,10 @@ inline int lidar_create_impl(int32_t W, int64_t V, const int64_t* vox_ptr, const
     case kLayoutBigInBatch:
       return fail(LVBA_ERR_UNSUPPORTED, "batched window BA: voxel %lld is seen from %lld poses (more than %d)", (long long)L.err_vox,
                   (long long)(vox_ptr[L.err_vox + 1] - vox_ptr[L.err_vox]), kSlots);
+  }
+  if (keep_structure && !sharded && n_groups == 0) {
+    outliers::voxel_home(V, vox_ptr, L, P->home);
+    P->have_home = true;
   }
   const int64_t Vl = (int64_t)L.slot0.size();
   const long long nnz = L.nnz;
@@ -603,7 +618,7 @@ inline int lidar_build_dev(lvba_lidar_problem* P, const double* d_poses, int slo
 inline int lidar_residual_dev(lvba_lidar_problem* P, const double* d_poses, int slot) {
   cudaStream_t s = P->stream;
   if (P->n_batches > 0) {
-    lidar_residual_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), d_poses, P->batch_res.p);
+    lidar_residual_kernel<false><<<P->n_batches, kSlots, 0, s>>>(P->view(), d_poses, P->batch_res.p, nullptr);
     ++P->launches;
   }
   if (P->n_big > 0) LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/true, P->n_batches));
@@ -702,6 +717,151 @@ inline int lidar_iterate_impl(lvba_lidar_problem* P, int n_iter, lvba_summary* s
   return LVBA_OK;
 }
 
+// ---------------------------------------------------------------- voxel outlier removal (lidar_outliers.h)
+// the calls that read or change the handle's voxel set: one GPU, the handle's host structure and the voxel homes
+inline int lidar_check_voxel_set(const lvba_lidar_problem* P) {
+  LVBA_TRY(lidar_check_usable(P));
+  if (comm().active()) return fail(LVBA_ERR_UNSUPPORTED, "per-voxel residuals and voxel removal run on one GPU: not with an active communicator");
+  if (!P->have_structure || !P->have_home)
+    return fail(LVBA_ERR_UNSUPPORTED, "this problem was created without its host-side structure copy: its voxels cannot be listed or removed");
+  return LVBA_OK;
+}
+
+// lambda_0 of every voxel at `d_poses` into d_vox_res, handle order: the residual pass with kPerVoxel for the batches, and the
+// big voxels' lambda_0 that lidar_big_passes leaves after them in batch_res scattered to their handle positions
+inline int lidar_voxel_residuals_dev(lvba_lidar_problem* P, const double* d_poses) {
+  cudaStream_t s = P->stream;
+  if (!P->vox_id_ready) {
+    if (!P->home.local_vox.empty()) LVBA_TRY(P->d_vox_id.upload(P->home.local_vox, s, &P->h2d)); else P->d_vox_id.release();
+    if (!P->home.big_vox.empty()) LVBA_TRY(P->d_big_id.upload(P->home.big_vox, s, &P->h2d)); else P->d_big_id.release();
+    P->vox_id_ready = true;
+  }
+  if (P->d_vox_res.n < (size_t)P->V_total) LVBA_TRY(P->d_vox_res.alloc((size_t)P->V_total));
+  if (P->n_batches > 0) {
+    lidar_residual_kernel<true><<<P->n_batches, kSlots, 0, s>>>(P->view(), d_poses, P->d_vox_res.p, P->d_vox_id.p);
+    ++P->launches;
+  }
+  if (P->n_big > 0) {
+    LVBA_TRY(lidar_big_passes(P, d_poses, /*residual_only=*/true, P->n_batches));
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(ex.for_each(P->n_big, outliers::ScatterF{P->batch_res.p + P->n_batches, P->d_big_id.p, P->d_vox_res.p}));
+    P->launches += ex.launches;
+  }
+  LVBA_CUDA(cudaGetLastError());
+  return LVBA_OK;
+}
+
+// The handle's plan after removing the voxels with remove[a] != 0 (host, [V_total], at least one voxel kept): the same plan as
+// lvba_lidar_create on the kept voxels' CSR and records with the handle's constant poses.  The records move device to device:
+// a gather fills new SoA and big-voxel buffers, built beside the old ones, from where each kept voxel lives (P->home); only
+// index arrays cross PCIe.  Then the rows, envelope, solver and tables of the kept CSR (as lidar_replan).  On failure the old
+// buffers and plan come back (or else the handle is marked unusable).  Poses stay; the LM state is reset as lvba_lidar_reset_lm
+// with the handle's opts would, and deterministic mode's records are set up again.
+inline int lidar_remove_impl(lvba_lidar_problem* P, const uint8_t* remove) {
+  cudaStream_t s = P->stream;
+  LVBA_CUDA(cudaStreamSynchronize(s));                         // nothing in flight reads the buffers replaced below
+  outliers::KeptPlan K;
+  static_assert(sizeof(long long) == sizeof(int64_t), "the host copy of vox_ptr is read as it is");
+  if (outliers::plan_kept(P->W, P->V_total, reinterpret_cast<const int64_t*>(P->h_vox_ptr_all.data()), P->h_pose_idx_all.data(), P->home,
+                          remove, K) != kLayoutOk)
+    return fail(LVBA_ERR_INVALID_ARG, "the kept voxels have no single-GPU layout");
+  const LidarLayout& L = K.L;
+  // ---- the new records beside the old ones
+  struct Set {
+    long long V_total = 0, V_local = 0, nnz_local = 0, n_pairs = 0, n_big = 0, n_big_slots = 0, n_big_pairs = 0;
+    int n_batches = 0, n_tiles = 0;
+    DevBuf<double2> cl;
+    DevBuf<int> pidx, vox_ptr, batch_vox, tile_vox;
+    DevBuf<int64_t> big_vox_ptr, big_pair_ptr;
+    DevBuf<int32_t> big_pose;
+    DevBuf<double> big_cl, big_params, big_feat, batch_res;
+  } N;
+  N.V_total = K.V; N.V_local = (long long)L.slot0.size(); N.nnz_local = L.nnz; N.n_pairs = L.n_pairs;
+  N.n_batches = (int)L.batch_vox.size() - 1; N.n_tiles = (int)L.tile_vox.size() - 1;
+  N.n_big = (long long)L.big_vox.size(); N.n_big_slots = (long long)L.big_src.size(); N.n_big_pairs = L.big_pair_ptr.back();
+  {
+    CudaExec ex;
+    ex.stream = s;
+    const long long nnz_pad = ((N.nnz_local + 31) / 32) * 32 + 32;  // as lidar_create_impl
+    LVBA_TRY(N.cl.alloc((size_t)5 * nnz_pad));
+    LVBA_TRY(N.cl.zero(s));
+    LVBA_TRY(N.vox_ptr.upload(L.l_vox_ptr, s, &P->h2d));
+    LVBA_TRY(N.pidx.alloc((size_t)N.nnz_local));
+    DevBuf<int> d_src0, d_bsrc;
+    if (N.nnz_local > 0) {
+      LVBA_TRY(d_src0.upload(K.src0, s, &P->h2d));
+      LVBA_TRY(ex.for_each(N.nnz_local, outliers::GatherSoaF{(int32_t)N.V_local, N.vox_ptr.p, d_src0.p, reinterpret_cast<const double*>(P->cl.p),
+                                                             (int64_t)(P->cl.n / 5), P->pidx.p, reinterpret_cast<double*>(N.cl.p), nnz_pad, N.pidx.p}));
+    }
+    if (N.n_big > 0) {
+      LVBA_TRY(d_bsrc.upload(K.big_src, s, &P->h2d));
+      LVBA_TRY(N.big_vox_ptr.upload(L.big_vox_ptr, s, &P->h2d));
+      LVBA_TRY(N.big_pair_ptr.upload(L.big_pair_ptr, s, &P->h2d));
+      LVBA_TRY(N.big_pose.upload(L.big_pose, s, &P->h2d));
+      LVBA_TRY(N.big_cl.alloc((size_t)N.n_big_slots * 10));
+      LVBA_TRY(N.big_params.alloc((size_t)N.n_big * big::kParams));
+      LVBA_TRY(N.big_feat.alloc((size_t)N.n_big_slots * big::kFeat));
+      LVBA_TRY(ex.for_each(N.n_big_slots, outliers::GatherAosF{d_bsrc.p, P->big_cl.p, N.big_cl.p}));
+    }
+    LVBA_TRY(N.batch_vox.upload(L.batch_vox, s, &P->h2d));
+    LVBA_TRY(N.tile_vox.upload(L.tile_vox, s, &P->h2d));
+    LVBA_TRY(N.batch_res.alloc((size_t)std::max<long long>(std::max(N.n_batches, N.n_tiles) + N.n_big, 1)));
+    LVBA_CUDA(cudaStreamSynchronize(s));                       // the gathers are done; d_src0 and d_bsrc are freed on scope exit
+    P->launches += ex.launches;
+  }
+  // ---- swap them in (swapping again restores the old set)
+  auto swap_set = [&](Set& o) {
+    std::swap(P->V_total, o.V_total); std::swap(P->V_local, o.V_local); std::swap(P->nnz_local, o.nnz_local); std::swap(P->n_pairs, o.n_pairs);
+    std::swap(P->n_big, o.n_big); std::swap(P->n_big_slots, o.n_big_slots); std::swap(P->n_big_pairs, o.n_big_pairs);
+    std::swap(P->n_batches, o.n_batches); std::swap(P->n_tiles, o.n_tiles);
+    P->cl.swap(o.cl); P->pidx.swap(o.pidx); P->vox_ptr.swap(o.vox_ptr); P->batch_vox.swap(o.batch_vox); P->tile_vox.swap(o.tile_vox);
+    P->big_vox_ptr.swap(o.big_vox_ptr); P->big_pair_ptr.swap(o.big_pair_ptr); P->big_pose.swap(o.big_pose);
+    P->big_cl.swap(o.big_cl); P->big_params.swap(o.big_params); P->big_feat.swap(o.big_feat); P->batch_res.swap(o.batch_res);
+  };
+  tiles::fixed_sum_release(P->det_H); tiles::fixed_sum_release(P->det_g);     // they follow the table: set up again below
+  P->det_ready = false;
+  swap_set(N);
+  // the new plan, with deterministic mode's records when the handle is in that mode: a failure anywhere here restores the old one
+  auto plan_with = [&](int64_t V, const int64_t* vp, const int32_t* pi, bool det) -> int {
+    LVBA_TRY(lidar_plan_rows(P, P->pose_fixed, V, vp, pi));
+    LVBA_TRY(lidar_plan_tables(P));
+    if (det) LVBA_TRY(lidar_det_setup(P));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    return LVBA_OK;
+  };
+  int rc;
+  try { rc = plan_with(K.V, K.vox_ptr.data(), K.pose_idx.data(), P->det); } catch (const std::bad_alloc&) { rc = fail(LVBA_ERR_NOMEM, "host allocation failed"); }
+  if (rc != LVBA_OK) {
+    const std::string why = last_error_ref();
+    cudaStreamSynchronize(s);
+    cudaGetLastError();
+    tiles::fixed_sum_release(P->det_H); tiles::fixed_sum_release(P->det_g);
+    P->det_ready = false;
+    swap_set(N);
+    int rc_back;
+    try { rc_back = plan_with(P->V_total, reinterpret_cast<const int64_t*>(P->h_vox_ptr_all.data()), P->h_pose_idx_all.data(), false); }
+    catch (const std::bad_alloc&) { rc_back = LVBA_ERR_NOMEM; }
+    P->det = false;
+    P->solver.set_deterministic(false);
+    if (rc_back != LVBA_OK) {
+      P->unusable = true;
+      return fail(rc, "re-plan after the voxel removal failed (%s), and so did restoring the previous plan: destroy the handle", why.c_str());
+    }
+    return fail(rc, "re-plan after the voxel removal failed (%s); the handle keeps its voxels, deterministic mode is off", why.c_str());
+  }
+  P->h_vox_ptr_all.assign(K.vox_ptr.begin(), K.vox_ptr.end());
+  P->h_pose_idx_all.swap(K.pose_idx);
+  P->home = std::move(K.home);
+  P->vox_id_ready = false;
+  // the LM state of lvba_lidar_reset_lm with the handle's opts
+  P->lm.reset(P->opts);
+  P->is_calc_hess = true;
+  P->builds = 0;
+  P->solver.set_deterministic(P->det);
+  return LVBA_OK;
+}
+
 // ---------------------------------------------------------------- batched window BA
 // damping_iter (bavoxel.hpp:662-767) for every window at once: the windows share the kernels (one block-diagonal
 // system, one CTA per window in the factorisation) but keep their own u, v, accept/reject decision and stop test,
@@ -730,7 +890,7 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
   if (any_constant) {                                          // windows whose poses are all constant: their residual once
     P->timers.begin(PH_RESID);
     if (P->n_batches > 0) {
-      lidar_residual_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->poses.p, P->batch_res.p);
+      lidar_residual_kernel<false><<<P->n_batches, kSlots, 0, s>>>(P->view(), P->poses.p, P->batch_res.p, nullptr);
       ++P->launches;
     }
     lidar_group_sum_kernel<<<G, 128, 0, s>>>(P->batch_res.p, P->d_grp_batch.p, P->d_grp_scal.p, 3);
@@ -774,7 +934,7 @@ inline int lidar_batch_lm_impl(lvba_lidar_problem* P, int min_voxels_per_pose, l
     P->timers.begin(PH_RESID);
     lidar_retract(P);
     if (P->n_batches > 0) {
-      lidar_residual_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), P->trial.p, P->batch_res.p);
+      lidar_residual_kernel<false><<<P->n_batches, kSlots, 0, s>>>(P->view(), P->trial.p, P->batch_res.p, nullptr);
       ++P->launches;
     }
     lidar_group_sum_kernel<<<G, 128, 0, s>>>(P->batch_res.p, P->d_grp_batch.p, P->d_grp_scal.p, 3);
@@ -1012,6 +1172,69 @@ int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env
   if (want_nz) *n_blocks_nonzero = (int64_t)seen.size();
   return LVBA_OK;
 } LVBA_ABI_END("lvba_lidar_counts")
+
+int lvba_lidar_voxel_residuals(lvba_lidar_problem* p, const double* poses, double* lambda0) LVBA_ABI_BEGIN {
+  if (!p || !lambda0) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_voxel_set(p));
+  LVBA_CUDA(cudaSetDevice(p->device));
+  const double* dp = p->poses.p;
+  if (poses) {
+    LVBA_TRY(p->trial.upload(poses, (size_t)p->W * 12, p->stream, &p->h2d));
+    dp = p->trial.p;
+  }
+  LVBA_TRY(lvba::lidar_voxel_residuals_dev(p, dp));
+  LVBA_CUDA(cudaMemcpyAsync(lambda0, p->d_vox_res.p, (size_t)p->V_total * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  LVBA_CUDA(cudaStreamSynchronize(p->stream));
+  p->d2h += p->V_total * 8;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_lidar_voxel_residuals")
+
+int lvba_lidar_remove_voxels(lvba_lidar_problem* p, const uint8_t* remove, int64_t* n_left) LVBA_ABI_BEGIN {
+  if (!p || !remove) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_voxel_set(p));
+  const int64_t V = p->V_total;
+  const int64_t n_rm = std::count_if(remove, remove + V, [](uint8_t b) { return b != 0; });
+  if (n_rm == V) return lvba::fail(LVBA_ERR_INVALID_ARG, "the removal would leave no voxel");
+  LVBA_CUDA(cudaSetDevice(p->device));
+  LVBA_TRY(lvba::lidar_remove_impl(p, remove));
+  if (n_left) *n_left = p->V_total;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_lidar_remove_voxels")
+
+int lvba_lidar_remove_outliers(lvba_lidar_problem* p, double ratio, uint8_t* removed, int64_t* n_removed) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::lidar_check_voxel_set(p));
+  const int64_t V = p->V_total;
+  int64_t k_thr = 0, reject_num = 0;
+  if (!lvba::outliers::rule_params(ratio, V, &k_thr, &reject_num))
+    return lvba::fail(LVBA_ERR_INVALID_ARG, "ratio=%g: it must be finite, in [0, 1), with floor((1 - ratio) * %lld) >= 1", ratio, (long long)V);
+  LVBA_CUDA(cudaSetDevice(p->device));
+  LVBA_TRY(lvba::lidar_voxel_residuals_dev(p, p->poses.p));
+  std::vector<uint8_t> mask((size_t)V);
+  {
+    lvba::CudaExec ex;
+    ex.stream = p->stream;
+    lvba::DevBuf<uint8_t> d_mask;
+    LVBA_TRY(d_mask.alloc((size_t)V));
+    lvba::outliers::RuleOut r;
+    LVBA_TRY(lvba::outliers::remove_rule(ex, p->d_vox_res.p, V, ratio, d_mask.p, r));
+    p->launches += ex.launches;
+    if (r.non_finite) return lvba::fail(LVBA_ERR_INVALID_ARG, "a voxel's lambda_0 is not finite at the current poses: no outlier threshold");
+    LVBA_TRY(ex.fetch(mask.data(), d_mask.p, (size_t)V));
+    p->d2h += V + 24;
+  }
+  const int64_t n_rm = std::count_if(mask.begin(), mask.end(), [](uint8_t b) { return b != 0; });
+  if (n_rm == V) return lvba::fail(LVBA_ERR_INVALID_ARG, "ratio=%g would remove every voxel (all lambda_0 at the threshold)", ratio);
+  if (n_rm > 0) LVBA_TRY(lvba::lidar_remove_impl(p, mask.data()));
+  else {                                                      // nothing to erase: the plan stays, the LM state is reset all the same
+    p->lm.reset(p->opts);
+    p->is_calc_hess = true;
+    p->builds = 0;
+  }
+  if (removed) std::copy(mask.begin(), mask.end(), removed);
+  if (n_removed) *n_removed = n_rm;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_lidar_remove_outliers")
 
 int lvba_lidar_lm(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx, const double* clusters,
                   double* poses, const lvba_lidar_opts* opts, lvba_summary* summary) LVBA_ABI_BEGIN {

@@ -5,6 +5,8 @@
 // src/lvba_system.cpp of the reference and inside tests/shim/test_shim.cpp with plain mock structs.
 //
 //   lvba_b200::damping_iter(x_stats, voxhess)        replaces BALM2::damping_iter   include/BALM/bavoxel.hpp:662-767
+//   lvba_b200::evaluate_residual(x_stats, voxhess)   VOX_HESS::evaluate_residual (commented out in the reference, :205-234)
+//   lvba_b200::remove_outlier(x_stats, voxhess, r)   BALM2::remove_outlier (commented out in the reference, :650-660)
 //   lvba_b200::solve_visual(...)                     replaces the Ceres block       src/lvba_system.cpp:1571-1656
 //   lvba_b200::WindowBatch                           collects the windows of runWindowBA (src/lvba_system.cpp:232-302) and
 //                                                    solves them in one lvba_lidar_lm_batch call
@@ -49,40 +51,91 @@ inline const lvba_lidar_opts* with_pose_fixed(const lvba_lidar_opts* opts, const
 }
 
 // ---- B1: x_stats[i].R (3x3), x_stats[i].p (3) ; voxhess.plvec_voxels[a] -> const vector<PointCluster>* with
-//      (*ptr)[i].P (3x3), .v (3), .N ; voxhess.win_size.  pose_fixed (null: none) holds poses constant (lvba_lidar_opts::pose_fixed).
-template <class PoseVec, class VoxHess>
-inline int damping_iter(PoseVec& x_stats, VoxHess& voxhess, const lvba_lidar_opts* opts = nullptr,
-                        lvba_summary* summary = nullptr, const std::vector<uint8_t>* pose_fixed = nullptr) {
-  const int W = voxhess.win_size;
-  if ((int)x_stats.size() < W) throw std::runtime_error("lvba_b200::damping_iter: x_stats smaller than win_size");
-  lvba_lidar_opts o;
-  opts = with_pose_fixed(opts, pose_fixed, W, o, "damping_iter");
-  const int64_t V = (int64_t)voxhess.plvec_voxels.size();
-  std::vector<int64_t> vox_ptr(V + 1, 0);
+//      (*ptr)[i].P (3x3), .v (3), .N ; voxhess.win_size.  The problem in the CSR of lvba_lidar_lm: the slots with N != 0
+//      (bavoxel.hpp:91, :113) of every voxel in plvec_voxels order, and the first win_size poses.
+struct LidarCsr {
+  int W = 0;
+  std::vector<int64_t> vox_ptr;
   std::vector<int32_t> pose_idx;
-  std::vector<double> clusters;
-  for (int64_t a = 0; a < V; ++a) {                    // pack slots with N != 0 (bavoxel.hpp:91, :113)
+  std::vector<double> clusters, poses;
+  int64_t V() const { return (int64_t)vox_ptr.size() - 1; }
+};
+
+template <class PoseVec, class VoxHess>
+inline LidarCsr pack_lidar(const PoseVec& x_stats, const VoxHess& voxhess, const char* who) {
+  LidarCsr c;
+  const int W = c.W = voxhess.win_size;
+  if ((int)x_stats.size() < W) throw std::runtime_error(std::string("lvba_b200::") + who + ": x_stats smaller than win_size");
+  const int64_t V = (int64_t)voxhess.plvec_voxels.size();
+  c.vox_ptr.assign((size_t)V + 1, 0);
+  for (int64_t a = 0; a < V; ++a) {
     const auto& sig = *voxhess.plvec_voxels[a];
     for (int i = 0; i < W; ++i) {
       if (sig[i].N == 0) continue;
-      pose_idx.push_back(i);
+      c.pose_idx.push_back(i);
       const auto& P = sig[i].P; const auto& v = sig[i].v;
       const double rec[10] = {P(0, 0), P(0, 1), P(0, 2), P(1, 1), P(1, 2), P(2, 2), v(0), v(1), v(2), (double)sig[i].N};
-      clusters.insert(clusters.end(), rec, rec + 10);
+      c.clusters.insert(c.clusters.end(), rec, rec + 10);
     }
-    vox_ptr[a + 1] = (int64_t)pose_idx.size();
+    c.vox_ptr[a + 1] = (int64_t)c.pose_idx.size();
   }
-  std::vector<double> poses((size_t)W * 12);
+  c.poses.resize((size_t)W * 12);
   for (int i = 0; i < W; ++i) {
-    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) poses[12 * i + 3 * r + c] = x_stats[i].R(r, c);
-    for (int r = 0; r < 3; ++r) poses[12 * i + 9 + r] = x_stats[i].p(r);
+    for (int r = 0; r < 3; ++r) for (int k = 0; k < 3; ++k) c.poses[12 * i + 3 * r + k] = x_stats[i].R(r, k);
+    for (int r = 0; r < 3; ++r) c.poses[12 * i + 9 + r] = x_stats[i].p(r);
   }
-  const int rc = lvba_lidar_lm(W, V, vox_ptr.data(), pose_idx.data(), clusters.data(), poses.data(), opts, summary);
+  return c;
+}
+
+// pose_fixed (null: none) holds poses constant (lvba_lidar_opts::pose_fixed).
+template <class PoseVec, class VoxHess>
+inline int damping_iter(PoseVec& x_stats, VoxHess& voxhess, const lvba_lidar_opts* opts = nullptr,
+                        lvba_summary* summary = nullptr, const std::vector<uint8_t>* pose_fixed = nullptr) {
+  LidarCsr c = pack_lidar(x_stats, voxhess, "damping_iter");
+  const int W = c.W;
+  lvba_lidar_opts o;
+  opts = with_pose_fixed(opts, pose_fixed, W, o, "damping_iter");
+  const int rc = lvba_lidar_lm(W, c.V(), c.vox_ptr.data(), c.pose_idx.data(), c.clusters.data(), c.poses.data(), opts, summary);
   if (rc != LVBA_OK) return rc;                        // reference: silent on failure, state untouched
   for (int i = 0; i < W; ++i) {                        // x_stats = x_stats_temp (bavoxel.hpp:746)
-    for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) x_stats[i].R(r, c) = poses[12 * i + 3 * r + c];
-    for (int r = 0; r < 3; ++r) x_stats[i].p(r) = poses[12 * i + 9 + r];
+    for (int r = 0; r < 3; ++r) for (int k = 0; k < 3; ++k) x_stats[i].R(r, k) = c.poses[12 * i + 3 * r + k];
+    for (int r = 0; r < 3; ++r) x_stats[i].p(r) = c.poses[12 * i + 9 + r];
   }
+  return LVBA_OK;
+}
+
+// VOX_HESS::evaluate_residual (bavoxel.hpp:205-234, commented out in the reference): lambda_0 of every voxel of plvec_voxels at
+// x_stats, through lvba_lidar_voxel_residuals on a handle of its own.  Throws std::runtime_error with the library's message.
+template <class PoseVec, class VoxHess>
+inline std::vector<double> evaluate_residual(const PoseVec& x_stats, const VoxHess& voxhess, int32_t device = -1) {
+  LidarCsr c = pack_lidar(x_stats, voxhess, "evaluate_residual");
+  std::vector<double> lam((size_t)c.V());
+  lvba_lidar_problem* p = nullptr;
+  int rc = lvba_lidar_create(c.W, c.V(), c.vox_ptr.data(), c.pose_idx.data(), c.clusters.data(), c.poses.data(), device, &p);
+  if (rc == LVBA_OK) rc = lvba_lidar_voxel_residuals(p, nullptr, lam.data());
+  const std::string why = rc == LVBA_OK ? "" : lvba_last_error();
+  lvba_lidar_destroy(p);
+  if (rc != LVBA_OK) throw std::runtime_error("lvba_b200::evaluate_residual: " + why);
+  return lam;
+}
+
+// BALM2::remove_outlier(x_stats, voxhess, ratio) (bavoxel.hpp:650-660 with VOX_HESS::remove_residual :236-268, commented out in
+// the reference): erases from voxhess.plvec_voxels exactly the voxels the reference's walk would (lvba_lidar_remove_outliers;
+// the rule and its quirks are in include/lvba_b200.h), keeping the others in order.  Returns the library's status; on an error
+// (a ratio outside [0, 1), floor((1 - ratio) V) < 1, a non-finite lambda_0, a removal of every voxel) plvec_voxels is untouched.
+template <class PoseVec, class VoxHess>
+inline int remove_outlier(const PoseVec& x_stats, VoxHess& voxhess, double ratio, int64_t* n_removed = nullptr, int32_t device = -1) {
+  LidarCsr c = pack_lidar(x_stats, voxhess, "remove_outlier");
+  std::vector<uint8_t> removed((size_t)c.V(), 0);
+  lvba_lidar_problem* p = nullptr;
+  int rc = lvba_lidar_create(c.W, c.V(), c.vox_ptr.data(), c.pose_idx.data(), c.clusters.data(), c.poses.data(), device, &p);
+  if (rc == LVBA_OK) rc = lvba_lidar_remove_outliers(p, ratio, removed.data(), n_removed);
+  lvba_lidar_destroy(p);
+  if (rc != LVBA_OK) return rc;
+  size_t w = 0;                                        // plvec_voxels.erase for every removed voxel, survivors in order
+  for (size_t a = 0; a < removed.size(); ++a)
+    if (!removed[a]) voxhess.plvec_voxels[w++] = voxhess.plvec_voxels[a];
+  voxhess.plvec_voxels.resize(w);
   return LVBA_OK;
 }
 
@@ -209,6 +262,42 @@ class SurfMap {
     if (rc != LVBA_OK) return rc;
     if (summary) *summary = local;
     if (local.termination == LVBA_TERM_SKIPPED) return LVBA_OK;
+    for (int i = 0; i < win_size_; ++i) {
+      for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) x_stats[i].R(r, c) = poses[12 * i + 3 * r + c];
+      for (int r = 0; r < 3; ++r) x_stats[i].p(r) = poses[12 * i + 9 + r];
+    }
+    return LVBA_OK;
+  }
+
+  // damping_iter, remove_outlier(ratio) and damping_iter again on ONE device handle of the map's plane voxels (the sequence the
+  // reference's commented-out BALM2::remove_outlier, bavoxel.hpp:650-660, was written for): the second solve runs on the kept
+  // voxels from the poses of the first, with a fresh LM state.  pose_fixed: as damping_iter.  n_removed (may be null): the voxels
+  // erased.  x_stats is written back only on success.
+  int damping_iter_remove_outlier(PoseVec& x_stats, double ratio, const lvba_lidar_opts* opts = nullptr, int64_t* n_removed = nullptr,
+                                  lvba_summary* first = nullptr, lvba_summary* second = nullptr, const std::vector<uint8_t>* pose_fixed = nullptr) {
+    if (!map_) throw std::runtime_error("lvba_b200::SurfMap::damping_iter_remove_outlier: map not built");
+    if ((int)x_stats.size() < win_size_) throw std::runtime_error("lvba_b200::SurfMap::damping_iter_remove_outlier: x_stats smaller than win_size");
+    lvba_lidar_opts o;
+    opts = with_pose_fixed(opts, pose_fixed, win_size_, o, "SurfMap::damping_iter_remove_outlier");
+    lvba_lidar_opts d;
+    if (opts) d = *opts; else lvba_lidar_default_opts(&d);
+    std::vector<double> poses((size_t)win_size_ * 12);
+    for (int i = 0; i < win_size_; ++i) {
+      for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) poses[12 * i + 3 * r + c] = x_stats[i].R(r, c);
+      for (int r = 0; r < 3; ++r) poses[12 * i + 9 + r] = x_stats[i].p(r);
+    }
+    lvba_lidar_problem* p = nullptr;
+    lvba_summary s1{}, s2{};
+    int rc = lvba_voxel_map_lidar_create(map_, poses.data(), &p);
+    if (rc == LVBA_OK) rc = lvba_lidar_reset_lm(p, &d);
+    if (rc == LVBA_OK) rc = lvba_lidar_iterate(p, d.max_iter, &s1);
+    if (rc == LVBA_OK) rc = lvba_lidar_remove_outliers(p, ratio, nullptr, n_removed);
+    if (rc == LVBA_OK) rc = lvba_lidar_iterate(p, d.max_iter, &s2);
+    if (rc == LVBA_OK) rc = lvba_lidar_get_poses(p, poses.data());
+    lvba_lidar_destroy(p);
+    if (rc != LVBA_OK) return rc;
+    if (first) *first = s1;
+    if (second) *second = s2;
     for (int i = 0; i < win_size_; ++i) {
       for (int r = 0; r < 3; ++r) for (int c = 0; c < 3; ++c) x_stats[i].R(r, c) = poses[12 * i + 3 * r + c];
       for (int r = 0; r < 3; ++r) x_stats[i].p(r) = poses[12 * i + 9 + r];

@@ -202,7 +202,7 @@ int lvba_lidar_lm_batch(int32_t n_windows, const int32_t* win_ptr, int64_t V, co
                         int32_t min_voxels_per_pose, const lvba_lidar_opts* opts,
                         lvba_summary* summaries, lvba_summary* total);
 /* Device-resident handle for the same problem: lets a caller (bench, parity tests, a ROS
- * node that re-solves after outlier removal) run single phases with inputs already in HBM. */
+ * node that re-solves after outlier removal: lvba_lidar_remove_outliers) run single phases with inputs already in HBM. */
 typedef struct lvba_lidar_problem lvba_lidar_problem;
 
 int lvba_lidar_create(int32_t W, int64_t V, const int64_t* vox_ptr, const int32_t* pose_idx,
@@ -237,6 +237,37 @@ int lvba_lidar_iterate(lvba_lidar_problem* p, int32_t n_iter, lvba_summary* summ
  * pose pairs: those of the row system) */
 int lvba_lidar_counts(lvba_lidar_problem* p, int64_t* nnz, int64_t* n_blocks_env,
                       int64_t* n_blocks_nonzero, int64_t* n_pairs);
+
+/* ---- voxel outlier removal: BALM2's own rule, which the reference carries commented out in include/BALM/bavoxel.hpp.
+ * The three calls run on one GPU (an active communicator is LVBA_ERR_UNSUPPORTED) on a handle from lvba_lidar_create or
+ * lvba_voxel_map_lidar_create.  The handle's voxel order is the caller's order minus the voxels removed so far.
+ *
+ * VOX_HESS::evaluate_residual (bavoxel.hpp:205-234): lambda0 of every voxel at `poses` (host, W*12), or at the current
+ * device poses when NULL.  lambda0 [V] is in the handle's voxel order.  The values come from the arithmetic of
+ * lvba_lidar_residual, whose sum they give up to summation order. */
+int lvba_lidar_voxel_residuals(lvba_lidar_problem* p, const double* poses, double* lambda0);
+/* plvec_voxels.erase for every voxel with remove[a] != 0 (remove [V], handle order).  Survivors keep their relative order
+ * and are renumbered 0..n_left-1 (n_left may be NULL).  Afterwards the handle is planned as lvba_lidar_create on the kept
+ * voxels with the current poses and the handle's constant poses would be: the AVG_THR divisor is the kept count, and counts,
+ * structure, get_system and residual follow the kept voxels.  The poses and the poses lvba_lidar_reset_state restores stay as
+ * they are; removal is one-way.  The LM state is reset as lvba_lidar_reset_lm with the handle's options would reset it
+ * (deterministic mode stays on, its records set up again).  A NULL mask or one that removes every voxel is
+ * LVBA_ERR_INVALID_ARG with nothing removed.  A failed re-plan (deterministic mode's record set-up included) keeps the
+ * previous voxels with deterministic mode off and writes nothing to n_left, or, if restoring them fails too, leaves a handle
+ * that refuses every call but destroy and the pose copies. */
+int lvba_lidar_remove_voxels(lvba_lidar_problem* p, const uint8_t* remove, int64_t* n_left);
+/* BALM2::remove_outlier(x_stats, voxhess, ratio) (bavoxel.hpp:650-660 with VOX_HESS::remove_residual :236-268) at the
+ * current poses, then the re-plan of lvba_lidar_remove_voxels.  The rule is the reference's, in double, quirks included:
+ *   thr = sorted(lambda0)[floor((1 - ratio) V) - 1],  reject_num = floor(ratio V);
+ *   the voxels are walked in order, every voxel with lambda0 >= thr is erased, and the walk stops after the first KEPT voxel
+ *   at which the count of erased voxels equals reject_num.
+ * So it removes between reject_num and #{lambda0 >= thr} voxels, depending on where they sit: without ties that count is
+ * ceil(ratio V) + 1 when ratio V is an integer and floor(ratio V) + 2 otherwise.  With ratio = 0 (reject_num = 0) the walk
+ * can only stop at a first voxel that is kept: ratio = 0 removes nothing when the first voxel is below the maximum, and
+ * every maximal voxel when it is not.  removed [V before the call] (may be NULL): 1 for every erased voxel;
+ * n_removed (may be NULL).  LVBA_ERR_INVALID_ARG with the handle unchanged when ratio is not finite or outside [0, 1), when
+ * floor((1 - ratio) V) < 1, when some lambda0 is not finite, or when the rule would erase every voxel. */
+int lvba_lidar_remove_outliers(lvba_lidar_problem* p, double ratio, uint8_t* removed, int64_t* n_removed);
 
 /* ======================================================================================
  * B2  visual LM — replaces the Ceres block of LvbaSystem::optimizeCameraPoses(),

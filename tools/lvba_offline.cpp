@@ -40,6 +40,9 @@
 //                (an index past the last scan is an error, --check included): e.g. the first scan as the gauge, or the scans of a
 //                session optimised earlier.  Without --window both global stages hold them; with --window the window stage holds
 //                the listed frames and a global stage holds an anchor when every frame of its window is listed.
+//   --outlier-ratio R   BALM2::remove_outlier between two solves: each global stage runs damping_iter, remove_outlier(R) and
+//                damping_iter on one device handle of its voxel map (lvba_lidar_remove_outliers; the reference's rule, quirks included,
+//                include/lvba_b200.h).  R in [0, 1), checked when parsed (--check included); the window stage is unchanged.
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -62,6 +65,7 @@ int main(int argc, char** argv) {
   int fuse_order = LVBA_FUSE_ORDER_LIBSTDCXX;         // the library's default: what a g++ build of the reference does
   int window = 0;
   double anchor_leaf = 0.1;
+  double outlier_ratio = -1.0;                                               // < 0: no outlier removal
   std::string db_path, sparse_dir, lidar_opt, visual_problem, fix_cameras, fix_scans;
   lvba_b200::offline::Config cfg;
   lvba_visual_opts visual_opts;
@@ -100,6 +104,15 @@ int main(int argc, char** argv) {
       std::string e;
       fix_scans = next();
       if (!lvba_b200::offline::parse_index_ranges(fix_scans.c_str(), -1, unused, &e)) { std::fprintf(stderr, "--fix-scans: %s\n", e.c_str()); return 64; }
+    }
+    else if (a == "--outlier-ratio") {
+      const char* v = next();
+      char* end = nullptr;
+      outlier_ratio = std::strtod(v, &end);
+      if (end == v || *end != '\0' || !(outlier_ratio >= 0.0 && outlier_ratio < 1.0)) {
+        std::fprintf(stderr, "--outlier-ratio: '%s' is not a number in [0, 1)\n", v);
+        return 64;
+      }
     }
     else if (a == "--reproj-loss" || a == "--plane-loss") {
       const bool reproj = a == "--reproj-loss";
@@ -182,8 +195,17 @@ int main(int argc, char** argv) {
     lvba_b200::SurfMap<std::vector<Pose>> surf;
     rc = windows ? surf.build(anchor_clouds, poses, voxel[idx], eigen[idx], &vs) : surf.build(frame_clouds, poses, voxel[idx], eigen[idx], &vs);
     if (rc != LVBA_OK) { std::fprintf(stderr, "stage %d voxel map failed (%d): %s\n", idx + 1, rc, lvba_last_error()); return rc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
-    rc = surf.damping_iter(poses, 0, &lidar_opts, &s, pose_fixed.empty() ? nullptr : &pose_fixed);
+    int64_t n_removed = -1;
+    if (outlier_ratio >= 0.0) {
+      lvba_summary s1{};
+      rc = surf.damping_iter_remove_outlier(poses, outlier_ratio, &lidar_opts, &n_removed, &s1, &s, pose_fixed.empty() ? nullptr : &pose_fixed);
+      s.cost_first = s1.cost_first;
+      s.iterations += s1.iterations; s.accepted += s1.accepted; s.ms_total += s1.ms_total;
+    } else {
+      rc = surf.damping_iter(poses, 0, &lidar_opts, &s, pose_fixed.empty() ? nullptr : &pose_fixed);
+    }
     if (rc != LVBA_OK) { std::fprintf(stderr, "stage %d LM failed (%d): %s\n", idx + 1, rc, lvba_last_error()); return 1; }
+    if (n_removed >= 0) std::printf("{\"stage\": %d, \"outliers_removed\": %lld}\n", idx + 1, (long long)n_removed);
     std::printf("{\"stage\": %d, \"voxels\": %lld, \"clusters\": %lld, \"map_ms\": %.3f, \"iterations\": %d, \"accepted\": %d, \"cost_first\": %.9e, \"cost_last\": %.9e, \"lm_ms\": %.3f}\n",
                 idx + 1, (long long)vs.n_voxels, (long long)vs.nnz, vs.ms_total, s.iterations, s.accepted, s.cost_first, s.cost_last, s.ms_total);
   }
