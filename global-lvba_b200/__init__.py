@@ -35,7 +35,7 @@ EXPORTS = [
     "lvba_visual_lm", "lvba_visual_create", "lvba_visual_destroy", "lvba_visual_set_state",
     "lvba_visual_get_state", "lvba_visual_cost", "lvba_visual_step", "lvba_visual_structure",
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
-    "lvba_visual_big_counts",
+    "lvba_visual_big_counts", "lvba_visual_obs_residuals", "lvba_visual_remove_observations", "lvba_visual_remove_outliers",
     "lvba_voxel_default_opts", "lvba_voxel_map_create", "lvba_voxel_map_create_windows", "lvba_voxel_map_windows",
     "lvba_voxel_map_lidar_lm_batch", "lvba_voxel_map_summary", "lvba_voxel_map_export",
     "lvba_voxel_map_lookup", "lvba_voxel_map_lidar_create", "lvba_voxel_map_lidar_lm", "lvba_voxel_map_destroy",
@@ -433,6 +433,7 @@ class VisualProblem:
         op = np.ascontiguousarray(obs_ptr, np.int64); oc = np.ascontiguousarray(obs_cam, np.int32)
         uv = np.ascontiguousarray(obs_uv, np.float32); it = _f64(intr)
         self.M, self.T = q.shape[0], X.shape[0]
+        self.n_obs = int(op[-1])
         self._h = C.c_void_p()
         _chk(lib.lvba_visual_create(C.c_int32(self.M), C.c_int64(self.T), _p(q, C.c_double), _p(t, C.c_double),
                                     _p(X, C.c_double), _p(pl, C.c_double), _p(op, C.c_int64), _p(oc, C.c_int32),
@@ -510,6 +511,34 @@ class VisualProblem:
         a, b, c = C.c_int64(), C.c_int64(), C.c_int64()
         _chk(self._lib.lvba_visual_big_counts(self._h, C.byref(a), C.byref(b), C.byref(c)))
         return dict(n_big=a.value, n_big_obs=b.value, n_big_pairs=c.value)
+
+    def obs_residuals(self):
+        """s_q = r0^2 + r1^2 [N_obs] of every observation at the current state (lvba_visual_obs_residuals), indexed as the
+        obs_cam / obs_uv given at create: +inf where the camera-frame depth fails z > 1e-8, NaN for observations not in the
+        problem (landmark without a plane or dropped, observation removed)."""
+        out = np.empty(self.n_obs)
+        _chk(self._lib.lvba_visual_obs_residuals(self._h, _p(out, C.c_double)))
+        return out
+
+    def remove_observations(self, mask, min_track_len=3):
+        """Erase the observations where mask [N_obs] is true, then drop the landmarks left with fewer than min_track_len
+        observations (lvba_visual_remove_observations); returns (observations left, landmarks left)."""
+        m = np.ascontiguousarray(np.asarray(mask, bool), np.uint8)
+        if m.shape != (self.n_obs,):
+            raise ValueError(f"mask has shape {m.shape}, expected ({self.n_obs},)")
+        a, b = C.c_int64(), C.c_int64()
+        _chk(self._lib.lvba_visual_remove_observations(self._h, _p(m, C.c_uint8), C.c_int32(min_track_len), C.byref(a), C.byref(b)))
+        return a.value, b.value
+
+    def remove_outliers(self, max_err_px, min_track_len=3):
+        """Remove every observation whose reprojection error is not <= max_err_px, then the landmarks left with fewer than
+        min_track_len observations (lvba_visual_remove_outliers); returns the boolean mask [N_obs] of the observations this
+        call took out, and the number of landmarks it dropped."""
+        out = np.zeros(self.n_obs, np.uint8)
+        a, b = C.c_int64(), C.c_int64()
+        _chk(self._lib.lvba_visual_remove_outliers(self._h, C.c_double(max_err_px), C.c_int32(min_track_len), _p(out, C.c_uint8),
+                                                   C.byref(a), C.byref(b)))
+        return out.astype(bool), b.value
 
 
 # ------------------------------------------------------------------ B3: adaptive voxel map

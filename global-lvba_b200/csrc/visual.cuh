@@ -605,4 +605,23 @@ __global__ void visual_add_kernel(long long n, const double* __restrict__ X0, co
   if (i < n) out[i] = X0[i] + delta[i];
 }
 
+// ------------------------------------------------------------------------------------------------
+// Per-observation reprojection errors (lvba_visual_obs_residuals): one thread per local observation w, tile and big landmarks
+// alike.  sq[obs_src[w]] = r0^2 + r1^2 of obs_eval<false>, the term the cost pass sums before any loss, or +inf where the
+// camera-frame depth fails z > 1e-8 (obs_eval's residual, and the cost, are 0 there).  The landmark of w: the last k with
+// trk_ptr[k] <= w.
+__global__ void visual_obs_sq_kernel(VisualView vv, VisualState st, long long nnz, int Tv, const int64_t* __restrict__ obs_src,
+                                     double* __restrict__ sq) {
+  const long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (w >= nnz) return;
+  int lo = 0, hi = Tv;
+  while (hi - lo > 1) { const int m = (lo + hi) >> 1; if (vv.trk_ptr[m] <= w) lo = m; else hi = m; }
+  const long long tr = vv.trk_id[lo];
+  const long long cam = vv.obs_cam[w];
+  const double X[3] = {st.X[3 * tr], st.X[3 * tr + 1], st.X[3 * tr + 2]};
+  ObsEval o;
+  obs_eval<false>(vv, st.q + 4 * cam, st.t + 3 * cam, X, vv.obs_uv[w], o);
+  sq[obs_src[w]] = (obs_depth(st.q + 4 * cam, st.t + 3 * cam, X) > 1e-8) ? o.r[0] * o.r[0] + o.r[1] * o.r[1] : (double)INFINITY;
+}
+
 }  // namespace lvba

@@ -8,6 +8,7 @@
 #include "exec.cuh"
 #include "runtime.cuh"   // (pulls comm.cuh in)
 #include "visual.cuh"
+#include "visual_outliers.h"
 #include "visual_plan.h"
 
 namespace lvba {
@@ -66,6 +67,13 @@ struct lvba_visual_problem {
   double* h_scal = nullptr;
   int64_t launches = 0, h2d = 0, d2h = 0;
   double ms_setup = 0.0;
+  // ---- per-observation calls (visual_outliers.h): the caller's observation CSR as given at create (T + 1 offsets), the caller
+  // index of every local observation (obs_src, derived when a call first needs it; once it exists every re-plan carries it
+  // along, since after a removal it can no longer be derived), and the caller-indexed s_q of lvba_visual_obs_residuals
+  std::vector<int64_t> h_obs_ptr;
+  lvba::DevBuf<int64_t> obs_src;
+  bool obs_src_ready = false;
+  lvba::DevBuf<double> obs_sq;
   // LM state
   lvba_visual_opts opts;
   lvba::TrustRegionState lm;
@@ -138,6 +146,7 @@ struct VisualSrc {
   const int* cam = nullptr;
   const float2* uv = nullptr;
   const double* plane = nullptr;
+  const int64_t* obs_src = nullptr;    // the caller index of every source observation, gathered into P->obs_src; null: none yet
 };
 
 // Everything the handle derives from its system rows (row_of_cam and P->cam_of_row): the envelope and the solver path, the
@@ -192,6 +201,8 @@ inline int visual_plan(lvba_visual_problem* P, const std::vector<int64_t>& valid
   LVBA_TRY(P->batch_trk.upload(L.batch_trk, s, &P->h2d));
   LVBA_TRY(P->tile_trk.upload(L.tile_trk, s, &P->h2d));
   P->n_pairs = 0;
+  P->obs_src.release();
+  P->obs_src_ready = false;
   if (Tv > 0) {
     VisualSrc src;
     LVBA_TRY(get_src(src));
@@ -213,6 +224,11 @@ inline int visual_plan(lvba_visual_problem* P, const std::vector<int64_t>& valid
     ++P->launches;
     CudaExec ex;                                               // the destination table covers the small landmarks only
     ex.stream = s;
+    if (src.obs_src) {
+      LVBA_TRY(P->obs_src.alloc((size_t)P->nnz));
+      LVBA_TRY(ex.for_each(Tv, voutliers::GatherSrcF{src_id ? d_src_trk.p : P->trk_id.p, P->trk_ptr.p, src.obs_ptr, src.obs_src, P->obs_src.p}));
+      P->obs_src_ready = true;
+    }
     int64_t np = 0;
     LVBA_TRY(visual_tables(ex, P->table_in(), Tv_small, L.n_ordered, L.trk_ptr[Tv_small], P->prun, P->drun, &np));
     P->launches += ex.launches;
@@ -274,6 +290,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   P->cam_fixed = visual_mask(M, cam_fixed);
   for (int i = 0; i < 8; ++i) P->intr[i] = intr[i];
   P->sigma_px = sigma_px; P->sigma_pl = sigma_plane;
+  P->h_obs_ptr.assign(obs_ptr, obs_ptr + T + 1);
   LVBA_CUDA(cudaGetDevice(&P->device));
   LVBA_CUDA(cudaStreamCreateWithFlags(&P->stream, cudaStreamNonBlocking));
   P->timers.stream = P->stream;
@@ -330,14 +347,29 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   return LVBA_OK;
 }
 
-// A new set of constant cameras on a handle (lvba_visual_reset_lm): visual_plan again, from the handle's own arrays.  The
-// source landmarks are the local landmarks of the current plan, taken in the caller's order, so that the new plan is the one
-// lvba_visual_create would make with this mask; observations, planes and the state stay on the device.  One GPU only: the
-// local landmarks are then all valid ones (visual_set_mode refuses a mask under an active communicator).
+inline int visual_det_setup(lvba_visual_problem* P);
+
+// A removal of observations (lvba_visual_remove_observations / _remove_outliers) for visual_replan: host copies of the rule's
+// keep flags [nnz] and kept counts [Tv] over the current local CSR, and the kept observations' camera, pixel and caller index,
+// compacted on the device in the local order (voutliers::CompactF).
+struct VisualKept {
+  const uint8_t* keep = nullptr;
+  const int32_t* kcnt = nullptr;
+  const int* cam = nullptr;
+  const float2* uv = nullptr;
+  const int64_t* src = nullptr;
+};
+
+// A new set of constant cameras on a handle (lvba_visual_reset_lm), or a removal (kept != null): visual_plan again, from the
+// handle's own arrays.  The source landmarks are the local landmarks of the current plan, taken in the caller's order, so that
+// the new plan is the one lvba_visual_create would make with this mask (and, after a removal, from the kept observations with
+// the dropped landmarks' planes left out); observations, planes and the state stay on the device.  One GPU only: the local
+// landmarks are then all valid ones (visual_set_mode and the removal calls refuse an active communicator).
+// Deterministic mode is off afterwards unless `det` asks for its records as part of the new plan.
 // A failure leaves the handle as it was (the previous plan is made again from the same source arrays) with deterministic mode
 // off; only if that fails too is the handle marked unusable, and then every call but destroy, get_state, set_state and
 // reset_state refuses it.
-inline int visual_replan(lvba_visual_problem* P, std::vector<uint8_t> mask) {
+inline int visual_replan(lvba_visual_problem* P, std::vector<uint8_t> mask, const VisualKept* kept = nullptr, bool det = false) {
   SetupLaps lap("visual re-plan", 26, P->stream, wall_ms());
   cudaStream_t s = P->stream;
   const int64_t Tv = P->Tv;
@@ -349,46 +381,63 @@ inline int visual_replan(lvba_visual_problem* P, std::vector<uint8_t> mask) {
     LVBA_CUDA(cudaStreamSynchronize(s));
     P->d2h += (int64_t)(trk_ptr.size() + trk_id.size() + cam.size()) * (int64_t)sizeof(int);
   }
-  std::vector<int64_t> valid((size_t)Tv), src_ptr(trk_ptr.begin(), trk_ptr.end());
-  for (int64_t k = 0; k < Tv; ++k) valid[k] = k;
-  std::sort(valid.begin(), valid.end(), [&](int64_t a, int64_t b) { return trk_id[a] < trk_id[b]; });
-  std::vector<char> used((size_t)P->M, 0);
-  for (int c : cam) used[c] = 1;
+  voutliers::ReplanSource all, cut;
+  voutliers::replan_source(Tv, trk_id.data(), trk_ptr.data(), cam.data(), nullptr, nullptr, all);
+  if (kept) voutliers::replan_source(Tv, trk_id.data(), trk_ptr.data(), cam.data(), kept->keep, kept->kcnt, cut);
   lap("rows");
   // the records of deterministic mode follow the table: set up again when the mode is next asked for (visual_set_mode)
-  tiles::fixed_sum_release(P->det_S); tiles::fixed_sum_release(P->det_G); P->det_C.release();
-  P->det_ready = false;
-  P->det = false;
-  P->solver.set_deterministic(false);
+  auto det_release = [&] {
+    tiles::fixed_sum_release(P->det_S); tiles::fixed_sum_release(P->det_G); P->det_C.release();
+    P->det_ready = false;
+    P->det = false;
+    P->solver.set_deterministic(false);
+  };
+  det_release();
   DevBuf<long long> d_src_ptr;
   DevBuf<int> old_cam;
   DevBuf<float2> old_uv;
   DevBuf<double> old_plane;
-  old_cam.swap(P->obs_cam); old_uv.swap(P->obs_uv); old_plane.swap(P->plane);
-  auto old_arrays = [&](VisualSrc& src) -> int {
-    LVBA_TRY(d_src_ptr.upload(reinterpret_cast<const long long*>(src_ptr.data()), src_ptr.size(), s, &P->h2d));
-    src = VisualSrc{d_src_ptr.p, old_cam.p, old_uv.p, old_plane.p};
-    return LVBA_OK;
-  };
-  auto plan_with = [&](const std::vector<uint8_t>& m) -> int {
+  DevBuf<int64_t> old_src;
+  const bool had_src = P->obs_src_ready;
+  old_cam.swap(P->obs_cam); old_uv.swap(P->obs_uv); old_plane.swap(P->plane); old_src.swap(P->obs_src);
+  auto plan_with = [&](const std::vector<uint8_t>& m, const voutliers::ReplanSource& S, const VisualSrc& arrays, bool with_det) -> int {
+    std::vector<char> used((size_t)P->M, 0);
+    for (int c : S.cam) used[c] = 1;
     std::vector<int> row_of_cam;
     visual_row_map(P->M, used, P->fixed_cam, m.empty() ? nullptr : m.data(), row_of_cam, P->cam_of_row);
-    LVBA_TRY(visual_plan(P, valid, src_ptr.data(), cam.data(), row_of_cam, trk_id.data(), old_arrays, lap));
+    auto get = [&](VisualSrc& src) -> int {
+      LVBA_TRY(d_src_ptr.upload(reinterpret_cast<const long long*>(S.src_ptr.data()), S.src_ptr.size(), s, &P->h2d));
+      src = arrays;
+      src.obs_ptr = d_src_ptr.p;
+      return LVBA_OK;
+    };
+    LVBA_TRY(visual_plan(P, S.valid, S.src_ptr.data(), S.cam.data(), row_of_cam, trk_id.data(), get, lap));
+    if (with_det) {
+      LVBA_TRY(visual_det_setup(P));
+      P->det = true;
+      P->solver.set_deterministic(true);
+    }
     return P->scal.zero(s);                                    // no stale camera gradient when the new plan has no rows
   };
+  const VisualSrc old_arrays{nullptr, old_cam.p, old_uv.p, old_plane.p, had_src ? old_src.p : nullptr};
+  const char* what = kept ? "re-plan after the removal" : "re-plan for the new cam_fixed";
+  const char* keeps = kept ? "nothing was removed" : "the handle keeps its previous constant cameras";
   int rc;
-  try { rc = plan_with(mask); } catch (const std::bad_alloc&) { rc = fail(LVBA_ERR_NOMEM, "host allocation failed"); }
+  try {
+    rc = kept ? plan_with(mask, cut, VisualSrc{nullptr, kept->cam, kept->uv, old_plane.p, kept->src}, det) : plan_with(mask, all, old_arrays, false);
+  } catch (const std::bad_alloc&) { rc = fail(LVBA_ERR_NOMEM, "host allocation failed"); }
   if (rc != LVBA_OK) {
     const std::string why = last_error_ref();
     cudaStreamSynchronize(s);
     cudaGetLastError();
+    det_release();
     int rc_back;
-    try { rc_back = plan_with(P->cam_fixed); } catch (const std::bad_alloc&) { rc_back = LVBA_ERR_NOMEM; }
+    try { rc_back = plan_with(P->cam_fixed, all, old_arrays, false); } catch (const std::bad_alloc&) { rc_back = LVBA_ERR_NOMEM; }
     if (rc_back != LVBA_OK) {
       P->unusable = true;
-      return fail(rc, "re-plan for the new cam_fixed failed (%s), and so did restoring the previous plan: destroy the handle", why.c_str());
+      return fail(rc, "%s failed (%s), and so did restoring the previous plan: destroy the handle", what, why.c_str());
     }
-    return fail(rc, "re-plan for the new cam_fixed failed (%s); the handle keeps its previous constant cameras", why.c_str());
+    return fail(rc, "%s failed (%s); %s", what, why.c_str(), keeps);
   }
   P->cam_fixed = std::move(mask);
   return LVBA_OK;
@@ -683,6 +732,114 @@ inline int visual_iterate_impl(lvba_visual_problem* P, int n_iter, lvba_summary*
   return LVBA_OK;
 }
 
+
+// ---------------------------------------------------------------- per-observation residuals and removal (visual_outliers.h)
+// the calls that read or change the handle's observation set: one GPU (a rank holds only its own landmarks)
+inline int visual_check_obs_calls(const lvba_visual_problem* P) {
+  LVBA_TRY(visual_check_usable(P));
+  if (comm().active()) return fail(LVBA_ERR_UNSUPPORTED, "per-observation residuals and removal run on one GPU: not with an active communicator");
+  return LVBA_OK;
+}
+
+// obs_src: derived from trk_id, trk_ptr and the caller's obs_ptr while nothing has been removed (afterwards it always exists)
+inline int visual_obs_src(lvba_visual_problem* P) {
+  if (P->obs_src_ready) return LVBA_OK;
+  cudaStream_t s = P->stream;
+  LVBA_TRY(P->obs_src.alloc((size_t)P->nnz));
+  if (P->Tv > 0) {
+    DevBuf<int64_t> d_ptr;
+    LVBA_TRY(d_ptr.upload(P->h_obs_ptr, s, &P->h2d));
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(ex.for_each(P->Tv, voutliers::DeriveSrcF{P->trk_id.p, P->trk_ptr.p, d_ptr.p, P->obs_src.p}));
+    P->launches += ex.launches;
+    LVBA_CUDA(cudaStreamSynchronize(s));                       // d_ptr is idle before it is parked
+  }
+  P->obs_src_ready = true;
+  return LVBA_OK;
+}
+
+// s_q of every caller observation at the current state into P->obs_sq [N_obs]: NaN everywhere, then the observations in the
+// problem (visual_obs_sq_kernel)
+inline int visual_obs_sq_dev(lvba_visual_problem* P) {
+  cudaStream_t s = P->stream;
+  const int64_t n_obs = P->h_obs_ptr[(size_t)P->T];
+  LVBA_TRY(visual_obs_src(P));
+  if (P->obs_sq.n < (size_t)n_obs) LVBA_TRY(P->obs_sq.alloc((size_t)n_obs));
+  CudaExec ex;
+  ex.stream = s;
+  LVBA_TRY(ex.for_each(n_obs, voutliers::NanFillF{P->obs_sq.p}));
+  P->launches += ex.launches;
+  if (P->nnz > 0) {
+    visual_obs_sq_kernel<<<(unsigned)((P->nnz + 255) / 256), 256, 0, s>>>(P->view(), P->state(), P->nnz, (int)P->Tv, P->obs_src.p, P->obs_sq.p);
+    LVBA_CUDA(cudaGetLastError());
+    ++P->launches;
+  }
+  return LVBA_OK;
+}
+
+// The removal: keep flags by the caller's device mask d_remove [N_obs] (or, when null, s_q in P->obs_sq <= tau), the dropped
+// landmarks, then the re-plan from the kept observations compacted on the device (visual_replan).  Only the keep flags and the
+// kept counts come to the host.  Refused with nothing changed when no observation would be left.  The LM state is reset as
+// lvba_visual_reset_lm with the handle's options would reset it; deterministic mode's records are set up again with the plan.
+// Outputs are written on success only.
+inline int visual_remove_impl(lvba_visual_problem* P, const uint8_t* d_remove, double tau, int32_t min_len, uint8_t* removed,
+                              int64_t* n_obs_left, int64_t* n_trk_left, int64_t* n_rm_obs, int64_t* n_rm_trk) {
+  cudaStream_t s = P->stream;
+  const int64_t n_obs = P->h_obs_ptr[(size_t)P->T], nnz = P->nnz, Tv = P->Tv;
+  LVBA_TRY(visual_obs_src(P));
+  CudaExec ex;
+  ex.stream = s;
+  voutliers::RuleBufs<CudaExec> B;
+  int64_t kept_obs = 0, kept_trk = 0;
+  LVBA_TRY(voutliers::keep_rule(ex, nnz, Tv, P->trk_ptr.p, P->obs_src.p, d_remove, P->obs_sq.p, tau, min_len, B, &kept_obs, &kept_trk));
+  P->d2h += 8;
+  if (kept_obs == 0) return fail(LVBA_ERR_INVALID_ARG, "the removal would leave no observation in the problem");
+  std::vector<uint8_t> h_removed;
+  if (removed) {
+    DevBuf<uint8_t> d_rm;
+    LVBA_TRY(d_rm.alloc((size_t)n_obs));
+    LVBA_TRY(ex.fill_zero(d_rm.p, (size_t)n_obs));
+    LVBA_TRY(ex.for_each(nnz, voutliers::RemovedF{B.keep.p, P->obs_src.p, d_rm.p}));
+    h_removed.resize((size_t)n_obs);
+    LVBA_TRY(ex.fetch(h_removed.data(), d_rm.p, (size_t)n_obs));
+    P->d2h += n_obs;
+  }
+  if (kept_obs < nnz || kept_trk < Tv) {
+    std::vector<uint8_t> keep((size_t)nnz);
+    std::vector<int32_t> kcnt((size_t)Tv);
+    DevBuf<uint8_t> d_keep;
+    LVBA_TRY(d_keep.alloc((size_t)nnz));
+    LVBA_TRY(ex.for_each(nnz, voutliers::KeepBytesF{B.keep.p, d_keep.p}));
+    LVBA_TRY(ex.fetch(keep.data(), d_keep.p, (size_t)nnz));
+    LVBA_TRY(ex.fetch(kcnt.data(), B.kcnt.p, (size_t)Tv));
+    P->d2h += nnz + Tv * 4;
+    DevBuf<int> ccam;
+    DevBuf<float2> cuv;
+    DevBuf<int64_t> csrc;
+    LVBA_TRY(ccam.alloc((size_t)kept_obs)); LVBA_TRY(cuv.alloc((size_t)kept_obs)); LVBA_TRY(csrc.alloc((size_t)kept_obs));
+    LVBA_TRY(ex.for_each(nnz, voutliers::CompactF{B.keep.p, B.pos.p, P->obs_cam.p, P->obs_uv.p, P->obs_src.p, ccam.p, cuv.p, csrc.p}));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    const VisualKept K{keep.data(), kcnt.data(), ccam.p, cuv.p, csrc.p};
+    LVBA_TRY(visual_replan(P, P->cam_fixed, &K, P->det));
+    // the candidate starts as the state: a dropped landmark or a camera without observations is no longer written by a step,
+    // and an accepted step swaps the buffers, so its candidate entry must hold its state
+    const size_t nq = (size_t)P->M * 4 * sizeof(double), nt = (size_t)P->M * 3 * sizeof(double), nx = (size_t)P->T * 3 * sizeof(double);
+    LVBA_CUDA(cudaMemcpyAsync(P->qc.p, P->q.p, nq, cudaMemcpyDeviceToDevice, s));
+    LVBA_CUDA(cudaMemcpyAsync(P->tc.p, P->t.p, nt, cudaMemcpyDeviceToDevice, s));
+    if (nx) LVBA_CUDA(cudaMemcpyAsync(P->Xc.p, P->X.p, nx, cudaMemcpyDeviceToDevice, s));
+    LVBA_CUDA(cudaStreamSynchronize(s));                       // the compacted arrays are idle before they are parked
+  }
+  P->launches += ex.launches;
+  P->lm.reset(P->opts);
+  if (removed) std::copy(h_removed.begin(), h_removed.end(), removed);
+  if (n_obs_left) *n_obs_left = kept_obs;
+  if (n_trk_left) *n_trk_left = kept_trk;
+  if (n_rm_obs) *n_rm_obs = nnz - kept_obs;
+  if (n_rm_trk) *n_rm_trk = Tv - kept_trk;
+  return LVBA_OK;
+}
+
 }  // namespace lvba
 
 extern "C" {
@@ -868,5 +1025,47 @@ int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const 
   return lvba::lm_one_shot(p, o, p->Tv > 0, lvba_visual_reset_lm, lvba_visual_iterate, lvba_visual_destroy,
                            [&] { return lvba_visual_get_state(p, q, t, X); }, t0, summary);   // write-back, src/lvba_system.cpp:1651-1665
 } LVBA_ABI_END("lvba_visual_lm")
+
+
+int lvba_visual_obs_residuals(lvba_visual_problem* p, double* sq_res) LVBA_ABI_BEGIN {
+  if (!p || !sq_res) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_obs_calls(p));
+  LVBA_CUDA(cudaSetDevice(p->device));
+  LVBA_TRY(lvba::visual_obs_sq_dev(p));
+  const int64_t n_obs = p->h_obs_ptr[(size_t)p->T];
+  LVBA_CUDA(cudaMemcpyAsync(sq_res, p->obs_sq.p, (size_t)n_obs * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  LVBA_CUDA(cudaStreamSynchronize(p->stream));
+  p->d2h += n_obs * 8;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_obs_residuals")
+
+int lvba_visual_remove_observations(lvba_visual_problem* p, const uint8_t* remove, int32_t min_track_len, int64_t* n_obs_left,
+                                    int64_t* n_tracks_left) LVBA_ABI_BEGIN {
+  if (!p || !remove) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_obs_calls(p));
+  if (min_track_len < 1) return lvba::fail(LVBA_ERR_INVALID_ARG, "min_track_len=%d: it must be >= 1", (int)min_track_len);
+  LVBA_CUDA(cudaSetDevice(p->device));
+  const int64_t n_obs = p->h_obs_ptr[(size_t)p->T];
+  lvba::DevBuf<uint8_t> d_mask;
+  LVBA_TRY(d_mask.upload(remove, (size_t)n_obs, p->stream, &p->h2d));
+  const int rc = lvba::visual_remove_impl(p, d_mask.p, 0.0, min_track_len, nullptr, n_obs_left, n_tracks_left, nullptr, nullptr);
+  cudaStreamSynchronize(p->stream);                            // d_mask is idle before it is parked
+  return rc;
+} LVBA_ABI_END("lvba_visual_remove_observations")
+
+int lvba_visual_remove_outliers(lvba_visual_problem* p, double max_err_px, int32_t min_track_len, uint8_t* removed,
+                                int64_t* n_removed_obs, int64_t* n_removed_tracks) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_obs_calls(p));
+  if (!(std::isfinite(max_err_px) && max_err_px > 0.0))
+    return lvba::fail(LVBA_ERR_INVALID_ARG, "max_err_px=%g: it must be finite and > 0", max_err_px);
+  if (min_track_len < 1) return lvba::fail(LVBA_ERR_INVALID_ARG, "min_track_len=%d: it must be >= 1", (int)min_track_len);
+  LVBA_CUDA(cudaSetDevice(p->device));
+  const double e = max_err_px / p->sigma_px;
+  // an overflowing threshold stays finite, so that +inf (the depth test failed) is still above it
+  const double tau = std::min(e * e, DBL_MAX);
+  LVBA_TRY(lvba::visual_obs_sq_dev(p));
+  return lvba::visual_remove_impl(p, nullptr, tau, min_track_len, removed, nullptr, nullptr, n_removed_obs, n_removed_tracks);
+} LVBA_ABI_END("lvba_visual_remove_outliers")
 
 }  // extern "C"

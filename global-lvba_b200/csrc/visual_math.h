@@ -153,6 +153,21 @@ LVBA_UNROLL
     }
 }
 
+// The camera-frame depth obs_eval tests (utils.hpp:78), with obs_eval's arithmetic step for step, so that the two agree on
+// every bit.  A function of its own rather than a part factored out of obs_eval: that keeps the code of the kernels that call
+// obs_eval as it was.
+LVBA_HD double obs_depth(const double* __restrict__ qp, const double* __restrict__ tp, const double* X) {
+  double q0 = qp[0], q1 = qp[1], q2 = qp[2], q3 = qp[3];
+  const double inv = 1.0 / sqrt(q0 * q0 + q1 * q1 + q2 * q2 + q3 * q3);
+  q0 *= inv; q1 *= inv; q2 *= inv; q3 *= inv;
+  const double v[3] = {q1, q2, q3};
+  double vxX[3], t2[3];
+  cross3(v, X, vxX);
+  const double uvv[3] = {2.0 * vxX[0], 2.0 * vxX[1], 2.0 * vxX[2]};
+  cross3(v, uvv, t2);
+  return X[2] + q0 * uvv[2] + t2[2] + tp[2];
+}
+
 // utils.hpp:133-139
 LVBA_HD void plane_eval(const VisualView& vv, const double* pl, const double* X, double& r, double J[3]) {
   const double e = -(pl[0] * X[0] + pl[1] * X[1] + pl[2] * X[2] + pl[3]);

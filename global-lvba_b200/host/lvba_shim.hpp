@@ -8,6 +8,7 @@
 //   lvba_b200::evaluate_residual(x_stats, voxhess)   VOX_HESS::evaluate_residual (commented out in the reference, :205-234)
 //   lvba_b200::remove_outlier(x_stats, voxhess, r)   BALM2::remove_outlier (commented out in the reference, :650-660)
 //   lvba_b200::solve_visual(...)                     replaces the Ceres block       src/lvba_system.cpp:1571-1656
+//   lvba_b200::solve_visual_remove_outliers(...)     the same, then a reprojection filter and a second solve on one handle
 //   lvba_b200::WindowBatch                           collects the windows of runWindowBA (src/lvba_system.cpp:232-302) and
 //                                                    solves them in one lvba_lidar_lm_batch call
 //   lvba_b200::SurfMap                               replaces the surf_map built by cut_voxel + recut (+ tras_opt) in front of
@@ -564,6 +565,40 @@ class DepthRenderer {
 //      observation list it walks at :1614-1631.  obs_of_point[pi] = list of (cam_id, u, v).
 struct Observation { int cam; float u, v; };
 
+// The ABI's CSR of the per-point observation lists and the (n, d) planes; throws on size mismatches (who: the caller's name)
+struct VisualCsr {
+  std::vector<int64_t> obs_ptr;
+  std::vector<int32_t> obs_cam;
+  std::vector<float> obs_uv;
+  std::vector<double> plane_nd;
+};
+inline VisualCsr pack_visual(int M, const std::vector<std::array<double, 3>>& ts, const std::vector<std::array<double, 3>>& Xs,
+                             const std::vector<std::array<double, 3>>& plane_n, const std::vector<double>& plane_d,
+                             const std::vector<std::vector<Observation>>& obs_of_point, const std::vector<uint8_t>* cam_fixed, const char* who) {
+  const int64_t T = (int64_t)Xs.size();
+  if ((int)ts.size() != M) throw std::runtime_error(std::string("lvba_b200::") + who + ": qs/ts size mismatch");      // cf. :1427
+  if ((int64_t)plane_n.size() != T || (int64_t)plane_d.size() != T || (int64_t)obs_of_point.size() != T)
+    throw std::runtime_error(std::string("lvba_b200::") + who + ": per-point array size mismatch");
+  if (cam_fixed && (int)cam_fixed->size() != M) throw std::runtime_error(std::string("lvba_b200::") + who + ": cam_fixed needs one entry per camera");
+  VisualCsr c;
+  c.obs_ptr.assign((size_t)T + 1, 0);
+  c.plane_nd.resize((size_t)T * 4);
+  for (int64_t i = 0; i < T; ++i) {
+    for (const auto& o : obs_of_point[i]) { c.obs_cam.push_back(o.cam); c.obs_uv.push_back(o.u); c.obs_uv.push_back(o.v); }
+    c.obs_ptr[i + 1] = (int64_t)c.obs_cam.size();
+    c.plane_nd[4 * i] = plane_n[i][0]; c.plane_nd[4 * i + 1] = plane_n[i][1]; c.plane_nd[4 * i + 2] = plane_n[i][2]; c.plane_nd[4 * i + 3] = plane_d[i];
+  }
+  return c;
+}
+
+// opts (null: the defaults) with cam_fixed (null: opts' own) in o; returns the options to pass
+inline const lvba_visual_opts* with_cam_fixed(const lvba_visual_opts* opts, const std::vector<uint8_t>* cam_fixed, lvba_visual_opts& o) {
+  if (!cam_fixed) return opts;
+  if (opts) o = *opts; else lvba_visual_default_opts(&o);
+  o.cam_fixed = cam_fixed->data();
+  return &o;
+}
+
 // opts: null = lvba_visual_default_opts, plain least squares as the reference's nullptr losses (:1630, :1639).  Its
 // loss_function_reproj / loss_function_plane (HuberLoss(1.0) / HuberLoss(0.1), :1585-1586) map to reproj_loss = plane_loss =
 // LVBA_LOSS_HUBER with the default scales 1.0 / 0.1 (INTEGRATION.md, B2).  Camera 0 is constant, as in the reference
@@ -577,30 +612,60 @@ inline int solve_visual(std::vector<std::array<double, 4>>& qs, std::vector<std:
                         lvba_summary* summary = nullptr, const std::vector<uint8_t>* cam_fixed = nullptr) {
   const int M = (int)qs.size();
   const int64_t T = (int64_t)Xs.size();
-  if ((int)ts.size() != M) throw std::runtime_error("lvba_b200::solve_visual: qs/ts size mismatch");      // cf. :1427
-  if ((int64_t)plane_n.size() != T || (int64_t)plane_d.size() != T || (int64_t)obs_of_point.size() != T)
-    throw std::runtime_error("lvba_b200::solve_visual: per-point array size mismatch");
-  if (cam_fixed && (int)cam_fixed->size() != M) throw std::runtime_error("lvba_b200::solve_visual: cam_fixed needs one entry per camera");
+  const VisualCsr c = pack_visual(M, ts, Xs, plane_n, plane_d, obs_of_point, cam_fixed, "solve_visual");
   lvba_visual_opts o;
-  if (cam_fixed) {
-    if (opts) o = *opts; else lvba_visual_default_opts(&o);
-    o.cam_fixed = cam_fixed->data();
-    opts = &o;
-  }
-  std::vector<int64_t> obs_ptr(T + 1, 0);
-  std::vector<int32_t> obs_cam;
-  std::vector<float> obs_uv;
-  std::vector<double> plane_nd((size_t)T * 4);
-  for (int64_t i = 0; i < T; ++i) {
-    for (const auto& o : obs_of_point[i]) { obs_cam.push_back(o.cam); obs_uv.push_back(o.u); obs_uv.push_back(o.v); }
-    obs_ptr[i + 1] = (int64_t)obs_cam.size();
-    plane_nd[4 * i] = plane_n[i][0]; plane_nd[4 * i + 1] = plane_n[i][1]; plane_nd[4 * i + 2] = plane_n[i][2]; plane_nd[4 * i + 3] = plane_d[i];
-  }
+  opts = with_cam_fixed(opts, cam_fixed, o);
   const double intr[8] = {fx, fy, cx, cy, k1, k2, p1, p2};
   // qs/ts/Xs are contiguous arrays of std::array<double,N>: exactly the M*4 / M*3 / T*3 layout of the ABI
   return lvba_visual_lm(M, T, qs.empty() ? nullptr : qs[0].data(), ts.empty() ? nullptr : ts[0].data(),
-                        Xs.empty() ? nullptr : Xs[0].data(), plane_nd.data(), obs_ptr.data(), obs_cam.data(), obs_uv.data(), intr,
+                        Xs.empty() ? nullptr : Xs[0].data(), c.plane_nd.data(), c.obs_ptr.data(), c.obs_cam.data(), c.obs_uv.data(), intr,
                         sigma_px, sigma_plane, /*fixed_cam=*/0, opts, summary);
+}
+
+// solve_visual, then lvba_visual_remove_outliers(max_err_px, min_track_len), then a second solve, on one device handle: the
+// solve, filter, solve-again loop of a Ceres bundle adjustment (include/lvba_b200.h, B2, states the rule).  Each solve is
+// lvba_visual_reset_lm with opts (and cam_fixed) and up to opts->max_iter iterations; summary_first / summary_second (may be
+// null) are their summaries.  removed (may be null) gets one entry per observation of obs_of_point, in its order: 1 for every
+// observation the filter took out, those of dropped landmarks included, so that a caller can erase the same entries from its
+// tr.inlier_indices.  A landmark whose observations are all removed is dropped: its Xs entry comes back as the first solve left
+// it, and the caller treats it as a landmark without a plane.  qs, ts, Xs are written back after the second solve.
+inline int solve_visual_remove_outliers(std::vector<std::array<double, 4>>& qs, std::vector<std::array<double, 3>>& ts,
+                                        std::vector<std::array<double, 3>>& Xs, const std::vector<std::array<double, 3>>& plane_n,
+                                        const std::vector<double>& plane_d, const std::vector<std::vector<Observation>>& obs_of_point,
+                                        double fx, double fy, double cx, double cy, double k1, double k2, double p1, double p2,
+                                        double sigma_px, double sigma_plane, const lvba_visual_opts* opts, double max_err_px,
+                                        int32_t min_track_len, std::vector<std::vector<uint8_t>>* removed = nullptr,
+                                        lvba_summary* summary_first = nullptr, lvba_summary* summary_second = nullptr,
+                                        const std::vector<uint8_t>* cam_fixed = nullptr) {
+  const int M = (int)qs.size();
+  const int64_t T = (int64_t)Xs.size();
+  const VisualCsr c = pack_visual(M, ts, Xs, plane_n, plane_d, obs_of_point, cam_fixed, "solve_visual_remove_outliers");
+  lvba_visual_opts o;
+  opts = with_cam_fixed(opts, cam_fixed, o);
+  lvba_visual_opts d;
+  lvba_visual_default_opts(&d);
+  const lvba_visual_opts& use = opts ? *opts : d;
+  const double intr[8] = {fx, fy, cx, cy, k1, k2, p1, p2};
+  lvba_visual_problem* p = nullptr;
+  int rc = lvba_visual_create(M, T, qs.empty() ? nullptr : qs[0].data(), ts.empty() ? nullptr : ts[0].data(), Xs.empty() ? nullptr : Xs[0].data(),
+                              c.plane_nd.data(), c.obs_ptr.data(), c.obs_cam.data(), c.obs_uv.data(), intr, sigma_px, sigma_plane,
+                              /*fixed_cam=*/0, use.device, &p);
+  if (rc != LVBA_OK) return rc;
+  std::vector<uint8_t> mask((size_t)c.obs_ptr[(size_t)T]);
+  if (rc == LVBA_OK) rc = lvba_visual_reset_lm(p, &use);
+  if (rc == LVBA_OK) rc = lvba_visual_iterate(p, use.max_iter, summary_first);
+  if (rc == LVBA_OK) rc = lvba_visual_remove_outliers(p, max_err_px, min_track_len, mask.data(), nullptr, nullptr);
+  if (rc == LVBA_OK) rc = lvba_visual_iterate(p, use.max_iter, summary_second);
+  if (rc == LVBA_OK)
+    rc = lvba_visual_get_state(p, qs.empty() ? nullptr : qs[0].data(), ts.empty() ? nullptr : ts[0].data(), Xs.empty() ? nullptr : Xs[0].data());
+  lvba_visual_destroy(p);
+  if (rc != LVBA_OK) return rc;
+  if (removed) {
+    removed->assign((size_t)T, {});
+    for (int64_t i = 0; i < T; ++i)
+      (*removed)[(size_t)i].assign(mask.begin() + c.obs_ptr[(size_t)i], mask.begin() + c.obs_ptr[(size_t)i + 1]);
+  }
+  return LVBA_OK;
 }
 
 // ---- B7: BuildTracksAndFuse3D (src/lvba_system.cpp:921-1263).  all_keypoints[i][k].x/.y, all_matches[pairIndex(i,j,N)] =

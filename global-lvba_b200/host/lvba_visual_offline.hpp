@@ -443,7 +443,9 @@ struct VisualResult {
   lvba_fuse_summary fuse{};
   lvba_depth_summary depth{};
   lvba_voxel_summary surf{};
-  lvba_summary solve{};
+  lvba_summary solve{};                        // the solve (with a reprojection filter: the second one)
+  lvba_summary solve_first{};                  // with a reprojection filter: the solve before it
+  int64_t obs_removed = 0, points_dropped = 0;  // with a reprojection filter: what it took out
   int64_t usable_tracks = 0, points_kept = 0, keypoints = 0, matches = 0, anchor_points = 0, depth_valid = 0;
   int anchors = 0;
 };
@@ -487,11 +489,13 @@ inline bool write_visual_problem(const std::string& path, const std::vector<std:
 // and before runLidarBA (equal when it was disabled); eigen_in_force: the eigen-ratio array the last set_eigen_ratio_array call
 // left behind (stage 2's after runLidarBA, bavoxel.hpp:17 otherwise).  opts: the visual LM's options (null: the defaults).
 // problem_path: when not empty, the problem of the solve and its result go there (write_visual_problem).
+// reproj_filter_px > 0: solve_visual_remove_outliers(reproj_filter_px, min_track_len) instead of solve_visual; the landmarks it
+// drops are treated as landmarks without a plane (neither written back nor listed as kept).
 inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls, const std::vector<Pose>& x_buf_opt,
                          const std::vector<Pose>& x_buf_before, const std::vector<double>& images_ids, const std::vector<Pose>& image_poses,
                          const KeypointImages& all_keypoints, const MatchTable& all_matches, const float eigen_in_force[4],
                          VisualResult& res, std::string* err = nullptr, const lvba_visual_opts* opts = nullptr,
-                         const std::string& problem_path = std::string()) {
+                         const std::string& problem_path = std::string(), double reproj_filter_px = 0.0, int32_t min_track_len = 3) {
   const int M = (int)images_ids.size();
   if ((int)image_poses.size() != M) { if (err) *err = "Number of images and poses do not match"; return LVBA_ERR_INVALID_ARG; }      // :458-461
   if ((int)all_keypoints.size() != M) { if (err) *err = "all_keypoints.size() must equal #cameras"; return LVBA_ERR_INVALID_ARG; }  // :1429
@@ -613,7 +617,20 @@ inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls,
   }
   const std::vector<std::array<double, 4>> qs0 = qs;
   const std::vector<std::array<double, 3>> ts0 = ts, Xs0 = Xs;
-  rc = solve_visual(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01, opts, &res.solve);
+  std::vector<uint8_t> dropped((size_t)Npts, 0);
+  if (reproj_filter_px > 0.0) {
+    std::vector<std::vector<uint8_t>> removed;
+    rc = solve_visual_remove_outliers(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01,
+                                      opts, reproj_filter_px, min_track_len, &removed, &res.solve_first, &res.solve);
+    for (int pi = 0; rc == LVBA_OK && pi < Npts; ++pi) {
+      const auto& r = removed[(size_t)pi];
+      for (uint8_t b : r) res.obs_removed += b != 0;
+      dropped[(size_t)pi] = !r.empty() && std::all_of(r.begin(), r.end(), [](uint8_t b) { return b != 0; });
+      res.points_dropped += dropped[(size_t)pi];
+    }
+  } else {
+    rc = solve_visual(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01, opts, &res.solve);
+  }
   if (rc != LVBA_OK) { if (err) *err = std::string("visual LM: ") + lvba_last_error(); return rc; }
   if (!problem_path.empty()) {
     const double intr[8] = {cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3};
@@ -635,7 +652,7 @@ inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls,
     const auto& n = plane_n[(size_t)pi];
     const bool has_plane = std::isfinite(n[0]) && std::isfinite(n[1]) && std::isfinite(n[2]) && std::isfinite(plane_d[(size_t)pi]) &&
                            !(std::abs(n[0]) <= 1e-6 && std::abs(n[1]) <= 1e-6 && std::abs(n[2]) <= 1e-6);
-    if (!has_plane) continue;
+    if (!has_plane || dropped[(size_t)pi]) continue;
     res.tracks[(size_t)track_ids[(size_t)pi]].Xw_fused = Xs[(size_t)pi];
     res.track_used[(size_t)track_ids[(size_t)pi]] = 1;
     ++res.points_kept;

@@ -320,6 +320,50 @@ int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_va
  * device passes: their number, their observations and their ordered observation pairs (sum of K (K - 1)). */
 int lvba_visual_big_counts(lvba_visual_problem* p, int64_t* n_big, int64_t* n_big_obs, int64_t* n_big_pairs);
 
+/* ---- per-observation reprojection errors and reprojection-outlier removal: the solve, filter, solve-again loop of a Ceres
+ * bundle adjustment (COLMAP: FilterPoints3DWithLargeReprojectionError, then another BA).  The three calls run on one GPU (an
+ * active communicator is LVBA_ERR_UNSUPPORTED: a rank holds only its own landmarks).
+ *
+ * Observations are named by the caller's arrays: entry q of the [N_obs] arrays below, N_obs = obs_ptr[T] as given to
+ * lvba_visual_create, is obs_cam[q] / obs_uv[q].  No index map is needed, and removals compose.  An observation is IN THE
+ * PROBLEM while its landmark has a valid plane and has not been dropped, and it has not been removed.  For each one
+ * s_q = r0^2 + r1^2, the squared whitened reprojection norm that lvba_visual_cost sums before any loss, from the same device
+ * function.
+ *
+ * The rule, in double, at the current device state:
+ *   1. tau = (max_err_px / sigma_px)^2, once on the host (DBL_MAX should it overflow);
+ *   2. an observation in the problem is removed iff !(z > 1e-8 && s_q <= tau), z its camera-frame depth: the cut-off case,
+ *      NaN and s_q > tau are removed, s_q == tau is kept;
+ *   3. a landmark left with fewer than min_track_len observations in the problem is DROPPED: its remaining observations are
+ *      removed too, its plane term leaves the cost, and its X stays as it is, as for a landmark without a plane.
+ *
+ * After a removal the handle has the plan lvba_visual_create would make from the kept observations (dropped landmarks without
+ * a plane), with the handle's fixed_cam, cam_fixed, losses and deterministic flag: rows, landmark layout, tiles, big
+ * landmarks, tables, counts and big_counts.  A camera that loses every observation loses its row (lvba_visual_step writes
+ * zeros for it); a landmark may move from the big path to the tiles (129 -> 128 observations).  The state and the restore
+ * point of lvba_visual_reset_state do not change: removal is one-way.  The LM state is reset as lvba_visual_reset_lm with the
+ * handle's options would reset it (radius, a fresh Jacobi scale; deterministic mode's records are set up again before the call
+ * returns).  A later cam_fixed change re-plans from the kept observations.
+ * Refused with LVBA_ERR_INVALID_ARG and the handle unchanged: a NULL mask, min_track_len < 1, max_err_px not finite or not > 0,
+ * a removal that would leave no observation in the problem.  A failed re-plan restores the previous plan with deterministic
+ * mode off (or, if that fails too, leaves a handle that refuses every call but destroy and the state copies); then nothing is
+ * removed and no output is written. */
+
+/* s_q of every observation in the problem at the current state into sq_res [N_obs]: +inf where z > 1e-8 fails (the residual
+ * and the cost are 0 there), NaN for every observation not in the problem.  1/2 the sum of the finite entries plus the plane
+ * terms is lvba_visual_cost without losses, up to summation order. */
+int lvba_visual_obs_residuals(lvba_visual_problem* p, double* sq_res);
+/* Removes every observation with remove[q] != 0 (remove [N_obs]; flags on observations already out of the problem are
+ * ignored), then step 3 of the rule, then the re-plan.  n_obs_left, n_tracks_left (may be NULL): observations and landmarks
+ * left in the problem. */
+int lvba_visual_remove_observations(lvba_visual_problem* p, const uint8_t* remove, int32_t min_track_len, int64_t* n_obs_left,
+                                    int64_t* n_tracks_left);
+/* The rule above, then the re-plan of lvba_visual_remove_observations.  removed [N_obs] (may be NULL): 1 for every observation
+ * this call took out, those of dropped landmarks included; n_removed_obs, n_removed_tracks (may be NULL): their numbers and the
+ * number of dropped landmarks. */
+int lvba_visual_remove_outliers(lvba_visual_problem* p, double max_err_px, int32_t min_track_len, uint8_t* removed,
+                                int64_t* n_removed_obs, int64_t* n_removed_tracks);
+
 /* ======================================================================================
  * B3  adaptive voxel map (set-up stage) — replaces the cut_voxel / recut / tras_opt sequence in front of every
  *     LiDAR solve and the plane lookup in front of the visual solve:

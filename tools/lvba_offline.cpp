@@ -43,6 +43,13 @@
 //   --outlier-ratio R   BALM2::remove_outlier between two solves: each global stage runs damping_iter, remove_outlier(R) and
 //                damping_iter on one device handle of its voxel map (lvba_lidar_remove_outliers; the reference's rule, quirks included,
 //                include/lvba_b200.h).  R in [0, 1), checked when parsed (--check included); the window stage is unchanged.
+//   --reproj-filter PX [--min-track-len N]   the visual stage solves, removes every observation whose reprojection error is not
+//                <= PX pixels and the landmarks left with fewer than N observations (lvba_visual_remove_outliers), and solves again
+//                on one device handle (lvba_b200::solve_visual_remove_outliers).  Dropped landmarks are treated as landmarks without
+//                a plane: not written back, not in points3D.txt.  PX finite and > 0, N >= 1 (default 3, the reference's obser_thr_),
+//                both checked when parsed (--check included).
+#include <climits>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -66,6 +73,8 @@ int main(int argc, char** argv) {
   int window = 0;
   double anchor_leaf = 0.1;
   double outlier_ratio = -1.0;                                               // < 0: no outlier removal
+  double reproj_filter = 0.0;                                                // 0: one visual solve, no reprojection filter
+  int32_t min_track_len = 3;
   std::string db_path, sparse_dir, lidar_opt, visual_problem, fix_cameras, fix_scans;
   lvba_b200::offline::Config cfg;
   lvba_visual_opts visual_opts;
@@ -113,6 +122,25 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "--outlier-ratio: '%s' is not a number in [0, 1)\n", v);
         return 64;
       }
+    }
+    else if (a == "--reproj-filter") {
+      const char* v = next();
+      char* end = nullptr;
+      reproj_filter = std::strtod(v, &end);
+      if (end == v || *end != '\0' || !(std::isfinite(reproj_filter) && reproj_filter > 0.0)) {
+        std::fprintf(stderr, "--reproj-filter: '%s' is not a finite number of pixels > 0\n", v);
+        return 64;
+      }
+    }
+    else if (a == "--min-track-len") {
+      const char* v = next();
+      char* end = nullptr;
+      const long n = std::strtol(v, &end, 10);
+      if (end == v || *end != '\0' || n < 1 || n > INT32_MAX) {
+        std::fprintf(stderr, "--min-track-len: '%s' is not an integer >= 1\n", v);
+        return 64;
+      }
+      min_track_len = (int32_t)n;
     }
     else if (a == "--reproj-loss" || a == "--plane-loss") {
       const bool reproj = a == "--reproj-loss";
@@ -291,7 +319,7 @@ int main(int argc, char** argv) {
   off::VisualResult vr;
   cfg.fuse_map_order = fuse_order;
   const int vrc = off::run_visual_ba(cfg, frame_clouds, frames, frames_before, images_ids, image_poses, keypoints, matches,
-                                     lidar ? eigen[1] : default_eigen, vr, &err, &visual_opts, visual_problem);
+                                     lidar ? eigen[1] : default_eigen, vr, &err, &visual_opts, visual_problem, reproj_filter, min_track_len);
   if (vrc != LVBA_OK) { std::fprintf(stderr, "visual stage failed (%d): %s\n", vrc, err.c_str()); return vrc == LVBA_ERR_NO_DEVICE ? 2 : 1; }
   std::printf("{\"stage\": \"visual\", \"images\": %zu, \"keypoints\": %lld, \"matches\": %lld, \"depth_valid\": %lld, \"components\": %lld, \"tracks\": %lld, "
               "\"usable_tracks\": %lld, \"anchors\": %d, \"anchor_points\": %lld, \"surf_voxels\": %lld, \"points_kept\": %lld, \"iterations\": %d, "
