@@ -36,6 +36,7 @@ EXPORTS = [
     "lvba_visual_get_state", "lvba_visual_cost", "lvba_visual_step", "lvba_visual_structure",
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
     "lvba_visual_big_counts", "lvba_visual_obs_residuals", "lvba_visual_remove_observations", "lvba_visual_remove_outliers",
+    "lvba_visual_get_intrinsics", "lvba_visual_set_intrinsics", "lvba_visual_get_intrinsics_system",
     "lvba_voxel_default_opts", "lvba_voxel_map_create", "lvba_voxel_map_create_windows", "lvba_voxel_map_windows",
     "lvba_voxel_map_lidar_lm_batch", "lvba_voxel_map_summary", "lvba_voxel_map_export",
     "lvba_voxel_map_lookup", "lvba_voxel_map_lidar_create", "lvba_voxel_map_lidar_lm", "lvba_voxel_map_destroy",
@@ -63,7 +64,7 @@ class LidarOpts(C.Structure):
 
 
 class VisualOpts(C.Structure):
-    _fields_ = [("max_iter", C.c_int32), ("initial_radius", C.c_double), ("max_radius", C.c_double),
+    _fields_ = [("max_iter", C.c_int32), ("refine_intrinsics", C.c_uint32), ("initial_radius", C.c_double), ("max_radius", C.c_double),
                 ("min_radius", C.c_double), ("min_lm_diagonal", C.c_double), ("max_lm_diagonal", C.c_double),
                 ("min_relative_decrease", C.c_double), ("function_tolerance", C.c_double),
                 ("gradient_tolerance", C.c_double), ("parameter_tolerance", C.c_double),
@@ -73,6 +74,9 @@ class VisualOpts(C.Structure):
                 ("plane_loss", C.c_int32), ("plane_loss_scale", C.c_double),
                 ("cam_fixed", C.POINTER(C.c_uint8))]
 
+
+# lvba_visual_opts::refine_intrinsics: bit i frees intr[i] of (fx fy cx cy k1 k2 p1 p2)
+INTR_FOCAL, INTR_PRINCIPAL, INTR_DISTORTION = 0x03, 0x0C, 0xF0
 
 # lvba_loss_kind: the robust loss of the reprojection / plane residual blocks (VisualOpts.reproj_loss / plane_loss)
 LOSS_NONE, LOSS_HUBER, LOSS_CAUCHY = 0, 1, 2
@@ -483,15 +487,40 @@ class VisualProblem:
         _chk(self._lib.lvba_visual_get_system(self._h, _p(rhs, C.c_double), _p(blocks, C.c_double)))
         return cam, rhs, br, bc, blocks
 
-    def reset_lm(self, opts=None, cam_fixed=None):
+    def reset_lm(self, opts=None, cam_fixed=None, refine_intrinsics=None):
         """lvba_visual_reset_lm; cam_fixed: boolean mask [M] of further constant cameras (a mask that differs from the
-        handle's re-plans it), or None for what opts.cam_fixed says."""
+        handle's re-plans it), or None for what opts.cam_fixed says; refine_intrinsics: the mask of free intrinsics
+        (INTR_* bits), or None for what opts.refine_intrinsics says."""
         opts, mask = _with_cam_fixed(opts, cam_fixed, self.M)
+        if refine_intrinsics is not None:
+            opts = visual_default_opts() if opts is None else VisualOpts.from_buffer_copy(opts)
+            opts.refine_intrinsics = int(refine_intrinsics)
         _chk(self._lib.lvba_visual_reset_lm(self._h, C.byref(opts) if opts is not None else None))
         del mask
 
     def reset_state(self):
         _chk(self._lib.lvba_visual_reset_state(self._h))
+
+    def get_intrinsics(self):
+        """The handle's current (fx fy cx cy k1 k2 p1 p2) (lvba_visual_get_intrinsics)."""
+        out = np.empty(8); _chk(self._lib.lvba_visual_get_intrinsics(self._h, _p(out, C.c_double))); return out
+
+    def set_intrinsics(self, intr):
+        it = _f64(intr)
+        if it.shape != (8,):
+            raise ValueError(f"intr has shape {it.shape}, expected (8,)")
+        _chk(self._lib.lvba_visual_set_intrinsics(self._h, _p(it, C.c_double)))
+
+    def intrinsics_system(self):
+        """The intrinsics block of the last step (lvba_visual_get_intrinsics_system): dict(border [n_active*6, k],
+        corner [k, k], rhs [k], step [8])."""
+        k = C.c_int32()
+        _chk(self._lib.lvba_visual_get_intrinsics_system(self._h, C.byref(k), None, None, None, None))
+        n6 = 6 * len(self.structure()[0])
+        B = np.zeros((n6, k.value)); Cc = np.zeros((k.value, k.value)); r = np.zeros(k.value); st = np.zeros(8)
+        _chk(self._lib.lvba_visual_get_intrinsics_system(self._h, C.byref(k), _p(B, C.c_double), _p(Cc, C.c_double),
+                                                         _p(r, C.c_double), _p(st, C.c_double)))
+        return dict(border=B, corner=Cc, rhs=r, step=st)
 
     def iterate(self, n):
         s = Summary(); _chk(self._lib.lvba_visual_iterate(self._h, C.c_int32(n), C.byref(s))); return s.as_dict()

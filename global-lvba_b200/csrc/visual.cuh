@@ -30,6 +30,7 @@
 #include "common.cuh"
 #include "envelope.cuh"
 #include "lidar.cuh"   // kSlots, kStageStride, reduce kernels
+#include "visual_intr.h"
 #include "visual_math.h"   // VisualView, obs_eval, plane_eval, sym3_inverse
 #include "visual_tiles.h"
 
@@ -543,6 +544,63 @@ __global__ void visual_cam_update_kernel(int n_rows, const int* __restrict__ cam
   const double ts = block_sum<128>(step2, red);
   const double tx = block_sum<128>(x2, red);
   if (threadIdx.x == 0) { out[2 * blockIdx.x] = ts; out[2 * blockIdx.x + 1] = tx; }
+}
+
+// The corner of the bordered system of the intrinsics block (visual_intr.h), one CTA.  Bk, Yk: [8][n6], column i the border
+// B[:, i] and Yk[:, i] = A^-1 B[:, i], A the damped camera system; y = A^-1 r_c.  For the free entries f (bits of mask):
+//   Sigma = C + D_k - B_f^T Y_f,  D_k = clamp(colsq, min_d, max_d) / radius,  r = rhs_k - B_f^T y,
+// Cholesky, y_k = Sigma^-1 r, then y <- y - Y_f y_k (the camera step).  dev[0..7] = y_k, dev[8..15] = sk o y_k (zeros in the held
+// entries); scal[9] = the unscaled intrinsics gradient max-norm, scal[10] = 1 on a pivot that is not finite and > 0 (y_k = 0),
+// else 0.  Every sum runs in a fixed order.
+__global__ void __launch_bounds__(256) visual_intr_corner_kernel(int64_t n6, const double* __restrict__ Bk, const double* __restrict__ Yk,
+                                                                 double* __restrict__ y, const double* __restrict__ sys,
+                                                                 const double* __restrict__ sk, unsigned mask, double min_d,
+                                                                 double max_d, double radius, double* __restrict__ dev,
+                                                                 double* __restrict__ scal) {
+  __shared__ double red[32];
+  __shared__ double sBY[36 + 8];        // B_f^T Y_f (upper triangle over the free entries), then B_f^T y
+  __shared__ double syk[8];
+  int fi[8], k = 0;
+  for (int i = 0; i < 8; ++i)
+    if ((mask >> i) & 1u) fi[k++] = i;
+  const int np = k * (k + 1) / 2;
+  for (int p = 0, a = 0, b = 0; p < np + k; ++p) {
+    const double* u;
+    const double* v;
+    if (p < np) { u = Bk + fi[a] * n6; v = Yk + fi[b] * n6; if (++b == k) { ++a; b = a; } }
+    else { u = Bk + fi[p - np] * n6; v = y; }
+    double s = 0.0;
+    for (int64_t m = threadIdx.x; m < n6; m += 256) s += u[m] * v[m];
+    const double tot = block_sum<256>(s, red);
+    if (threadIdx.x == 0) sBY[p] = tot;
+  }
+  if (threadIdx.x == 0) {
+    double S[64], r[8];
+    for (int a = 0; a < k; ++a) {
+      for (int b = 0; b < k; ++b) {
+        const int lo = a < b ? a : b, hi = a < b ? b : a;
+        S[a * k + b] = sys[vintr::kC + vintr::ut(fi[lo], fi[hi])] - sBY[lo * k - lo * (lo - 1) / 2 + (hi - lo)];
+      }
+      S[a * k + a] += fmin(fmax(sys[vintr::kCol + fi[a]], min_d), max_d) / radius;
+      r[a] = sys[vintr::kRhs + fi[a]] - sBY[np + a];
+    }
+    const bool ok = vintr::corner_solve(k, S, r);
+    double gm = 0.0;
+    for (int i = 0; i < 8; ++i) syk[i] = 0.0;
+    for (int a = 0; a < k; ++a) {
+      if (ok) syk[fi[a]] = r[a];
+      gm = fmax(gm, fabs(sys[vintr::kGrad + fi[a]] / sk[fi[a]]));
+    }
+    for (int i = 0; i < 8; ++i) { dev[i] = syk[i]; dev[8 + i] = sk[i] * syk[i]; }
+    scal[9] = gm;
+    scal[10] = ok ? 0.0 : 1.0;
+  }
+  __syncthreads();
+  for (int64_t m = threadIdx.x; m < n6; m += 256) {
+    double v = y[m];
+    for (int a = 0; a < k; ++a) v -= Yk[fi[a] * n6 + m] * syk[fi[a]];
+    y[m] = v;
+  }
 }
 
 // dadd = clamp(colsq, min, max) / radius  (camera LM diagonal) ; also camera gradient max-norm (unscaled)

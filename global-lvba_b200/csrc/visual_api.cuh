@@ -63,6 +63,17 @@ struct lvba_visual_problem {
   int loss_px = LVBA_LOSS_NONE, loss_pl = LVBA_LOSS_NONE;
   double loss_a_px = 1.0, loss_a_pl = 0.1;
   bool robust() const { return loss_px != LVBA_LOSS_NONE || loss_pl != LVBA_LOSS_NONE; }
+  // ---- the intrinsics block (lvba_visual_opts::refine_intrinsics, set by lvba_visual_reset_lm; visual_intr.h).  The kernels take
+  // the intrinsics by value in VisualView, so the handle keeps them on the host: intr above is the current value, intr_c the
+  // candidate of the last pass (intr + intr_step), intr0 the value given at create.  The row CSR of the border gather
+  // (intr_row_ptr / intr_row_obs, the observations of every camera row in ascending order) follows the plan: visual_plan clears
+  // intr_ready and the next pass with the block builds it again.
+  uint32_t intr_mask = 0;
+  double intr0[8], intr_c[8], intr_step[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  bool intr_ready = false;
+  bool intr_have_sys = false;                       // intr_B / intr_sys / intr_step hold the block of the last pass since the last reset
+  lvba::DevBuf<int64_t> intr_row_ptr, intr_row_obs;
+  lvba::DevBuf<double> intr_slot, intr_rec, intr_part, intr_sys, intr_B, intr_Y, intr_dev;   // intr_dev: sk | colsq | y_k | dk
   lvba::PhaseTimers timers;
   double* h_scal = nullptr;
   int64_t launches = 0, h2d = 0, d2h = 0;
@@ -160,6 +171,8 @@ inline int visual_plan(lvba_visual_problem* P, const std::vector<int64_t>& valid
                        const std::vector<int>& row_of_cam, const int* src_id, const GetSrc& get_src, SetupLaps& lap) {
   cudaStream_t s = P->stream;
   P->n_rows = (int)P->cam_of_row.size();
+  P->intr_ready = false;
+  P->intr_have_sys = false;
   const int64_t Tv_all = (int64_t)valid.size();
   DevBuf<int> d_row_of_cam, d_src_trk;
 
@@ -288,7 +301,7 @@ inline int visual_create_impl(int32_t M, int64_t T, const double* q, const doubl
   std::unique_ptr<lvba_visual_problem> P(new lvba_visual_problem());
   P->M = M; P->T = T; P->fixed_cam = fixed_cam;
   P->cam_fixed = visual_mask(M, cam_fixed);
-  for (int i = 0; i < 8; ++i) P->intr[i] = intr[i];
+  for (int i = 0; i < 8; ++i) P->intr[i] = P->intr0[i] = P->intr_c[i] = intr[i];
   P->sigma_px = sigma_px; P->sigma_pl = sigma_plane;
   P->h_obs_ptr.assign(obs_ptr, obs_ptr + T + 1);
   LVBA_CUDA(cudaGetDevice(&P->device));
@@ -486,10 +499,20 @@ inline int visual_check_mask(bool has_mask) {
   return LVBA_OK;
 }
 
+// no intrinsics system or step until the next pass (a reset or a new mask): lvba_visual_get_intrinsics_system returns nothing older
+inline void visual_intr_forget(lvba_visual_problem* P) {
+  P->intr_have_sys = false;
+  for (int i = 0; i < 8; ++i) P->intr_step[i] = 0.0;
+}
+
 // the LM mode of the handle (lvba_visual_reset_lm and the one-shot call): the constant cameras, deterministic mode and the
 // robust losses
 inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   LVBA_TRY(visual_check_loss(o));
+  if (o.refine_intrinsics >> 8)
+    return fail(LVBA_ERR_INVALID_ARG, "refine_intrinsics = 0x%x: only bits 0..7 name intrinsics", (unsigned)o.refine_intrinsics);
+  if (o.refine_intrinsics && comm().active())
+    return fail(LVBA_ERR_UNSUPPORTED, "refine_intrinsics runs on one GPU: not with an active communicator");
   if (o.deterministic && comm().active())
     return fail(LVBA_ERR_UNSUPPORTED, "deterministic mode runs on one GPU: the multi-GPU sums of NCCL have no fixed order");
   std::vector<uint8_t> mask = visual_mask(P->M, o.cam_fixed);
@@ -510,7 +533,52 @@ inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   P->solver.set_deterministic(P->det);
   P->loss_px = o.reproj_loss; P->loss_a_px = o.reproj_loss_scale;
   P->loss_pl = o.plane_loss; P->loss_a_pl = o.plane_loss_scale;
+  P->intr_mask = o.refine_intrinsics;
+  visual_intr_forget(P);
   return LVBA_OK;
+}
+
+// ---------------------------------------------------------------- the intrinsics block (visual_intr.h)
+// The row CSR of the border gather and the block's buffers, for the current plan
+inline int visual_intr_setup(lvba_visual_problem* P) {
+  if (P->intr_ready) return LVBA_OK;
+  cudaStream_t s = P->stream;
+  std::vector<int> row((size_t)P->nnz);
+  if (P->nnz > 0) {
+    LVBA_CUDA(cudaMemcpyAsync(row.data(), P->obs_row.p, row.size() * sizeof(int), cudaMemcpyDeviceToHost, s));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    P->d2h += P->nnz * (int64_t)sizeof(int);
+  }
+  std::vector<int64_t> ptr((size_t)P->n_rows + 1, 0), obs;
+  for (int r : row)
+    if (r >= 0) ++ptr[(size_t)r + 1];
+  for (int r = 0; r < P->n_rows; ++r) ptr[(size_t)r + 1] += ptr[(size_t)r];
+  obs.resize((size_t)ptr[(size_t)P->n_rows]);
+  {
+    std::vector<int64_t> at(ptr.begin(), ptr.end() - 1);
+    for (int64_t w = 0; w < P->nnz; ++w)
+      if (row[(size_t)w] >= 0) obs[(size_t)at[(size_t)row[(size_t)w]]++] = w;
+  }
+  LVBA_TRY(P->intr_row_ptr.upload(ptr, s, &P->h2d));
+  LVBA_TRY(P->intr_row_obs.alloc(std::max<size_t>(obs.size(), 1)));
+  if (!obs.empty()) LVBA_TRY(P->intr_row_obs.upload(obs, s, &P->h2d));
+  const size_t Tv = (size_t)std::max<int64_t>(P->Tv, 1), n6 = (size_t)std::max(P->n_rows, 1) * 6;
+  LVBA_TRY(P->intr_slot.alloc(Tv * vintr::kSys));
+  LVBA_TRY(P->intr_rec.alloc((size_t)std::max<int64_t>(P->nnz, 1) * vintr::kRec));
+  LVBA_TRY(P->intr_part.alloc(((Tv + 255) / 256) * vintr::kSys));
+  LVBA_TRY(P->intr_sys.alloc(vintr::kSys));
+  LVBA_TRY(P->intr_B.alloc(8 * n6)); LVBA_TRY(P->intr_Y.alloc(8 * n6));
+  if (P->intr_dev.n == 0) { LVBA_TRY(P->intr_dev.alloc(32)); LVBA_TRY(P->intr_dev.zero(s)); }
+  LVBA_CUDA(cudaStreamSynchronize(s));                         // the host vectors are idle before they go out of scope
+  P->intr_ready = true;
+  return LVBA_OK;
+}
+
+// out[j] = sum_r in[r][j] (j < W, r < n), in row order: chunks of 256 rows, then the chunks
+inline int visual_intr_reduce(lvba_visual_problem* P, CudaExec& ex, const double* in, int64_t n, int W, double* out) {
+  const int64_t nch = std::max<int64_t>((n + 255) / 256, 1);
+  LVBA_TRY(ex.for_each(nch * W, vintr::ReduceF{in, n, 256, W, P->intr_part.p}));
+  return ex.for_each(W, vintr::ReduceF{P->intr_part.p, nch, nch, W, out});
 }
 
 // Jacobi scaling vectors from the Jacobian at the current state (Ceres: once, at iteration 0)
@@ -542,6 +610,15 @@ inline int visual_compute_scale_t(lvba_visual_problem* P, int enabled) {
   const long long nc = (long long)P->n_rows * 6, np = (long long)P->Tv * 3;
   if (nc > 0) { visual_scale_kernel<<<(unsigned)((nc + 255) / 256), 256, 0, s>>>(nc, P->cam_colsq.p, enabled, P->s_cam.p); ++P->launches; }
   if (np > 0) { visual_scale_kernel<<<(unsigned)((np + 255) / 256), 256, 0, s>>>(np, P->pt_colsq.p, enabled, P->s_pt.p); ++P->launches; }
+  if (P->intr_mask) {                                          // the block's scale: sk in intr_dev[0..7], its column norms in [8..15]
+    LVBA_TRY(visual_intr_setup(P));
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(ex.for_each(P->Tv, vintr::ColF<kLoss>{P->view(), P->state(), P->intr_slot.p}));
+    LVBA_TRY(visual_intr_reduce(P, ex, P->intr_slot.p, P->Tv, 8, P->intr_dev.p + 8));
+    LVBA_TRY(ex.for_each(8, vintr::ScaleF{P->intr_dev.p + 8, P->intr_mask, enabled, P->intr_dev.p}));
+    P->launches += ex.launches;
+  }
   LVBA_CUDA(cudaGetLastError());
   P->lm.have_scale = true;
   return LVBA_OK;
@@ -550,16 +627,19 @@ inline int visual_compute_scale(lvba_visual_problem* P, int enabled) {
   return P->robust() ? visual_compute_scale_t<true>(P, enabled) : visual_compute_scale_t<false>(P, enabled);
 }
 
-// 1/2 sum r^2 (with a loss: 1/2 sum rho) at the state `st` into *out (device): batches, big landmarks, reduction
+// 1/2 sum r^2 (with a loss: 1/2 sum rho) at the state `st` into *out (device): batches, big landmarks, reduction.  intr: the
+// intrinsics to evaluate with (null: the handle's current ones)
 template <bool kLoss>
-inline void visual_cost_t(lvba_visual_problem* P, const VisualState& st, double* out) {
+inline void visual_cost_t(lvba_visual_problem* P, const VisualState& st, double* out, const double* intr = nullptr) {
   cudaStream_t s = P->stream;
+  VisualView vv = P->view();
+  if (intr) for (int i = 0; i < 8; ++i) vv.intr[i] = intr[i];
   if (P->n_batches > 0) {
-    if constexpr (kLoss) visual_cost_loss_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), st, P->batch_cost.p);
-    else visual_cost_kernel<<<P->n_batches, kSlots, 0, s>>>(P->view(), st, P->batch_cost.p);
+    if constexpr (kLoss) visual_cost_loss_kernel<<<P->n_batches, kSlots, 0, s>>>(vv, st, P->batch_cost.p);
+    else visual_cost_kernel<<<P->n_batches, kSlots, 0, s>>>(vv, st, P->batch_cost.p);
     ++P->launches;
   }
-  if (P->n_big > 0) wide_pass(s, P->n_big, vbig::CostPass<kLoss>{P->view(), P->big_view(), st, P->batch_cost.p + P->n_batches}, &P->launches);
+  if (P->n_big > 0) wide_pass(s, P->n_big, vbig::CostPass<kLoss>{vv, P->big_view(), st, P->batch_cost.p + P->n_batches}, &P->launches);
   reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_batches + P->n_big), out);
   ++P->launches;
 }
@@ -626,6 +706,17 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
     LVBA_TRY(cm.allreduce_sum(P->cam_grad.p, (size_t)P->n_rows * 6, s));
     LVBA_TRY(cm.allreduce_sum(P->scal.p + 0, 1, s));
   }
+  const bool intr = P->intr_mask != 0;
+  const int64_t n6 = (int64_t)P->n_rows * 6;
+  if (intr) {                                                  // the border, the corner and rhs_k of the intrinsics block
+    LVBA_TRY(visual_intr_setup(P));
+    CudaExec ex;
+    ex.stream = s;
+    LVBA_TRY(ex.for_each(P->Tv, vintr::TrackF<kLoss>{P->view(), P->state(), lm, P->intr_dev.p, P->intr_slot.p, P->intr_rec.p}));
+    LVBA_TRY(visual_intr_reduce(P, ex, P->intr_slot.p, P->Tv, vintr::kSys, P->intr_sys.p));
+    LVBA_TRY(ex.for_each(P->n_rows * (int64_t)vintr::kRec, vintr::RowGatherF{P->intr_row_ptr.p, P->intr_row_obs.p, P->intr_rec.p, n6, P->intr_B.p}));
+    P->launches += ex.launches;
+  }
   P->timers.end();
   ++P->lm.builds;
   P->timers.begin(PH_SOLVE);
@@ -633,22 +724,52 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
     visual_cam_diag_kernel<<<1, 256, 0, s>>>(6 * P->n_rows, P->cam_colsq.p, P->cam_grad.p, P->s_cam.p, P->opts.min_lm_diagonal,
                                              P->opts.max_lm_diagonal, radius, P->dadd.p, P->scal.p + 5);
     ++P->launches;
+    if (intr)                                                  // Y[:, i] = A^-1 B[:, i] for every free entry, through solver.z and y
+      for (int i = 0; i < 8; ++i) {
+        if (!((P->intr_mask >> i) & 1u)) continue;
+        LVBA_CUDA(cudaMemcpyAsync(P->solver.z.p, P->intr_B.p + i * n6, (size_t)n6 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+        LVBA_TRY(P->solver.solve(P->env, P->S.p, P->dadd.p, P->y.p, s, &P->launches));
+        LVBA_CUDA(cudaMemcpyAsync(P->intr_Y.p + i * n6, P->y.p, (size_t)n6 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+      }
     LVBA_CUDA(cudaMemcpyAsync(P->solver.z.p, P->rhs.p, (size_t)P->n_rows * 6 * sizeof(double), cudaMemcpyDeviceToDevice, s));
     LVBA_TRY(P->solver.solve(P->env, P->S.p, P->dadd.p, P->y.p, s, &P->launches));
   }
+  double yk[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (intr) {                                                  // the corner, y_k and the camera step y - Y y_k
+    visual_intr_corner_kernel<<<1, 256, 0, s>>>(n6, P->intr_B.p, P->intr_Y.p, P->y.p, P->intr_sys.p, P->intr_dev.p, P->intr_mask,
+                                                P->opts.min_lm_diagonal, P->opts.max_lm_diagonal, radius, P->intr_dev.p + 16, P->scal.p);
+    ++P->launches;
+    // the candidate intrinsics go into the cost kernels' VisualView by value: the step comes to the host here
+    double h[16];
+    LVBA_CUDA(cudaMemcpyAsync(h, P->intr_dev.p + 16, sizeof(h), cudaMemcpyDeviceToHost, s));
+    LVBA_CUDA(cudaStreamSynchronize(s));
+    P->d2h += sizeof(h);
+    for (int i = 0; i < 8; ++i) { yk[i] = h[i]; P->intr_step[i] = h[8 + i]; P->intr_c[i] = P->intr[i] + h[8 + i]; }
+    P->intr_have_sys = true;
+  }
   P->timers.end();
   P->timers.begin(PH_RESID);
-  if (P->n_batches > 0) {
+  if (intr) {
+    CudaExec ex;
+    ex.stream = s;
+    vintr::BacksubF<kLoss> f{P->view(), P->state(), lm, P->intr_dev.p, P->y.p, {}, P->Xc.p, want_steps ? P->pt_step.p : nullptr, P->intr_slot.p};
+    for (int i = 0; i < 8; ++i) f.yk[i] = yk[i];
+    LVBA_TRY(ex.for_each(P->Tv, f));
+    LVBA_TRY(visual_intr_reduce(P, ex, P->intr_slot.p, P->Tv, 3, P->scal.p + 2));
+    P->launches += ex.launches;
+  } else if (P->n_batches > 0) {
     visual_backsub_kernel<kLoss><<<P->n_batches, kSlots, visual_backsub_smem_bytes(), s>>>(
         P->view(), P->state(), lm, P->y.p, P->Xc.p, want_steps ? P->pt_step.p : nullptr, P->batch_out.p);
     ++P->launches;
   }
-  if (P->n_big > 0)
-    wide_pass(s, P->n_big, vbig::BacksubPass<kLoss>{P->view(), P->big_view(), P->state(), lm, P->big_obs.p, P->big_params.p, P->y.p,
-                                                    P->Xc.p, want_steps ? P->pt_step.p : nullptr,
-                                                    P->batch_out.p + 4 * (int64_t)P->n_batches}, &P->launches);
-  reduce_cols_kernel<<<1, 256, 0, s>>>(P->batch_out.p, (int)(P->n_batches + P->n_big), 4, 3, P->scal.p + 2);
-  ++P->launches;
+  if (!intr) {
+    if (P->n_big > 0)
+      wide_pass(s, P->n_big, vbig::BacksubPass<kLoss>{P->view(), P->big_view(), P->state(), lm, P->big_obs.p, P->big_params.p, P->y.p,
+                                                      P->Xc.p, want_steps ? P->pt_step.p : nullptr,
+                                                      P->batch_out.p + 4 * (int64_t)P->n_batches}, &P->launches);
+    reduce_cols_kernel<<<1, 256, 0, s>>>(P->batch_out.p, (int)(P->n_batches + P->n_big), 4, 3, P->scal.p + 2);
+    ++P->launches;
+  }
   const int ncb = (P->n_rows + 127) / 128;
   if (ncb > 0) {
     visual_cam_update_kernel<<<ncb, 128, 0, s>>>(P->n_rows, P->d_cam_of_row.p, P->q.p, P->t.p, P->y.p, P->s_cam.p, P->qc.p, P->tc.p,
@@ -658,7 +779,7 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   reduce_cols_kernel<<<1, 256, 0, s>>>(P->cam_out.p, ncb, 2, 2, P->scal.p + 6);
   ++P->launches;
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 2, 3, s));   // model, step^2, x^2 of the landmark shard
-  visual_cost_t<kLoss>(P, P->cand(), P->scal.p + 8);                      // candidate cost
+  visual_cost_t<kLoss>(P, P->cand(), P->scal.p + 8, intr ? P->intr_c : nullptr);   // candidate cost
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 8, 1, s));
   P->timers.end();
   LVBA_CUDA(cudaGetLastError());
@@ -667,6 +788,12 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   LVBA_CUDA(cudaStreamSynchronize(s));
   if (P->n_rows == 0) *reinterpret_cast<int*>(P->h_scal + 15) = 0;   // every camera constant: nothing was factorised
   P->d2h += 16 * sizeof(double);
+  if (intr) {        // the block in the gradient max-norm, the status and the norms (Ceres: ||x|| over all 8 entries of the block)
+    double* h = P->h_scal;
+    h[1] = std::max(h[1], h[9]);
+    if (h[10] != 0.0) *reinterpret_cast<int*>(h + 15) |= 1;
+    for (int i = 0; i < 8; ++i) { h[3] += P->intr_step[i] * P->intr_step[i]; h[4] += P->intr[i] * P->intr[i]; }
+  }
   return LVBA_OK;
 }
 inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool want_steps) {
@@ -711,6 +838,7 @@ inline int visual_iterate_impl(lvba_visual_problem* P, int n_iter, lvba_summary*
     }
     if (std::isfinite(cand) && rho > o.min_relative_decrease) {             // StepAccepted
       std::swap(P->q.p, P->qc.p); std::swap(P->t.p, P->tc.p); std::swap(P->X.p, P->Xc.p);
+      if (P->intr_mask) std::copy(P->intr_c, P->intr_c + 8, P->intr);
       // keep untouched entries (constant cameras, skipped landmarks) identical in both buffers: they never change
       lm.cost = cand;
       ++lm.accepted;
@@ -854,6 +982,7 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
   o->reproj_loss = LVBA_LOSS_NONE; o->reproj_loss_scale = 1.0;
   o->plane_loss = LVBA_LOSS_NONE; o->plane_loss_scale = 0.1;
   o->cam_fixed = nullptr;
+  o->refine_intrinsics = 0;
 }
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
@@ -980,6 +1109,9 @@ int lvba_visual_reset_state(lvba_visual_problem* p) LVBA_ABI_BEGIN {
   LVBA_CUDA(cudaMemcpyAsync(p->q.p, p->q0.p, nq, cudaMemcpyDeviceToDevice, s)); LVBA_CUDA(cudaMemcpyAsync(p->qc.p, p->q0.p, nq, cudaMemcpyDeviceToDevice, s));
   LVBA_CUDA(cudaMemcpyAsync(p->t.p, p->t0.p, nt, cudaMemcpyDeviceToDevice, s)); LVBA_CUDA(cudaMemcpyAsync(p->tc.p, p->t0.p, nt, cudaMemcpyDeviceToDevice, s));
   if (nx) { LVBA_CUDA(cudaMemcpyAsync(p->X.p, p->X0.p, nx, cudaMemcpyDeviceToDevice, s)); LVBA_CUDA(cudaMemcpyAsync(p->Xc.p, p->X0.p, nx, cudaMemcpyDeviceToDevice, s)); }
+  std::copy(p->intr0, p->intr0 + 8, p->intr);
+  std::copy(p->intr0, p->intr0 + 8, p->intr_c);
+  lvba::visual_intr_forget(p);
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_reset_state")
 
@@ -1016,6 +1148,8 @@ int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const 
   lvba_visual_opts o;
   if (opts) o = *opts; else lvba_visual_default_opts(&o);
   LVBA_TRY(lvba::visual_check_loss(o));                       // before any device work: the buffers stay untouched
+  if (o.refine_intrinsics)
+    return lvba::fail(LVBA_ERR_INVALID_ARG, "refine_intrinsics needs a handle (lvba_visual_reset_lm): the one-shot call's intr is const");
   LVBA_TRY(lvba::visual_check_mask(M > 0 && !lvba::visual_mask(M, o.cam_fixed).empty()));
   lvba_visual_problem* p = nullptr;
   // planned once, with the constant cameras: the reset below finds the handle's mask equal to the options'
@@ -1067,5 +1201,47 @@ int lvba_visual_remove_outliers(lvba_visual_problem* p, double max_err_px, int32
   LVBA_TRY(lvba::visual_obs_sq_dev(p));
   return lvba::visual_remove_impl(p, nullptr, tau, min_track_len, removed, nullptr, nullptr, n_removed_obs, n_removed_tracks);
 } LVBA_ABI_END("lvba_visual_remove_outliers")
+
+int lvba_visual_get_intrinsics(lvba_visual_problem* p, double intr[8]) LVBA_ABI_BEGIN {
+  if (!p || !intr) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  std::copy(p->intr, p->intr + 8, intr);
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_get_intrinsics")
+
+int lvba_visual_set_intrinsics(lvba_visual_problem* p, const double intr[8]) LVBA_ABI_BEGIN {
+  if (!p || !intr) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  for (int i = 0; i < 8; ++i)
+    if (!std::isfinite(intr[i])) return lvba::fail(LVBA_ERR_INVALID_ARG, "intr[%d] = %g is not finite", i, intr[i]);
+  std::copy(intr, intr + 8, p->intr);
+  std::copy(intr, intr + 8, p->intr_c);
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_set_intrinsics")
+
+int lvba_visual_get_intrinsics_system(lvba_visual_problem* p, int32_t* k, double* border, double* corner, double* rhs,
+                                      double* step) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
+  int fi[8], nk = 0;
+  for (int i = 0; i < 8; ++i)
+    if ((p->intr_mask >> i) & 1u) fi[nk++] = i;
+  if (k) *k = nk;
+  if (step) std::copy(p->intr_step, p->intr_step + 8, step);
+  if (nk == 0 || !p->intr_have_sys || !(border || corner || rhs)) return LVBA_OK;
+  LVBA_CUDA(cudaSetDevice(p->device));
+  const size_t n6 = (size_t)p->n_rows * 6;
+  std::vector<double> B(8 * n6), sys(lvba::vintr::kSys);
+  if (n6) LVBA_CUDA(cudaMemcpyAsync(B.data(), p->intr_B.p, B.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  LVBA_CUDA(cudaMemcpyAsync(sys.data(), p->intr_sys.p, sys.size() * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
+  LVBA_CUDA(cudaStreamSynchronize(p->stream));
+  if (border)
+    for (size_t m = 0; m < n6; ++m)
+      for (int a = 0; a < nk; ++a) border[m * nk + a] = B[fi[a] * n6 + m];
+  for (int a = 0; a < nk; ++a) {
+    if (rhs) rhs[a] = sys[lvba::vintr::kRhs + fi[a]];
+    if (corner)
+      for (int b = 0; b < nk; ++b) corner[a * nk + b] = sys[lvba::vintr::kC + lvba::vintr::ut(std::min(fi[a], fi[b]), std::max(fi[a], fi[b]))];
+  }
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_get_intrinsics_system")
 
 }  // extern "C"

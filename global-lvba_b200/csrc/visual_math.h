@@ -153,6 +153,38 @@ LVBA_UNROLL
     }
 }
 
+// d r / d (fx fy cx cy k1 k2 p1 p2) of the whitened residual of obs_eval (2x8, row-major: Jk[8 rho + i]), with obs_eval's
+// projection step for step; zero where the depth test z > 1e-8 fails (utils.hpp:78).  A function of its own, as obs_depth, so
+// that the kernels that call obs_eval keep their code.
+LVBA_HD void intr_jac(const VisualView& vv, const double* __restrict__ qp, const double* __restrict__ tp, const double* X,
+                      double Jk[16]) {
+  double q0 = qp[0], q1 = qp[1], q2 = qp[2], q3 = qp[3];
+  const double inv = 1.0 / sqrt(q0 * q0 + q1 * q1 + q2 * q2 + q3 * q3);
+  q0 *= inv; q1 *= inv; q2 *= inv; q3 *= inv;
+  const double v[3] = {q1, q2, q3};
+  double vxX[3], t2[3];
+  cross3(v, X, vxX);
+  const double uvv[3] = {2.0 * vxX[0], 2.0 * vxX[1], 2.0 * vxX[2]};
+  cross3(v, uvv, t2);
+  const double Xc[3] = {X[0] + q0 * uvv[0] + t2[0] + tp[0], X[1] + q0 * uvv[1] + t2[1] + tp[1],
+                        X[2] + q0 * uvv[2] + t2[2] + tp[2]};
+  const double z = Xc[2];
+  for (int i = 0; i < 16; ++i) Jk[i] = 0.0;
+  if (!(z > 1e-8)) return;
+  const double fx = vv.intr[0], fy = vv.intr[1], k1 = vv.intr[4], k2 = vv.intr[5], p1 = vv.intr[6], p2 = vv.intr[7];
+  const double iz = 1.0 / z;
+  const double xn = Xc[0] * iz, yn = Xc[1] * iz;
+  const double r2 = xn * xn + yn * yn;
+  const double rad = 1.0 + k1 * r2 + k2 * r2 * r2;
+  const double xd = xn * rad + 2.0 * p1 * xn * yn + p2 * (r2 + 2.0 * xn * xn);
+  const double yd = yn * rad + p1 * (r2 + 2.0 * yn * yn) + 2.0 * p2 * xn * yn;
+  const double is = vv.inv_sigma_px, sx = fx * is, sy = fy * is;
+  Jk[0] = xd * is; Jk[2] = is;
+  Jk[4] = sx * xn * r2; Jk[5] = sx * xn * r2 * r2; Jk[6] = sx * 2.0 * xn * yn; Jk[7] = sx * (r2 + 2.0 * xn * xn);
+  Jk[9] = yd * is; Jk[11] = is;
+  Jk[12] = sy * yn * r2; Jk[13] = sy * yn * r2 * r2; Jk[14] = sy * (r2 + 2.0 * yn * yn); Jk[15] = sy * 2.0 * xn * yn;
+}
+
 // The camera-frame depth obs_eval tests (utils.hpp:78), with obs_eval's arithmetic step for step, so that the two agree on
 // every bit.  A function of its own rather than a part factored out of obs_eval: that keeps the code of the kernels that call
 // obs_eval as it was.

@@ -9,6 +9,7 @@
 //   lvba_b200::remove_outlier(x_stats, voxhess, r)   BALM2::remove_outlier (commented out in the reference, :650-660)
 //   lvba_b200::solve_visual(...)                     replaces the Ceres block       src/lvba_system.cpp:1571-1656
 //   lvba_b200::solve_visual_remove_outliers(...)     the same, then a reprojection filter and a second solve on one handle
+//   lvba_b200::solve_visual_refine_intrinsics(...)   solve_visual with the intrinsics a parameter block, refined and written back
 //   lvba_b200::WindowBatch                           collects the windows of runWindowBA (src/lvba_system.cpp:232-302) and
 //                                                    solves them in one lvba_lidar_lm_batch call
 //   lvba_b200::SurfMap                               replaces the surf_map built by cut_voxel + recut (+ tras_opt) in front of
@@ -622,13 +623,51 @@ inline int solve_visual(std::vector<std::array<double, 4>>& qs, std::vector<std:
                         sigma_px, sigma_plane, /*fixed_cam=*/0, opts, summary);
 }
 
+// solve_visual_refine_intrinsics: solve_visual on a device handle with the intrinsics a parameter block of every
+// ReprojErrorWhitenedDistorted, as a Ceres user gets by passing fx_ .. d3_ to the cost functor as a parameter block instead of
+// constants: the entries whose bit is set in `refine` (lvba_visual_opts::refine_intrinsics, LVBA_INTR_*) are refined, the others
+// held by a SubsetManifold.  qs, ts, Xs and fx .. p2 are written back after the solve (refine = 0: the intrinsics come back
+// unchanged, and the solve is solve_visual's).  opts->refine_intrinsics is ignored; a bad mask is LVBA_ERR_INVALID_ARG.
+inline int solve_visual_refine_intrinsics(std::vector<std::array<double, 4>>& qs, std::vector<std::array<double, 3>>& ts,
+                                          std::vector<std::array<double, 3>>& Xs, const std::vector<std::array<double, 3>>& plane_n,
+                                          const std::vector<double>& plane_d, const std::vector<std::vector<Observation>>& obs_of_point,
+                                          double& fx, double& fy, double& cx, double& cy, double& k1, double& k2, double& p1, double& p2,
+                                          uint32_t refine, double sigma_px = 0.5, double sigma_plane = 0.01,
+                                          const lvba_visual_opts* opts = nullptr, lvba_summary* summary = nullptr,
+                                          const std::vector<uint8_t>* cam_fixed = nullptr) {
+  const int M = (int)qs.size();
+  const int64_t T = (int64_t)Xs.size();
+  const VisualCsr c = pack_visual(M, ts, Xs, plane_n, plane_d, obs_of_point, cam_fixed, "solve_visual_refine_intrinsics");
+  lvba_visual_opts o;
+  opts = with_cam_fixed(opts, cam_fixed, o);
+  lvba_visual_opts use;
+  if (opts) use = *opts; else lvba_visual_default_opts(&use);
+  use.refine_intrinsics = refine;
+  double intr[8] = {fx, fy, cx, cy, k1, k2, p1, p2};
+  lvba_visual_problem* p = nullptr;
+  int rc = lvba_visual_create(M, T, qs.empty() ? nullptr : qs[0].data(), ts.empty() ? nullptr : ts[0].data(), Xs.empty() ? nullptr : Xs[0].data(),
+                              c.plane_nd.data(), c.obs_ptr.data(), c.obs_cam.data(), c.obs_uv.data(), intr, sigma_px, sigma_plane,
+                              /*fixed_cam=*/0, use.device, &p);
+  if (rc != LVBA_OK) return rc;
+  rc = lvba_visual_reset_lm(p, &use);
+  if (rc == LVBA_OK) rc = lvba_visual_iterate(p, use.max_iter, summary);
+  if (rc == LVBA_OK)
+    rc = lvba_visual_get_state(p, qs.empty() ? nullptr : qs[0].data(), ts.empty() ? nullptr : ts[0].data(), Xs.empty() ? nullptr : Xs[0].data());
+  if (rc == LVBA_OK) rc = lvba_visual_get_intrinsics(p, intr);
+  lvba_visual_destroy(p);
+  if (rc != LVBA_OK) return rc;
+  fx = intr[0]; fy = intr[1]; cx = intr[2]; cy = intr[3]; k1 = intr[4]; k2 = intr[5]; p1 = intr[6]; p2 = intr[7];
+  return LVBA_OK;
+}
+
 // solve_visual, then lvba_visual_remove_outliers(max_err_px, min_track_len), then a second solve, on one device handle: the
 // solve, filter, solve-again loop of a Ceres bundle adjustment (include/lvba_b200.h, B2, states the rule).  Each solve is
 // lvba_visual_reset_lm with opts (and cam_fixed) and up to opts->max_iter iterations; summary_first / summary_second (may be
 // null) are their summaries.  removed (may be null) gets one entry per observation of obs_of_point, in its order: 1 for every
 // observation the filter took out, those of dropped landmarks included, so that a caller can erase the same entries from its
 // tr.inlier_indices.  A landmark whose observations are all removed is dropped: its Xs entry comes back as the first solve left
-// it, and the caller treats it as a landmark without a plane.  qs, ts, Xs are written back after the second solve.
+// it, and the caller treats it as a landmark without a plane.  qs, ts, Xs are written back after the second solve, and, when
+// intr_out is not null, the handle's intrinsics (refined by both solves when opts->refine_intrinsics is set).
 inline int solve_visual_remove_outliers(std::vector<std::array<double, 4>>& qs, std::vector<std::array<double, 3>>& ts,
                                         std::vector<std::array<double, 3>>& Xs, const std::vector<std::array<double, 3>>& plane_n,
                                         const std::vector<double>& plane_d, const std::vector<std::vector<Observation>>& obs_of_point,
@@ -636,7 +675,7 @@ inline int solve_visual_remove_outliers(std::vector<std::array<double, 4>>& qs, 
                                         double sigma_px, double sigma_plane, const lvba_visual_opts* opts, double max_err_px,
                                         int32_t min_track_len, std::vector<std::vector<uint8_t>>* removed = nullptr,
                                         lvba_summary* summary_first = nullptr, lvba_summary* summary_second = nullptr,
-                                        const std::vector<uint8_t>* cam_fixed = nullptr) {
+                                        const std::vector<uint8_t>* cam_fixed = nullptr, double* intr_out = nullptr) {
   const int M = (int)qs.size();
   const int64_t T = (int64_t)Xs.size();
   const VisualCsr c = pack_visual(M, ts, Xs, plane_n, plane_d, obs_of_point, cam_fixed, "solve_visual_remove_outliers");
@@ -658,6 +697,7 @@ inline int solve_visual_remove_outliers(std::vector<std::array<double, 4>>& qs, 
   if (rc == LVBA_OK) rc = lvba_visual_iterate(p, use.max_iter, summary_second);
   if (rc == LVBA_OK)
     rc = lvba_visual_get_state(p, qs.empty() ? nullptr : qs[0].data(), ts.empty() ? nullptr : ts[0].data(), Xs.empty() ? nullptr : Xs[0].data());
+  if (rc == LVBA_OK && intr_out) rc = lvba_visual_get_intrinsics(p, intr_out);
   lvba_visual_destroy(p);
   if (rc != LVBA_OK) return rc;
   if (removed) {

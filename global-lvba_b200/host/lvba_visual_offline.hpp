@@ -446,6 +446,8 @@ struct VisualResult {
   lvba_summary solve{};                        // the solve (with a reprojection filter: the second one)
   lvba_summary solve_first{};                  // with a reprojection filter: the solve before it
   int64_t obs_removed = 0, points_dropped = 0;  // with a reprojection filter: what it took out
+  bool intr_refined = false;                   // with lvba_visual_opts::refine_intrinsics: intr holds the refined intrinsics
+  double intr[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // fx fy cx cy d0 d1 d2 d3 after the solve (those of the config without refinement)
   int64_t usable_tracks = 0, points_kept = 0, keypoints = 0, matches = 0, anchor_points = 0, depth_valid = 0;
   int anchors = 0;
 };
@@ -485,12 +487,40 @@ inline bool write_visual_problem(const std::string& path, const std::vector<std:
   return (bool)f;
 }
 
+// the intrinsics of a config as the visual problem takes them: fx fy cx cy d0 d1 d2 d3
+inline std::array<double, 8> cfg_intr(const Config& cfg) { return {cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3}; }
+
+// A set of intrinsics groups as `focal,principal,distortion` (any non-empty comma-separated subset, each once) as an
+// lvba_visual_opts::refine_intrinsics mask.  Anything else is refused with a message in *err; mask is then untouched.
+inline bool parse_intr_groups(const char* text, uint32_t& mask, std::string* err = nullptr) {
+  const std::string s = text ? text : "";
+  uint32_t m = 0;
+  size_t at = 0;
+  while (true) {
+    const size_t comma = s.find(',', at);
+    const std::string g = s.substr(at, comma == std::string::npos ? std::string::npos : comma - at);
+    uint32_t b;
+    if (g == "focal") b = LVBA_INTR_FOCAL;
+    else if (g == "principal") b = LVBA_INTR_PRINCIPAL;
+    else if (g == "distortion") b = LVBA_INTR_DISTORTION;
+    else { if (err) *err = "'" + s + "': a comma-separated list of focal, principal, distortion"; return false; }
+    if (m & b) { if (err) *err = "'" + s + "': '" + g + "' is listed twice"; return false; }
+    m |= b;
+    if (comma == std::string::npos) break;
+    at = comma + 1;
+  }
+  mask = m;
+  return true;
+}
+
 // runVisualBAWithLidarAssist (:144-154) minus the drawing / publishing calls.  x_buf_opt / x_buf_before: the LiDAR poses after
 // and before runLidarBA (equal when it was disabled); eigen_in_force: the eigen-ratio array the last set_eigen_ratio_array call
 // left behind (stage 2's after runLidarBA, bavoxel.hpp:17 otherwise).  opts: the visual LM's options (null: the defaults).
 // problem_path: when not empty, the problem of the solve and its result go there (write_visual_problem).
 // reproj_filter_px > 0: solve_visual_remove_outliers(reproj_filter_px, min_track_len) instead of solve_visual; the landmarks it
-// drops are treated as landmarks without a plane (neither written back nor listed as kept).
+// drops are treated as landmarks without a plane (neither written back nor listed as kept).  opts->refine_intrinsics != 0: the
+// solve runs on a handle with the intrinsics a parameter block (solve_visual_refine_intrinsics, or the filter's handle) and
+// res.intr gets the refined ones; otherwise res.intr is the config's.
 inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls, const std::vector<Pose>& x_buf_opt,
                          const std::vector<Pose>& x_buf_before, const std::vector<double>& images_ids, const std::vector<Pose>& image_poses,
                          const KeypointImages& all_keypoints, const MatchTable& all_matches, const float eigen_in_force[4],
@@ -618,16 +648,22 @@ inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls,
   const std::vector<std::array<double, 4>> qs0 = qs;
   const std::vector<std::array<double, 3>> ts0 = ts, Xs0 = Xs;
   std::vector<uint8_t> dropped((size_t)Npts, 0);
+  const uint32_t refine = opts ? opts->refine_intrinsics : 0u;
+  double intr[8] = {cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3};
   if (reproj_filter_px > 0.0) {
     std::vector<std::vector<uint8_t>> removed;
     rc = solve_visual_remove_outliers(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01,
-                                      opts, reproj_filter_px, min_track_len, &removed, &res.solve_first, &res.solve);
+                                      opts, reproj_filter_px, min_track_len, &removed, &res.solve_first, &res.solve, nullptr,
+                                      refine ? intr : nullptr);
     for (int pi = 0; rc == LVBA_OK && pi < Npts; ++pi) {
       const auto& r = removed[(size_t)pi];
       for (uint8_t b : r) res.obs_removed += b != 0;
       dropped[(size_t)pi] = !r.empty() && std::all_of(r.begin(), r.end(), [](uint8_t b) { return b != 0; });
       res.points_dropped += dropped[(size_t)pi];
     }
+  } else if (refine) {
+    rc = solve_visual_refine_intrinsics(qs, ts, Xs, plane_n, plane_d, obs, intr[0], intr[1], intr[2], intr[3], intr[4], intr[5], intr[6],
+                                        intr[7], refine, 0.5, 0.01, opts, &res.solve);
   } else {
     rc = solve_visual(qs, ts, Xs, plane_n, plane_d, obs, cfg.fx, cfg.fy, cfg.cx, cfg.cy, cfg.d0, cfg.d1, cfg.d2, cfg.d3, 0.5, 0.01, opts, &res.solve);
   }
@@ -639,7 +675,10 @@ inline int run_visual_ba(const Config& cfg, const std::vector<Cloud*>& pl_fulls,
       return LVBA_ERR_INVALID_ARG;
     }
   }
+  const std::array<double, 8> given = cfg_intr(cfg);
+  std::copy(given.begin(), given.end(), res.intr);
   if (res.solve.termination == LVBA_TERM_INVALID_STEPS) return LVBA_OK;                                // ceres::FAILURE, :1647-1650: nothing written back
+  if (refine) { std::copy(intr, intr + 8, res.intr); res.intr_refined = true; }
   for (int k = 0; k < M; ++k) {                                                                       // :1652-1656
     const auto& q = qs[(size_t)k];
     const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);

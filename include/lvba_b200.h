@@ -90,6 +90,19 @@ typedef enum lvba_loss_kind {
  *      (ceres-solver 2.1.0 defaults everywhere else, SURVEY.md Q10) */
 typedef struct lvba_visual_opts {
   int32_t max_iter;              /* 50      options.max_num_iterations (:1573) */
+  /* Refined intrinsics (a variable ceres::Problem parameter block of size 8 in every ReprojErrorWhitenedDistorted, held by a
+   * SubsetManifold): 0 (the default: the intr given at create stay constant, and every pass is the one without this field) or a
+   * mask whose bit i frees intr[i] of (fx fy cx cy k1 k2 p1 p2); LVBA_INTR_FOCAL, LVBA_INTR_PRINCIPAL, LVBA_INTR_DISTORTION
+   * name the groups.  One block shared by every camera.  The free entries get their Jacobi scale, LM diagonal and gradient
+   * entries; the reduced camera system gains a border that is solved with the camera system (one more solve per free entry)
+   * and a k x k corner; the parameter tolerance takes ||x|| over all 8 entries and the step over the free ones (Ceres).  As
+   * `deterministic`: a handle takes it from lvba_visual_reset_lm, and lvba_visual_step / _iterate / _cost then follow the handle's
+   * current intrinsics (lvba_visual_get_intrinsics).  The sums of the block run in a fixed order whatever `deterministic` says.
+   * Refused before any device work: bits above 7 (LVBA_ERR_INVALID_ARG), a nonzero mask with an active communicator
+   * (LVBA_ERR_UNSUPPORTED), a nonzero mask in the one-shot lvba_visual_lm, whose intr is const (LVBA_ERR_INVALID_ARG). */
+  uint32_t refine_intrinsics;     /* 0; in the padding after max_iter, so that the struct keeps its size and the offsets of
+                                  * every other field.  A caller that fills the struct field by field instead of starting from
+                                  * lvba_visual_default_opts must set it too: what the padding held before is read as a mask */
   double initial_radius;         /* 1e4  */
   double max_radius;             /* 1e16 */
   double min_radius;             /* 1e-32 */
@@ -130,6 +143,10 @@ typedef struct lvba_visual_opts {
    * NULL; any nonzero entry with an active communicator is LVBA_ERR_UNSUPPORTED.  The library keeps no copy of the pointer. */
   const uint8_t* cam_fixed;
 } lvba_visual_opts;
+
+#define LVBA_INTR_FOCAL      0x03u   /* fx fy */
+#define LVBA_INTR_PRINCIPAL  0x0Cu   /* cx cy */
+#define LVBA_INTR_DISTORTION 0xF0u   /* k1 k2 p1 p2 */
 
 typedef enum lvba_termination {
   LVBA_TERM_MAX_ITER = 0,
@@ -311,8 +328,21 @@ int lvba_visual_structure(lvba_visual_problem* p, int32_t* n_active, int32_t* ca
                           int64_t* nblocks, int32_t* brow, int32_t* bcol);
 int lvba_visual_get_system(lvba_visual_problem* p, double* rhs /* [n_active*6] */, double* blocks /* [nblocks*36] */);
 int lvba_visual_reset_lm(lvba_visual_problem* p, const lvba_visual_opts* opts);
-/* restore q, t, X passed to lvba_visual_create (device-to-device) */
+/* restore q, t, X and the intrinsics passed to lvba_visual_create (device-to-device) */
 int lvba_visual_reset_state(lvba_visual_problem* p);
+/* The handle's current intrinsics (fx fy cx cy k1 k2 p1 p2): those given at create until an accepted step of a refining
+ * solve (lvba_visual_opts::refine_intrinsics) or lvba_visual_set_intrinsics changes them.  Set refuses a non-finite entry
+ * with LVBA_ERR_INVALID_ARG and leaves the handle unchanged. */
+int lvba_visual_get_intrinsics(lvba_visual_problem* p, double intr[8]);
+int lvba_visual_set_intrinsics(lvba_visual_problem* p, const double intr[8]);
+/* The intrinsics block of the last lvba_visual_step (for parity tests, beside lvba_visual_get_system), k = the number of free
+ * entries, in ascending order of their index.  border [n_active*6*k]: B, row 6 r + a of camera row r, column j of free entry
+ * j; corner [k*k]: C = sum J_k^T J_k - sum E V^-1 E^T, without the LM diagonal (as the blocks of lvba_visual_get_system);
+ * rhs [k]: -(g_k - sum E V^-1 g_X), these three with the Jacobi scaling applied, as the camera system; step [8]: the change of
+ * the intrinsics, zeros in the held entries.  Any pointer may be NULL.  Until the first lvba_visual_step after create,
+ * lvba_visual_reset_lm, lvba_visual_reset_state or a removal, only k and step (all zeros) are written. */
+int lvba_visual_get_intrinsics_system(lvba_visual_problem* p, int32_t* k, double* border, double* corner, double* rhs,
+                                      double* step);
 int lvba_visual_iterate(lvba_visual_problem* p, int32_t n_iter, lvba_summary* summary);
 int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_valid_tracks,
                        int64_t* n_blocks_env, int64_t* n_pairs);

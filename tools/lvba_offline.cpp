@@ -48,6 +48,10 @@
 //                on one device handle (lvba_b200::solve_visual_remove_outliers).  Dropped landmarks are treated as landmarks without
 //                a plane: not written back, not in points3D.txt.  PX finite and > 0, N >= 1 (default 3, the reference's obser_thr_),
 //                both checked when parsed (--check included).
+//   --refine-intrinsics LIST   refine these intrinsics groups in the visual stage (lvba_visual_opts::refine_intrinsics), LIST a
+//                comma-separated subset of focal,principal,distortion, checked when parsed (--check included).  The stage then runs
+//                on a device handle (lvba_b200::solve_visual_refine_intrinsics), prints the refined intrinsics, and --points3d lidar
+//                projects with them.  Without the flag the output is as before.
 #include <climits>
 #include <cmath>
 #include <cstdio>
@@ -129,6 +133,13 @@ int main(int argc, char** argv) {
       reproj_filter = std::strtod(v, &end);
       if (end == v || *end != '\0' || !(std::isfinite(reproj_filter) && reproj_filter > 0.0)) {
         std::fprintf(stderr, "--reproj-filter: '%s' is not a finite number of pixels > 0\n", v);
+        return 64;
+      }
+    }
+    else if (a == "--refine-intrinsics") {
+      std::string e;
+      if (!lvba_b200::offline::parse_intr_groups(next(), visual_opts.refine_intrinsics, &e)) {
+        std::fprintf(stderr, "--refine-intrinsics: %s\n", e.c_str());
         return 64;
       }
     }
@@ -327,12 +338,18 @@ int main(int argc, char** argv) {
               images_ids.size(), (long long)vr.keypoints, (long long)vr.matches, (long long)vr.depth_valid, (long long)vr.fuse.n_components,
               (long long)vr.fuse.n_tracks, (long long)vr.usable_tracks, vr.anchors, (long long)vr.anchor_points, (long long)vr.surf.n_voxels,
               (long long)vr.points_kept, vr.solve.iterations, vr.solve.cost_first, vr.solve.cost_last, vr.solve.termination, vr.solve.ms_total);
+  if (vr.intr_refined)
+    std::printf("{\"stage\": \"intrinsics\", \"fx\": %.12g, \"fy\": %.12g, \"cx\": %.12g, \"cy\": %.12g, \"d0\": %.12g, \"d1\": %.12g, "
+                "\"d2\": %.12g, \"d3\": %.12g}\n", vr.intr[0], vr.intr[1], vr.intr[2], vr.intr[3], vr.intr[4], vr.intr[5], vr.intr[6], vr.intr[7]);
   if (sparse_dir.empty()) sparse_dir = data + "Colmap/sparse/";
   if (sparse_dir.back() != '/') sparse_dir += '/';
   std::error_code ec;
   std::filesystem::create_directories(sparse_dir, ec);
   std::vector<off::LidarPoint3D> lp; std::vector<uint8_t> listed;
-  if (points3d_lidar) off::colmap_points_from_lidar(cfg, frame_clouds, frames, images_ids, vr.Rcw_after, vr.tcw_after, lp, &listed);
+  off::Config cfg_out = cfg;                                                  // the refined intrinsics, when the visual stage refined them
+  cfg_out.fx = vr.intr[0]; cfg_out.fy = vr.intr[1]; cfg_out.cx = vr.intr[2]; cfg_out.cy = vr.intr[3];
+  cfg_out.d0 = vr.intr[4]; cfg_out.d1 = vr.intr[5]; cfg_out.d2 = vr.intr[6]; cfg_out.d3 = vr.intr[7];
+  if (points3d_lidar) off::colmap_points_from_lidar(vr.intr_refined ? cfg_out : cfg, frame_clouds, frames, images_ids, vr.Rcw_after, vr.tcw_after, lp, &listed);
   if (!off::write_images_txt(sparse_dir + "images.txt", vr.Rcw_after, vr.tcw_after, points3d_lidar ? &listed : nullptr) ||
       !off::write_images_txt(sparse_dir + "images_before.txt", vr.Rcw_before, vr.tcw_before) ||
       !(points3d_lidar ? off::write_points3D_lidar_txt(sparse_dir + "points3D.txt", lp) : off::write_points3D_txt(sparse_dir + "points3D.txt", vr.tracks, vr.track_used))) {
