@@ -9,6 +9,7 @@
 #include "runtime.cuh"   // (pulls comm.cuh in)
 #include "visual.cuh"
 #include "visual_outliers.h"
+#include "visual_pcg.h"
 #include "visual_plan.h"
 
 namespace lvba {
@@ -85,6 +86,14 @@ struct lvba_visual_problem {
   lvba::DevBuf<int64_t> obs_src;
   bool obs_src_ready = false;
   lvba::DevBuf<double> obs_sq;
+  // ---- ITERATIVE_SCHUR (lvba_visual_opts::linear_solver, visual_pcg.h): r z p q [4][n_rows*6], the preconditioner [n_rows][36],
+  // the dot-product partials and the status words, allocated when a solve first needs them; the CG iterations since the last
+  // reset and the iteration count and termination of the last solve (lvba_visual_linear_stats)
+  lvba::DevBuf<double> pcg_vec, pcg_minv, pcg_part, pcg_sd;
+  lvba::DevBuf<int> pcg_si;
+  int64_t cg_total = 0;
+  int cg_last = 0, cg_term = 0;
+  bool iterative() const { return opts.linear_solver == LVBA_LINEAR_ITERATIVE_SCHUR; }
   // LM state
   lvba_visual_opts opts;
   lvba::TrustRegionState lm;
@@ -486,6 +495,24 @@ inline int visual_check_loss(const lvba_visual_opts& o) {
   return LVBA_OK;
 }
 
+// the linear solver of lvba_visual_opts: a known one, and for ITERATIVE_SCHUR a finite eta > 0 and 0 <= min_linear_iter,
+// max(1, min_linear_iter) <= max_linear_iter; not with the intrinsics block or an active communicator (checked before any device
+// work)
+inline int visual_check_linear(const lvba_visual_opts& o) {
+  if (o.linear_solver != LVBA_LINEAR_DENSE_SCHUR && o.linear_solver != LVBA_LINEAR_ITERATIVE_SCHUR)
+    return fail(LVBA_ERR_INVALID_ARG, "linear_solver = %d is not an lvba_linear_solver", (int)o.linear_solver);
+  if (o.linear_solver != LVBA_LINEAR_ITERATIVE_SCHUR) return LVBA_OK;
+  if (!(std::isfinite(o.eta) && o.eta > 0.0)) return fail(LVBA_ERR_INVALID_ARG, "eta = %g: it must be finite and > 0", o.eta);
+  if (o.min_linear_iter < 0) return fail(LVBA_ERR_INVALID_ARG, "min_linear_iter = %d: it must be >= 0", (int)o.min_linear_iter);
+  if (o.max_linear_iter < std::max(1, (int)o.min_linear_iter))
+    return fail(LVBA_ERR_INVALID_ARG, "max_linear_iter = %d: it must be >= max(1, min_linear_iter)", (int)o.max_linear_iter);
+  if (o.refine_intrinsics)
+    return fail(LVBA_ERR_UNSUPPORTED, "ITERATIVE_SCHUR does not solve the intrinsics block: refine_intrinsics needs DENSE_SCHUR");
+  if (comm().active())
+    return fail(LVBA_ERR_UNSUPPORTED, "ITERATIVE_SCHUR runs on one GPU: not with an active communicator");
+  return LVBA_OK;
+}
+
 // a handle whose failed re-plan could not be undone (visual_replan) takes no further calls but destroy and the state copies
 inline int visual_check_usable(const lvba_visual_problem* P) {
   if (P->unusable) return fail(LVBA_ERR_INVALID_ARG, "this handle lost its plan in a failed lvba_visual_reset_lm: destroy it");
@@ -509,6 +536,7 @@ inline void visual_intr_forget(lvba_visual_problem* P) {
 // robust losses
 inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   LVBA_TRY(visual_check_loss(o));
+  LVBA_TRY(visual_check_linear(o));
   if (o.refine_intrinsics >> 8)
     return fail(LVBA_ERR_INVALID_ARG, "refine_intrinsics = 0x%x: only bits 0..7 name intrinsics", (unsigned)o.refine_intrinsics);
   if (o.refine_intrinsics && comm().active())
@@ -648,6 +676,80 @@ inline VisualLM visual_lm_params(const lvba_visual_problem* P, double radius) {
   return VisualLM{radius, P->opts.min_lm_diagonal, P->opts.max_lm_diagonal, P->s_cam.p, P->s_pt.p};
 }
 
+// ---------------------------------------------------------------- ITERATIVE_SCHUR (visual_pcg.h)
+// y = A x for the conjugate gradients: one warp per block row.  The row's elements are taken 32 at a time in storage order, the
+// row's own blocks (the diagonal block through its lower triangle) and then the blocks below it, each lane accumulating the six
+// components of y_r; a fixed shuffle tree sums the lanes.  Same terms as vpcg::ProdF, in another fixed order.  A no-op once the
+// solve is done (*done).
+LVBA_DEV void pcg_add6(double acc[6], int k, double v) {
+#pragma unroll
+  for (int j = 0; j < 6; ++j) acc[j] += (j == k) ? v : 0.0;
+}
+__global__ void __launch_bounds__(256) visual_pcg_product_kernel(EnvView e, const double* __restrict__ S, const double* __restrict__ dadd,
+                                                                 const double* __restrict__ x, double* __restrict__ y,
+                                                                 const int* __restrict__ done) {
+  if (*done) return;
+  const int lane = threadIdx.x & 31;
+  const int r = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (r >= e.n) return;
+  const int f = e.first[r], m1 = r - f, m2 = e.last[r] - r;
+  const double* row = S + e.row_start[r] * 36;
+  double acc[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int t = lane; t < (m1 + 1) * 36; t += 32) {
+    const int blk = t / 36, el = t - blk * 36, a = el / 6, b = el - a * 6;
+    const double v = row[t];
+    if (blk < m1) {
+      pcg_add6(acc, a, v * x[6 * (long long)(f + blk) + b]);
+    } else if (a >= b) {
+      pcg_add6(acc, a, v * x[6 * (long long)r + b]);
+      if (a > b) pcg_add6(acc, b, v * x[6 * (long long)r + a]);
+    }
+  }
+  for (int t = lane; t < m2 * 36; t += 32) {
+    const int j = t / 36, el = t - j * 36, a = el / 6, b = el - a * 6;
+    const int r2 = r + 1 + j;
+    const double v = S[(e.row_start[r2] + (r - e.first[r2])) * 36 + el];
+    pcg_add6(acc, b, v * x[6 * (long long)r2 + a]);
+  }
+#pragma unroll
+  for (int j = 0; j < 6; ++j) acc[j] = warp_sum(acc[j]);
+  if (lane < 6) {
+    const double v = (lane == 0) ? acc[0] : (lane == 1) ? acc[1] : (lane == 2) ? acc[2] : (lane == 3) ? acc[3] : (lane == 4) ? acc[4] : acc[5];
+    const long long i = 6 * (long long)r + lane;
+    y[i] = v + dadd[i] * x[i];
+  }
+}
+
+// (S + diag(dadd)) y = rhs by vpcg::solve into P->y; the status words stay in P->pcg_si (kFail: the LM's invalid step)
+inline int visual_pcg_solve(lvba_visual_problem* P) {
+  cudaStream_t s = P->stream;
+  const int64_t n6 = (int64_t)P->n_rows * 6, nch = vpcg::chunks(n6);
+  if (P->pcg_vec.n < (size_t)(4 * n6)) LVBA_TRY(P->pcg_vec.alloc((size_t)(4 * n6)));
+  if (P->pcg_minv.n < (size_t)(6 * n6)) LVBA_TRY(P->pcg_minv.alloc((size_t)(6 * n6)));
+  if (P->pcg_part.n < (size_t)nch) LVBA_TRY(P->pcg_part.alloc((size_t)nch));
+  if (P->pcg_sd.n == 0) { LVBA_TRY(P->pcg_sd.alloc(vpcg::kNDouble)); LVBA_TRY(P->pcg_si.alloc(vpcg::kNInt)); }
+  double* v = P->pcg_vec.p;
+  const vpcg::Bufs B{v, v + n6, v + 2 * n6, v + 3 * n6, P->pcg_minv.p, vpcg::Ctl{P->pcg_si.p, P->pcg_sd.p, P->pcg_part.p}};
+  const vpcg::Params o{P->opts.eta, P->opts.min_linear_iter, P->opts.max_linear_iter};
+  const EnvView ev = P->env.view();
+  CudaExec ex;
+  ex.stream = s;
+  auto prod = [&](const double* in, double* out) -> int {
+    visual_pcg_product_kernel<<<(unsigned)((P->n_rows + 7) / 8), 256, 0, s>>>(ev, P->S.p, P->dadd.p, in, out, B.c.si + vpcg::kDone);
+    LVBA_CUDA(cudaGetLastError());
+    ++ex.launches;
+    return LVBA_OK;
+  };
+  int si[vpcg::kNInt];
+  const int rc = vpcg::solve(ex, ev, P->S.p, P->dadd.p, P->rhs.p, P->y.p, B, o, prod, si, &P->d2h);
+  P->launches += ex.launches;
+  LVBA_TRY(rc);
+  P->cg_last = si[vpcg::kIter];
+  P->cg_term = si[vpcg::kTerm];
+  P->cg_total += si[vpcg::kIter];
+  return LVBA_OK;
+}
+
 // scal layout: [0] cost  [1] gmax  [2] model  [3] step^2 (pts)  [4] x^2 (pts)  [5] -  [6] step^2 (cams) [7] x^2 (cams)
 //              [8] candidate cost
 template <bool kLoss>
@@ -731,8 +833,12 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
         LVBA_TRY(P->solver.solve(P->env, P->S.p, P->dadd.p, P->y.p, s, &P->launches));
         LVBA_CUDA(cudaMemcpyAsync(P->intr_Y.p + i * n6, P->y.p, (size_t)n6 * sizeof(double), cudaMemcpyDeviceToDevice, s));
       }
-    LVBA_CUDA(cudaMemcpyAsync(P->solver.z.p, P->rhs.p, (size_t)P->n_rows * 6 * sizeof(double), cudaMemcpyDeviceToDevice, s));
-    LVBA_TRY(P->solver.solve(P->env, P->S.p, P->dadd.p, P->y.p, s, &P->launches));
+    if (P->iterative()) {
+      LVBA_TRY(visual_pcg_solve(P));
+    } else {
+      LVBA_CUDA(cudaMemcpyAsync(P->solver.z.p, P->rhs.p, (size_t)P->n_rows * 6 * sizeof(double), cudaMemcpyDeviceToDevice, s));
+      LVBA_TRY(P->solver.solve(P->env, P->S.p, P->dadd.p, P->y.p, s, &P->launches));
+    }
   }
   double yk[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   if (intr) {                                                  // the corner, y_k and the camera step y - Y y_k
@@ -784,7 +890,9 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   P->timers.end();
   LVBA_CUDA(cudaGetLastError());
   LVBA_CUDA(cudaMemcpyAsync(P->h_scal, P->scal.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, s));
-  if (P->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(P->h_scal + 15, P->solver.status.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  if (P->n_rows > 0)
+    LVBA_CUDA(cudaMemcpyAsync(P->h_scal + 15, P->iterative() ? P->pcg_si.p + vpcg::kFail : P->solver.status.p, sizeof(int),
+                              cudaMemcpyDeviceToHost, s));
   LVBA_CUDA(cudaStreamSynchronize(s));
   if (P->n_rows == 0) *reinterpret_cast<int*>(P->h_scal + 15) = 0;   // every camera constant: nothing was factorised
   P->d2h += 16 * sizeof(double);
@@ -960,6 +1068,7 @@ inline int visual_remove_impl(lvba_visual_problem* P, const uint8_t* d_remove, d
   }
   P->launches += ex.launches;
   P->lm.reset(P->opts);
+  P->cg_total = 0; P->cg_last = 0; P->cg_term = 0;
   if (removed) std::copy(h_removed.begin(), h_removed.end(), removed);
   if (n_obs_left) *n_obs_left = kept_obs;
   if (n_trk_left) *n_trk_left = kept_trk;
@@ -983,6 +1092,9 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
   o->plane_loss = LVBA_LOSS_NONE; o->plane_loss_scale = 0.1;
   o->cam_fixed = nullptr;
   o->refine_intrinsics = 0;
+  // Ceres' Solver::Options: DENSE_SCHUR (src/lvba_system.cpp:1574); eta, min / max_linear_solver_iterations
+  o->linear_solver = LVBA_LINEAR_DENSE_SCHUR;
+  o->eta = 1e-1; o->min_linear_iter = 0; o->max_linear_iter = 500;
 }
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
@@ -1098,6 +1210,7 @@ int lvba_visual_reset_lm(lvba_visual_problem* p, const lvba_visual_opts* opts) L
   LVBA_TRY(lvba::visual_set_mode(p, o));
   p->opts = o;
   p->lm.reset(o);
+  p->cg_total = 0; p->cg_last = 0; p->cg_term = 0;
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_reset_lm")
 
@@ -1148,6 +1261,7 @@ int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const 
   lvba_visual_opts o;
   if (opts) o = *opts; else lvba_visual_default_opts(&o);
   LVBA_TRY(lvba::visual_check_loss(o));                       // before any device work: the buffers stay untouched
+  LVBA_TRY(lvba::visual_check_linear(o));
   if (o.refine_intrinsics)
     return lvba::fail(LVBA_ERR_INVALID_ARG, "refine_intrinsics needs a handle (lvba_visual_reset_lm): the one-shot call's intr is const");
   LVBA_TRY(lvba::visual_check_mask(M > 0 && !lvba::visual_mask(M, o.cam_fixed).empty()));
@@ -1243,5 +1357,13 @@ int lvba_visual_get_intrinsics_system(lvba_visual_problem* p, int32_t* k, double
   }
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_get_intrinsics_system")
+
+int lvba_visual_linear_stats(lvba_visual_problem* p, int64_t* cg_iters_total, int32_t* cg_iters_last, int32_t* term_last) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  if (cg_iters_total) *cg_iters_total = p->cg_total;
+  if (cg_iters_last) *cg_iters_last = p->cg_last;
+  if (term_last) *term_last = p->cg_term;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_linear_stats")
 
 }  // extern "C"

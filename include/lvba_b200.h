@@ -127,6 +127,26 @@ typedef struct lvba_visual_opts {
   double reproj_loss_scale;      /* 1.0 */
   int32_t plane_loss;            /* LVBA_LOSS_NONE (:1639) */
   double plane_loss_scale;       /* 0.1 */
+  /* The solver of the damped reduced camera system (Ceres' linear_solver_type), lvba_linear_solver:
+   *   LVBA_LINEAR_DENSE_SCHUR (the default, the reference's choice, src/lvba_system.cpp:1574): the envelope LDL^T.
+   *   LVBA_LINEAR_ITERATIVE_SCHUR: Ceres' ITERATIVE_SCHUR with the explicit Schur complement and the SCHUR_JACOBI
+   *     preconditioner, restated from ceres-solver 2.1.0: conjugate gradients on (S + D) y = rhs preconditioned by the inverses
+   *     of its 6x6 diagonal blocks, stopped by the inexact-Newton test on the quadratic model, zeta < eta after at least
+   *     min_linear_iter iterations, or after max_linear_iter.  An inexact step is a different algorithm: iterates, iteration
+   *     counts and the final cost differ from DENSE_SCHUR's within the forcing tolerance.  A solve that fails (a preconditioner
+   *     pivot that is not finite and > 0, a rho, beta or alpha that is 0 or not finite) is an invalid LM step; one that stops
+   *     on a non-positive curvature p.Ap or at the iteration limit gives its current step.  Its envelope need not be narrow:
+   *     long tracks and loop closures, where the LDL^T fills the whole envelope, cost only their nonzero blocks per iteration.
+   *     In deterministic mode the solve adds no records: given S it has the same bits on every run.
+   * As `deterministic`: the one-shot call takes these from its opts, a handle from lvba_visual_reset_lm.  Refused before any
+   * device work: an unknown solver, and for ITERATIVE_SCHUR an eta that is not finite and > 0, min_linear_iter < 0 or
+   * max_linear_iter < max(1, min_linear_iter) (LVBA_ERR_INVALID_ARG); ITERATIVE_SCHUR with refine_intrinsics != 0 or an active
+   * communicator (LVBA_ERR_UNSUPPORTED).  lvba_visual_linear_stats reports the iterations.  The four fields sit before
+   * cam_fixed, which stays the last field. */
+  int32_t linear_solver;         /* LVBA_LINEAR_DENSE_SCHUR */
+  double eta;                    /* 0.1   Solver::Options::eta */
+  int32_t min_linear_iter;       /* 0     min_linear_solver_iterations */
+  int32_t max_linear_iter;       /* 500   max_linear_solver_iterations */
   /* Constant cameras (ceres::Problem::SetParameterBlockConstant, which the reference calls on camera 0 at
    * src/lvba_system.cpp:1582-1583): NULL (the default) or M bytes, nonzero = camera held constant.  The constant cameras are
    * fixed_cam and every camera c with cam_fixed[c] != 0; they get no row in the reduced camera system and come back
@@ -143,6 +163,11 @@ typedef struct lvba_visual_opts {
    * NULL; any nonzero entry with an active communicator is LVBA_ERR_UNSUPPORTED.  The library keeps no copy of the pointer. */
   const uint8_t* cam_fixed;
 } lvba_visual_opts;
+
+typedef enum lvba_linear_solver {
+  LVBA_LINEAR_DENSE_SCHUR = 0,
+  LVBA_LINEAR_ITERATIVE_SCHUR = 1
+} lvba_linear_solver;
 
 #define LVBA_INTR_FOCAL      0x03u   /* fx fy */
 #define LVBA_INTR_PRINCIPAL  0x0Cu   /* cx cy */
@@ -343,6 +368,10 @@ int lvba_visual_set_intrinsics(lvba_visual_problem* p, const double intr[8]);
  * lvba_visual_reset_lm, lvba_visual_reset_state or a removal, only k and step (all zeros) are written. */
 int lvba_visual_get_intrinsics_system(lvba_visual_problem* p, int32_t* k, double* border, double* corner, double* rhs,
                                       double* step);
+/* The conjugate gradients of LVBA_LINEAR_ITERATIVE_SCHUR: cg_iters_total, the iterations of every solve since the last
+ * lvba_visual_reset_lm or removal; cg_iters_last and term_last, the iteration count and termination of the last solve
+ * (0 SUCCESS, 1 NO_CONVERGENCE, 2 FAILURE).  All zero until a solve has run.  Any pointer may be NULL. */
+int lvba_visual_linear_stats(lvba_visual_problem* p, int64_t* cg_iters_total, int32_t* cg_iters_last, int32_t* term_last);
 int lvba_visual_iterate(lvba_visual_problem* p, int32_t n_iter, lvba_summary* summary);
 int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_valid_tracks,
                        int64_t* n_blocks_env, int64_t* n_pairs);

@@ -52,6 +52,9 @@
 //                comma-separated subset of focal,principal,distortion, checked when parsed (--check included).  The stage then runs
 //                on a device handle (lvba_b200::solve_visual_refine_intrinsics), prints the refined intrinsics, and --points3d lidar
 //                projects with them.  Without the flag the output is as before.
+//   --linear-solver dense_schur|iterative_schur   the solver of the visual stage's reduced camera system
+//                (lvba_visual_opts::linear_solver): the envelope LDL^T (the default) or Ceres' ITERATIVE_SCHUR, conjugate gradients at
+//                Ceres' default forcing tolerance.  Checked when parsed (--check included); without the flag the output is as before.
 #include <climits>
 #include <cmath>
 #include <cstdio>
@@ -140,6 +143,15 @@ int main(int argc, char** argv) {
       std::string e;
       if (!lvba_b200::offline::parse_intr_groups(next(), visual_opts.refine_intrinsics, &e)) {
         std::fprintf(stderr, "--refine-intrinsics: %s\n", e.c_str());
+        return 64;
+      }
+    }
+    else if (a == "--linear-solver") {
+      const std::string v = next();
+      if (v == "dense_schur") visual_opts.linear_solver = LVBA_LINEAR_DENSE_SCHUR;
+      else if (v == "iterative_schur") visual_opts.linear_solver = LVBA_LINEAR_ITERATIVE_SCHUR;
+      else {
+        std::fprintf(stderr, "--linear-solver: '%s' is not dense_schur or iterative_schur\n", v.c_str());
         return 64;
       }
     }
