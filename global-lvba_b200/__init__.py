@@ -37,6 +37,7 @@ EXPORTS = [
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
     "lvba_visual_big_counts", "lvba_visual_obs_residuals", "lvba_visual_remove_observations", "lvba_visual_remove_outliers",
     "lvba_visual_get_intrinsics", "lvba_visual_set_intrinsics", "lvba_visual_get_intrinsics_system", "lvba_visual_linear_stats",
+    "lvba_visual_schur_product", "lvba_visual_apply_system",
     "lvba_voxel_default_opts", "lvba_voxel_map_create", "lvba_voxel_map_create_windows", "lvba_voxel_map_windows",
     "lvba_voxel_map_lidar_lm_batch", "lvba_voxel_map_summary", "lvba_voxel_map_export",
     "lvba_voxel_map_lookup", "lvba_voxel_map_lidar_create", "lvba_voxel_map_lidar_lm", "lvba_voxel_map_destroy",
@@ -552,6 +553,20 @@ class VisualProblem:
         a, b, c = C.c_int64(), C.c_int32(), C.c_int32()
         _chk(self._lib.lvba_visual_linear_stats(self._h, C.byref(a), C.byref(b), C.byref(c)))
         return dict(cg_iters_total=a.value, cg_iters_last=b.value, term_last=c.value)
+
+    def schur_product(self):
+        """lvba_visual_schur_product: 1 when ITERATIVE_SCHUR runs on the matrix-free product for this plan, 0 on the explicit S."""
+        m = C.c_int32(); _chk(self._lib.lvba_visual_schur_product(self._h, C.byref(m))); return m.value
+
+    def apply_system(self, x):
+        """lvba_visual_apply_system: (S + D) x of the last ITERATIVE_SCHUR pass, x and the result [n_active*6]."""
+        x = _f64(x).ravel()
+        n6 = 6 * len(self.structure()[0])
+        if x.shape != (n6,):
+            raise ValueError(f"x has shape {x.shape}, expected ({n6},)")
+        y = np.empty(n6)
+        _chk(self._lib.lvba_visual_apply_system(self._h, _p(x, C.c_double), _p(y, C.c_double)))
+        return y
 
     def iterate(self, n):
         s = Summary(); _chk(self._lib.lvba_visual_iterate(self._h, C.c_int32(n), C.byref(s))); return s.as_dict()

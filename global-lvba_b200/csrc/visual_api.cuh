@@ -9,6 +9,7 @@
 #include "runtime.cuh"   // (pulls comm.cuh in)
 #include "visual.cuh"
 #include "visual_outliers.h"
+#include "visual_implicit.h"
 #include "visual_pcg.h"
 #include "visual_plan.h"
 
@@ -66,14 +67,17 @@ struct lvba_visual_problem {
   bool robust() const { return loss_px != LVBA_LOSS_NONE || loss_pl != LVBA_LOSS_NONE; }
   // ---- the intrinsics block (lvba_visual_opts::refine_intrinsics, set by lvba_visual_reset_lm; visual_intr.h).  The kernels take
   // the intrinsics by value in VisualView, so the handle keeps them on the host: intr above is the current value, intr_c the
-  // candidate of the last pass (intr + intr_step), intr0 the value given at create.  The row CSR of the border gather
-  // (intr_row_ptr / intr_row_obs, the observations of every camera row in ascending order) follows the plan: visual_plan clears
-  // intr_ready and the next pass with the block builds it again.
+  // candidate of the last pass (intr + intr_step), intr0 the value given at create.  Its buffers follow the plan: visual_plan
+  // clears intr_ready and the next pass with the block sets them up again.
   uint32_t intr_mask = 0;
   double intr0[8], intr_c[8], intr_step[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   bool intr_ready = false;
   bool intr_have_sys = false;                       // intr_B / intr_sys / intr_step hold the block of the last pass since the last reset
-  lvba::DevBuf<int64_t> intr_row_ptr, intr_row_obs;
+  // the row CSR of the border gather and of the matrix-free product (visual_row_csr): the observations of every camera row in
+  // ascending order, and their local landmarks (row_trk, set up with the matrix-free buffers); built again after a re-plan
+  bool rows_ready = false;
+  lvba::DevBuf<int64_t> row_ptr, row_obs;
+  lvba::DevBuf<int> row_trk;
   lvba::DevBuf<double> intr_slot, intr_rec, intr_part, intr_sys, intr_B, intr_Y, intr_dev;   // intr_dev: sk | colsq | y_k | dk
   lvba::PhaseTimers timers;
   double* h_scal = nullptr;
@@ -94,6 +98,16 @@ struct lvba_visual_problem {
   int64_t cg_total = 0;
   int cg_last = 0, cg_term = 0;
   bool iterative() const { return opts.linear_solver == LVBA_LINEAR_ITERATIVE_SCHUR; }
+  // ---- the matrix-free product of ITERATIVE_SCHUR (visual_implicit.h): the plan's choice (vimp::visual_matrix_free of its
+  // free observations, pair contributions, envelope blocks and rows), whether the last pass ran CG and on which product
+  // (lvba_visual_apply_system, lvba_visual_get_system), and the buffers, set up when a matrix-free pass first needs them:
+  // the observation records, the landmarks' params, cost and gradient slots and product vector u, the row partials and the
+  // diagonal blocks
+  int64_t n_free = 0;
+  bool matrix_free = false, imp_ready = false, cg_sys = false, imp_sys = false;
+  lvba::DevBuf<double> imp_rec, imp_params, imp_cost, imp_gmax, imp_u, imp_part, imp_D;
+  lvba::DevBuf<int> imp_zero;                       // an int 0: the "done" word of a product outside a solve
+  bool implicit_pass() const { return iterative() && matrix_free; }
   // LM state
   lvba_visual_opts opts;
   lvba::TrustRegionState lm;
@@ -182,6 +196,10 @@ inline int visual_plan(lvba_visual_problem* P, const std::vector<int64_t>& valid
   P->n_rows = (int)P->cam_of_row.size();
   P->intr_ready = false;
   P->intr_have_sys = false;
+  P->rows_ready = false;
+  P->imp_ready = false;
+  P->cg_sys = false;
+  P->imp_sys = false;
   const int64_t Tv_all = (int64_t)valid.size();
   DevBuf<int> d_row_of_cam, d_src_trk;
 
@@ -274,6 +292,11 @@ inline int visual_plan(lvba_visual_problem* P, const std::vector<int64_t>& valid
   const size_t nb = (size_t)std::max<long long>(std::max(P->n_batches, P->n_tiles) + P->n_big, 1);   // partial slots, big landmarks last
   LVBA_TRY(P->batch_cost.alloc(nb)); LVBA_TRY(P->batch_gmax.alloc(nb)); LVBA_TRY(P->batch_out.alloc(nb * 4));
   LVBA_TRY(P->cam_out.alloc((size_t)((P->n_rows + 127) / 128 + 1) * 2));
+  // the product of ITERATIVE_SCHUR for this plan (one GPU: ITERATIVE_SCHUR refuses an active communicator)
+  P->n_free = 0;
+  for (int64_t k = 0; k < Tv_all; ++k)
+    for (int64_t q = obs_ptr[valid[k]]; q < obs_ptr[valid[k] + 1]; ++q) P->n_free += row_of_cam[obs_cam[q]] >= 0;
+  P->matrix_free = vimp::visual_matrix_free(P->n_free, P->n_pairs, P->env.nblocks, P->n_rows);
   LVBA_CUDA(cudaStreamSynchronize(s));                         // the temporaries above are idle before they are parked
   return LVBA_OK;
 }
@@ -566,10 +589,11 @@ inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   return LVBA_OK;
 }
 
-// ---------------------------------------------------------------- the intrinsics block (visual_intr.h)
-// The row CSR of the border gather and the block's buffers, for the current plan
-inline int visual_intr_setup(lvba_visual_problem* P) {
-  if (P->intr_ready) return LVBA_OK;
+// ---------------------------------------------------------------- the row CSR
+// The observations of every camera row in ascending order (row_ptr / row_obs), for the current plan: the border gather of the
+// intrinsics block and the matrix-free product read it
+inline int visual_row_csr(lvba_visual_problem* P) {
+  if (P->rows_ready) return LVBA_OK;
   cudaStream_t s = P->stream;
   std::vector<int> row((size_t)P->nnz);
   if (P->nnz > 0) {
@@ -577,19 +601,22 @@ inline int visual_intr_setup(lvba_visual_problem* P) {
     LVBA_CUDA(cudaStreamSynchronize(s));
     P->d2h += P->nnz * (int64_t)sizeof(int);
   }
-  std::vector<int64_t> ptr((size_t)P->n_rows + 1, 0), obs;
-  for (int r : row)
-    if (r >= 0) ++ptr[(size_t)r + 1];
-  for (int r = 0; r < P->n_rows; ++r) ptr[(size_t)r + 1] += ptr[(size_t)r];
-  obs.resize((size_t)ptr[(size_t)P->n_rows]);
-  {
-    std::vector<int64_t> at(ptr.begin(), ptr.end() - 1);
-    for (int64_t w = 0; w < P->nnz; ++w)
-      if (row[(size_t)w] >= 0) obs[(size_t)at[(size_t)row[(size_t)w]]++] = w;
-  }
-  LVBA_TRY(P->intr_row_ptr.upload(ptr, s, &P->h2d));
-  LVBA_TRY(P->intr_row_obs.alloc(std::max<size_t>(obs.size(), 1)));
-  if (!obs.empty()) LVBA_TRY(P->intr_row_obs.upload(obs, s, &P->h2d));
+  std::vector<int64_t> ptr, obs;
+  vimp::row_csr(P->n_rows, P->nnz, row.data(), ptr, obs);
+  LVBA_TRY(P->row_ptr.upload(ptr, s, &P->h2d));
+  LVBA_TRY(P->row_obs.alloc(std::max<size_t>(obs.size(), 1)));
+  if (!obs.empty()) LVBA_TRY(P->row_obs.upload(obs, s, &P->h2d));
+  LVBA_CUDA(cudaStreamSynchronize(s));                         // the host vectors are idle before they go out of scope
+  P->rows_ready = true;
+  return LVBA_OK;
+}
+
+// ---------------------------------------------------------------- the intrinsics block (visual_intr.h)
+// The row CSR of the border gather and the block's buffers, for the current plan
+inline int visual_intr_setup(lvba_visual_problem* P) {
+  if (P->intr_ready) return LVBA_OK;
+  cudaStream_t s = P->stream;
+  LVBA_TRY(visual_row_csr(P));
   const size_t Tv = (size_t)std::max<int64_t>(P->Tv, 1), n6 = (size_t)std::max(P->n_rows, 1) * 6;
   LVBA_TRY(P->intr_slot.alloc(Tv * vintr::kSys));
   LVBA_TRY(P->intr_rec.alloc((size_t)std::max<int64_t>(P->nnz, 1) * vintr::kRec));
@@ -610,28 +637,40 @@ inline int visual_intr_reduce(lvba_visual_problem* P, CudaExec& ex, const double
 }
 
 // Jacobi scaling vectors from the Jacobian at the current state (Ceres: once, at iteration 0)
+inline int visual_imp_setup(lvba_visual_problem* P);
 template <bool kLoss>
 inline int visual_compute_scale_t(lvba_visual_problem* P, int enabled) {
   cudaStream_t s = P->stream;
-  LVBA_TRY(P->cam_colsq.zero(s));
-  if (P->n_tiles > 0) {
-    if (P->det) visual_colnorm_kernel<true, kLoss><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->det_C.p, P->pt_colsq.p);
-    else visual_colnorm_kernel<false, kLoss><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
-    ++P->launches;
-  }
-  if (P->n_big > 0) {
-    if (P->det)
-      wide_pass(s, P->n_big_obs, vbig::ColObsPass<true, kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p,
-                                                               P->det_C.p + 6 * P->drun.n_runs}, &P->launches);
-    else
-      wide_pass(s, P->n_big_obs, vbig::ColObsPass<false, kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p}, &P->launches);
-    wide_pass(s, P->n_big, vbig::ColTrackPass<kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p, P->pt_colsq.p}, &P->launches);
-  }
-  if (P->det) {
+  if (P->implicit_pass()) {                                    // the column norms in a fixed order (visual_implicit.h)
+    LVBA_TRY(visual_imp_setup(P));
+    const vimp::View iv{(int64_t)P->Tv, P->n_rows, P->row_ptr.p, P->row_obs.p, P->row_trk.p, P->imp_rec.p, P->imp_params.p};
     CudaExec ex;
     ex.stream = s;
-    LVBA_TRY(ex.for_each(P->det_G.by_dst.n_runs * 6, tiles::gather_part(P->det_G, P->det_C.p, 6, 0, 6, P->cam_colsq.p)));
+    LVBA_TRY(ex.for_each(P->nnz, vimp::ColObsF<kLoss>{P->view(), iv, P->state()}));
+    LVBA_TRY(ex.for_each((int64_t)P->n_rows * 6, vimp::ColRowF{iv, P->cam_colsq.p}));
+    LVBA_TRY(ex.for_each(P->Tv, vimp::ColTrkF<kLoss>{P->view(), iv, P->state(), P->pt_colsq.p}));
     P->launches += ex.launches;
+  } else {
+    LVBA_TRY(P->cam_colsq.zero(s));
+    if (P->n_tiles > 0) {
+      if (P->det) visual_colnorm_kernel<true, kLoss><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->det_C.p, P->pt_colsq.p);
+      else visual_colnorm_kernel<false, kLoss><<<P->n_tiles, kVisTileSlots, 0, s>>>(P->view(), P->state(), P->cam_colsq.p, P->pt_colsq.p);
+      ++P->launches;
+    }
+    if (P->n_big > 0) {
+      if (P->det)
+        wide_pass(s, P->n_big_obs, vbig::ColObsPass<true, kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p,
+                                                                 P->det_C.p + 6 * P->drun.n_runs}, &P->launches);
+      else
+        wide_pass(s, P->n_big_obs, vbig::ColObsPass<false, kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p, P->cam_colsq.p}, &P->launches);
+      wide_pass(s, P->n_big, vbig::ColTrackPass<kLoss>{P->view(), P->big_view(), P->state(), P->big_obs.p, P->pt_colsq.p}, &P->launches);
+    }
+    if (P->det) {
+      CudaExec ex;
+      ex.stream = s;
+      LVBA_TRY(ex.for_each(P->det_G.by_dst.n_runs * 6, tiles::gather_part(P->det_G, P->det_C.p, 6, 0, 6, P->cam_colsq.p)));
+      P->launches += ex.launches;
+    }
   }
   Comm& cm = comm();
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->cam_colsq.p, (size_t)P->n_rows * 6, s));
@@ -720,7 +759,146 @@ __global__ void __launch_bounds__(256) visual_pcg_product_kernel(EnvView e, cons
   }
 }
 
-// (S + diag(dadd)) y = rhs by vpcg::solve into P->y; the status words stay in P->pcg_si (kFail: the LM's invalid step)
+
+// ---- the matrix-free product (visual_implicit.h), the hot path of ITERATIVE_SCHUR on a plan that chose it
+// u_k = C_k^-1 sum J_X^T (J_c x_row) in double-double (vimp::DD) for the landmarks k0 + g (g < k1 - k0): a group of W threads
+// per landmark, lane j taking
+// the observations j, j + W, ... of the landmark, a fixed xor tree over the group's lanes (W <= 32: one landmark per W lanes of a
+// warp; W = 128: one landmark per CTA, the warps' sums then added in warp order).  A no-op once the solve is done (*done).
+template <int W>
+__global__ void __launch_bounds__(W > 32 ? W : 256) visual_imp_track_kernel(vimp::View iv, const int* __restrict__ trk_ptr,
+                                                                              const int* __restrict__ obs_row, int64_t k0, int64_t k1,
+                                                                              const double* __restrict__ x, double* __restrict__ u,
+                                                                              const int* __restrict__ done) {
+  if (*done) return;
+  constexpr int G = W > 32 ? 32 : W;                 // lanes of the shuffle tree
+  const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t k = k0 + (W > 32 ? (int64_t)blockIdx.x : t / W);
+  const int lane = W > 32 ? (int)threadIdx.x : (int)(t % W);
+  vimp::DD a[3] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+  if (k < k1) {
+    const int64_t hi = trk_ptr[k + 1];
+    for (int64_t s = trk_ptr[k] + lane; s < hi; s += W) {
+      const int row = obs_row[s];
+      if (row >= 0) vimp::track_term(iv.rec + vimp::kRec * s, x + 6 * (int64_t)row, a);
+    }
+  }
+#pragma unroll
+  for (int o = G / 2; o > 0; o >>= 1)
+#pragma unroll
+    for (int m = 0; m < 3; ++m)
+      a[m] = vimp::dd_add(a[m], vimp::DD{__shfl_xor_sync(0xffffffffu, a[m].hi, o, G), __shfl_xor_sync(0xffffffffu, a[m].lo, o, G)});
+  if constexpr (W > 32) {
+    __shared__ vimp::DD red[W / 32][3];
+    if ((threadIdx.x & 31) == 0)
+      for (int m = 0; m < 3; ++m) red[threadIdx.x >> 5][m] = a[m];
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    for (int m = 0; m < 3; ++m) {
+      vimp::DD v = red[0][m];
+      for (int w = 1; w < W / 32; ++w) v = vimp::dd_add(v, red[w][m]);
+      a[m] = v;
+    }
+  }
+  if (lane == 0 && k < k1) vimp::track_finish(iv.params + kTrkParams * k, a, u + 6 * k);
+}
+
+// y_r = sum J_c^T (J_c x_r - J_X u) + dadd_r o x_r in double-double, rounded once: one warp per camera row, lane j taking the
+// positions j, j + 32, ... of the row's list, a fixed shuffle tree over the lanes.  A no-op once the solve is done (*done).
+__global__ void __launch_bounds__(256) visual_imp_row_kernel(vimp::View iv, const double* __restrict__ dadd, const double* __restrict__ x,
+                                                             const double* __restrict__ u, double* __restrict__ y,
+                                                             const int* __restrict__ done) {
+  if (*done) return;
+  const int lane = threadIdx.x & 31;
+  const int r = (int)(((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5);
+  if (r >= iv.n_rows) return;
+  const double* xr = x + 6 * (int64_t)r;
+  vimp::DD acc[6] = {{0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}, {0.0, 0.0}};
+  const int64_t hi = iv.row_ptr[r + 1];
+  for (int64_t p = iv.row_ptr[r] + lane; p < hi; p += 32)
+    vimp::row_term(iv.rec + vimp::kRec * iv.row_obs[p], xr, u + 6 * (int64_t)iv.row_trk[p], acc);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+    for (int j = 0; j < 6; ++j)
+      acc[j] = vimp::dd_add(acc[j], vimp::DD{__shfl_xor_sync(0xffffffffu, acc[j].hi, o), __shfl_xor_sync(0xffffffffu, acc[j].lo, o)});
+  if (lane < 6) {
+    vimp::DD v = acc[0];
+#pragma unroll
+    for (int j = 1; j < 6; ++j) if (lane == j) v = acc[j];
+    const int64_t i = 6 * (int64_t)r + lane;
+    y[i] = vimp::row_finish(v, dadd[i], x[i]);
+  }
+}
+
+// Landmarks of up to kImpShort observations take 8 lanes each, longer ones a CTA of 128 threads
+constexpr int kImpShort = 128;
+
+inline vimp::View visual_imp_view(const lvba_visual_problem* P) {
+  return vimp::View{(int64_t)P->Tv, P->n_rows, P->row_ptr.p, P->row_obs.p, P->row_trk.p, P->imp_rec.p, P->imp_params.p};
+}
+
+// out = (S + diag(dadd)) in through the Jacobian records of the last matrix-free linearisation; done: the solve's status word
+inline int visual_imp_product(lvba_visual_problem* P, const double* in, double* out, const int* done, int64_t* launches) {
+  cudaStream_t s = P->stream;
+  const vimp::View iv = visual_imp_view(P);
+  const int64_t ns = P->Tv_small, nb = P->Tv - P->Tv_small;
+  static_assert(kImpShort == tiles::kSlots, "the small landmarks are those of at most kSlots observations");
+  if (ns > 0) {
+    visual_imp_track_kernel<8><<<(unsigned)((ns * 8 + 255) / 256), 256, 0, s>>>(iv, P->trk_ptr.p, P->obs_row.p, 0, ns, in, P->imp_u.p, done);
+    ++*launches;
+  }
+  if (nb > 0) {
+    visual_imp_track_kernel<128><<<(unsigned)nb, 128, 0, s>>>(iv, P->trk_ptr.p, P->obs_row.p, ns, P->Tv, in, P->imp_u.p, done);
+    ++*launches;
+  }
+  visual_imp_row_kernel<<<(unsigned)((P->n_rows + 7) / 8), 256, 0, s>>>(iv, P->dadd.p, in, P->imp_u.p, out, done);
+  ++*launches;
+  LVBA_CUDA(cudaGetLastError());
+  return LVBA_OK;
+}
+
+// The buffers of the matrix-free linearisation and product, for the current plan: the row CSR with its landmarks, the records
+inline int visual_imp_setup(lvba_visual_problem* P) {
+  if (P->imp_ready) return LVBA_OK;
+  cudaStream_t s = P->stream;
+  LVBA_TRY(visual_row_csr(P));
+  const int64_t n_list = std::max<int64_t>(P->n_free, 1), Tv = std::max<int64_t>(P->Tv, 1), nr = std::max(P->n_rows, 1);
+  LVBA_TRY(P->row_trk.alloc((size_t)n_list));
+  CudaExec ex;
+  ex.stream = s;
+  LVBA_TRY(ex.for_each(P->n_free, vimp::RowTrkF{P->trk_ptr.p, P->Tv, P->row_obs.p, P->row_trk.p}));
+  P->launches += ex.launches;
+  LVBA_TRY(P->imp_rec.alloc((size_t)std::max<int64_t>(P->nnz, 1) * vimp::kRec));
+  LVBA_TRY(P->imp_params.alloc((size_t)Tv * kTrkParams));
+  LVBA_TRY(P->imp_cost.alloc((size_t)Tv)); LVBA_TRY(P->imp_gmax.alloc((size_t)Tv)); LVBA_TRY(P->imp_u.alloc((size_t)Tv * 6));
+  LVBA_TRY(P->imp_part.alloc((size_t)nr * vimp::kLanes * vimp::kRowOut)); LVBA_TRY(P->imp_D.alloc((size_t)nr * 36));
+  if (P->imp_zero.n == 0) { LVBA_TRY(P->imp_zero.alloc(1)); LVBA_TRY(P->imp_zero.zero(s)); }
+  P->imp_ready = true;
+  return LVBA_OK;
+}
+
+// The build of a matrix-free pass: the records, the landmarks' params and partial slots, rhs, cam_colsq, cam_grad and the
+// diagonal blocks, the cost and gradient max into scal[0] / scal[1].  No S.
+template <bool kLoss>
+inline int visual_imp_build(lvba_visual_problem* P, const VisualLM& lm) {
+  cudaStream_t s = P->stream;
+  LVBA_TRY(visual_imp_setup(P));
+  const vimp::View iv = visual_imp_view(P);
+  CudaExec ex;
+  ex.stream = s;
+  wide_pass(s, P->nnz, vimp::ObsF<kLoss>{P->view(), iv, P->state(), lm}, &P->launches);   // as vbig::ObsPass: no spill at 128 threads
+  LVBA_TRY(ex.for_each(P->Tv, vimp::TrackF<kLoss>{P->view(), iv, P->state(), lm, P->imp_cost.p, P->imp_gmax.p}));
+  LVBA_TRY(ex.for_each((int64_t)P->n_rows * vimp::kLanes, vimp::RowPartF{iv, P->imp_part.p}));
+  LVBA_TRY(ex.for_each((int64_t)P->n_rows * vimp::kRowOut, vimp::RowSumF{P->imp_part.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->imp_D.p}));
+  P->launches += ex.launches;
+  reduce_partials_kernel<<<1, 256, 0, s>>>(P->imp_cost.p, (int)P->Tv, P->scal.p + 0);
+  reduce_max_kernel<<<1, 256, 0, s>>>(P->imp_gmax.p, (int)P->Tv, P->scal.p + 1);
+  P->launches += 2;
+  return LVBA_OK;
+}
+
+// (S + diag(dadd)) y = rhs by vpcg::solve into P->y, on the explicit or the matrix-free product (P->implicit_pass()); the status words stay in P->pcg_si (kFail: the LM's invalid step)
 inline int visual_pcg_solve(lvba_visual_problem* P) {
   cudaStream_t s = P->stream;
   const int64_t n6 = (int64_t)P->n_rows * 6, nch = vpcg::chunks(n6);
@@ -734,14 +912,20 @@ inline int visual_pcg_solve(lvba_visual_problem* P) {
   const EnvView ev = P->env.view();
   CudaExec ex;
   ex.stream = s;
-  auto prod = [&](const double* in, double* out) -> int {
-    visual_pcg_product_kernel<<<(unsigned)((P->n_rows + 7) / 8), 256, 0, s>>>(ev, P->S.p, P->dadd.p, in, out, B.c.si + vpcg::kDone);
-    LVBA_CUDA(cudaGetLastError());
-    ++ex.launches;
-    return LVBA_OK;
-  };
   int si[vpcg::kNInt];
-  const int rc = vpcg::solve(ex, ev, P->S.p, P->dadd.p, P->rhs.p, P->y.p, B, o, prod, si, &P->d2h);
+  int rc;
+  if (P->implicit_pass()) {
+    auto prod = [&](const double* in, double* out) { return visual_imp_product(P, in, out, B.c.si + vpcg::kDone, &ex.launches); };
+    rc = vpcg::solve_with(ex, P->n_rows, vpcg::PrecDF{P->imp_D.p, P->dadd.p, B.minv, B.c}, P->rhs.p, P->y.p, B, o, prod, si, &P->d2h);
+  } else {
+    auto prod = [&](const double* in, double* out) -> int {
+      visual_pcg_product_kernel<<<(unsigned)((P->n_rows + 7) / 8), 256, 0, s>>>(ev, P->S.p, P->dadd.p, in, out, B.c.si + vpcg::kDone);
+      LVBA_CUDA(cudaGetLastError());
+      ++ex.launches;
+      return LVBA_OK;
+    };
+    rc = vpcg::solve(ex, ev, P->S.p, P->dadd.p, P->rhs.p, P->y.p, B, o, prod, si, &P->d2h);
+  }
   P->launches += ex.launches;
   LVBA_TRY(rc);
   P->cg_last = si[vpcg::kIter];
@@ -759,54 +943,58 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   const EnvView ev = P->env.view();
   Comm& cm = comm();
   P->timers.begin(PH_BUILD);
-  LVBA_TRY(P->S.zero(s)); LVBA_TRY(P->rhs.zero(s)); LVBA_TRY(P->cam_colsq.zero(s)); LVBA_TRY(P->cam_grad.zero(s));
-  LVBA_CUDA(cudaMemsetAsync(P->scal.p + 1, 0, sizeof(double), s));
-  if (P->n_tiles > 0) {
-    if (P->det)
-      visual_build_kernel<true, kLoss><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
-          P->view(), ev, P->state(), lm, P->det_S.rec.p, P->det_G.rec.p, nullptr, nullptr, P->batch_cost.p, P->batch_gmax.p);
-    else
-      visual_build_kernel<false, kLoss><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
-          P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
-    ++P->launches;
-  }
-  if (P->n_big > 0) {        // cost and gradient max of landmark b in the partial slots n_tiles + b
-    const VisualView vv = P->view();
-    const vbig::View bv = P->big_view();
-    wide_pass(s, P->n_big_obs, vbig::ObsPass<kLoss>{vv, bv, P->state(), lm, P->big_obs.p}, &P->launches);
-    wide_pass(s, P->n_big, vbig::TrackPass<kLoss>{vv, bv, P->state(), lm, P->big_obs.p, P->big_params.p,
-                                                  P->batch_cost.p + P->n_tiles, P->batch_gmax.p + P->n_tiles}, &P->launches);
-    if (P->det) {
-      const int64_t s0 = P->prun.n_runs + P->drun.n_runs, g0 = P->drun.n_runs;
-      wide_pass(s, P->n_big_obs, vbig::SlotsDetF{vv, bv, P->big_params.p, P->big_obs.p, P->det_S.rec.p + 36 * s0,
-                                                 P->det_G.rec.p + 18 * g0, nullptr, nullptr}, &P->launches);
-      wide_pass(s, P->n_big_pairs, vbig::PairsDetF{vv, bv, P->big_obs.p, P->det_S.rec.p + 36 * (s0 + P->n_big_obs)}, &P->launches);
-    } else {
-      wide_pass(s, P->n_big_obs, vbig::SlotsF{vv, bv, P->big_params.p, P->big_obs.p, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p}, &P->launches);
-      wide_pass(s, P->n_big_pairs, vbig::PairsF{vv, bv, P->big_obs.p, P->S.p}, &P->launches);
+  const bool imp = P->implicit_pass();
+  if (imp) LVBA_TRY(visual_imp_build<kLoss>(P, lm));
+  if (!imp) {
+    LVBA_TRY(P->S.zero(s)); LVBA_TRY(P->rhs.zero(s)); LVBA_TRY(P->cam_colsq.zero(s)); LVBA_TRY(P->cam_grad.zero(s));
+    LVBA_CUDA(cudaMemsetAsync(P->scal.p + 1, 0, sizeof(double), s));
+    if (P->n_tiles > 0) {
+      if (P->det)
+        visual_build_kernel<true, kLoss><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
+            P->view(), ev, P->state(), lm, P->det_S.rec.p, P->det_G.rec.p, nullptr, nullptr, P->batch_cost.p, P->batch_gmax.p);
+      else
+        visual_build_kernel<false, kLoss><<<P->n_tiles, kVisTileSlots, visual_build_smem_bytes(), s>>>(
+            P->view(), ev, P->state(), lm, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p, P->batch_cost.p, P->batch_gmax.p);
+      ++P->launches;
     }
-  }
-  if (P->det) {
-    CudaExec ex;
-    ex.stream = s;
-    const int64_t nr = P->det_G.by_dst.n_runs;
-    LVBA_TRY(ex.for_each(P->det_S.by_dst.n_runs * 36, tiles::gather_of(P->det_S, P->S.p)));
-    LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 0, 6, P->rhs.p)));
-    LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 6, 6, P->cam_colsq.p)));
-    LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 12, 6, P->cam_grad.p)));
-    P->launches += ex.launches;
-  }
-  reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_tiles + P->n_big), P->scal.p + 0);
-  reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, (int)(P->n_tiles + P->n_big), P->scal.p + 1);
-  P->launches += 2;
-  if (cm.active()) {
-    // row-owned reduced camera system (SURVEY.md 8(e)): see lidar_build_dev
-    if (P->solver.dist()) LVBA_TRY(P->solver.exchange_rows(P->env, P->S.p, s, &P->launches));
-    else LVBA_TRY(cm.allreduce_sum(P->S.p, (size_t)P->env.nblocks * 36, s));
-    LVBA_TRY(cm.allreduce_sum(P->rhs.p, (size_t)P->n_rows * 6, s));
-    LVBA_TRY(cm.allreduce_sum(P->cam_colsq.p, (size_t)P->n_rows * 6, s));
-    LVBA_TRY(cm.allreduce_sum(P->cam_grad.p, (size_t)P->n_rows * 6, s));
-    LVBA_TRY(cm.allreduce_sum(P->scal.p + 0, 1, s));
+    if (P->n_big > 0) {        // cost and gradient max of landmark b in the partial slots n_tiles + b
+      const VisualView vv = P->view();
+      const vbig::View bv = P->big_view();
+      wide_pass(s, P->n_big_obs, vbig::ObsPass<kLoss>{vv, bv, P->state(), lm, P->big_obs.p}, &P->launches);
+      wide_pass(s, P->n_big, vbig::TrackPass<kLoss>{vv, bv, P->state(), lm, P->big_obs.p, P->big_params.p,
+                                                    P->batch_cost.p + P->n_tiles, P->batch_gmax.p + P->n_tiles}, &P->launches);
+      if (P->det) {
+        const int64_t s0 = P->prun.n_runs + P->drun.n_runs, g0 = P->drun.n_runs;
+        wide_pass(s, P->n_big_obs, vbig::SlotsDetF{vv, bv, P->big_params.p, P->big_obs.p, P->det_S.rec.p + 36 * s0,
+                                                   P->det_G.rec.p + 18 * g0, nullptr, nullptr}, &P->launches);
+        wide_pass(s, P->n_big_pairs, vbig::PairsDetF{vv, bv, P->big_obs.p, P->det_S.rec.p + 36 * (s0 + P->n_big_obs)}, &P->launches);
+      } else {
+        wide_pass(s, P->n_big_obs, vbig::SlotsF{vv, bv, P->big_params.p, P->big_obs.p, P->S.p, P->rhs.p, P->cam_colsq.p, P->cam_grad.p}, &P->launches);
+        wide_pass(s, P->n_big_pairs, vbig::PairsF{vv, bv, P->big_obs.p, P->S.p}, &P->launches);
+      }
+    }
+    if (P->det) {
+      CudaExec ex;
+      ex.stream = s;
+      const int64_t nr = P->det_G.by_dst.n_runs;
+      LVBA_TRY(ex.for_each(P->det_S.by_dst.n_runs * 36, tiles::gather_of(P->det_S, P->S.p)));
+      LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 0, 6, P->rhs.p)));
+      LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 6, 6, P->cam_colsq.p)));
+      LVBA_TRY(ex.for_each(nr * 6, tiles::gather_part(P->det_G, P->det_G.rec.p, 18, 12, 6, P->cam_grad.p)));
+      P->launches += ex.launches;
+    }
+    reduce_partials_kernel<<<1, 256, 0, s>>>(P->batch_cost.p, (int)(P->n_tiles + P->n_big), P->scal.p + 0);
+    reduce_max_kernel<<<1, 256, 0, s>>>(P->batch_gmax.p, (int)(P->n_tiles + P->n_big), P->scal.p + 1);
+    P->launches += 2;
+    if (cm.active()) {
+      // row-owned reduced camera system (SURVEY.md 8(e)): see lidar_build_dev
+      if (P->solver.dist()) LVBA_TRY(P->solver.exchange_rows(P->env, P->S.p, s, &P->launches));
+      else LVBA_TRY(cm.allreduce_sum(P->S.p, (size_t)P->env.nblocks * 36, s));
+      LVBA_TRY(cm.allreduce_sum(P->rhs.p, (size_t)P->n_rows * 6, s));
+      LVBA_TRY(cm.allreduce_sum(P->cam_colsq.p, (size_t)P->n_rows * 6, s));
+      LVBA_TRY(cm.allreduce_sum(P->cam_grad.p, (size_t)P->n_rows * 6, s));
+      LVBA_TRY(cm.allreduce_sum(P->scal.p + 0, 1, s));
+    }
   }
   const bool intr = P->intr_mask != 0;
   const int64_t n6 = (int64_t)P->n_rows * 6;
@@ -816,7 +1004,7 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
     ex.stream = s;
     LVBA_TRY(ex.for_each(P->Tv, vintr::TrackF<kLoss>{P->view(), P->state(), lm, P->intr_dev.p, P->intr_slot.p, P->intr_rec.p}));
     LVBA_TRY(visual_intr_reduce(P, ex, P->intr_slot.p, P->Tv, vintr::kSys, P->intr_sys.p));
-    LVBA_TRY(ex.for_each(P->n_rows * (int64_t)vintr::kRec, vintr::RowGatherF{P->intr_row_ptr.p, P->intr_row_obs.p, P->intr_rec.p, n6, P->intr_B.p}));
+    LVBA_TRY(ex.for_each(P->n_rows * (int64_t)vintr::kRec, vintr::RowGatherF{P->row_ptr.p, P->row_obs.p, P->intr_rec.p, n6, P->intr_B.p}));
     P->launches += ex.launches;
   }
   P->timers.end();
@@ -869,7 +1057,13 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
     ++P->launches;
   }
   if (!intr) {
-    if (P->n_big > 0)
+    if (P->n_big > 0 && imp)                                   // the big landmarks' records and params of the matrix-free build
+      wide_pass(s, P->n_big, vbig::BacksubStridePass<kLoss, vimp::kRec>{P->view(), P->big_view(), P->state(), lm,
+                                                                  P->imp_rec.p + vimp::kRec * (P->nnz - P->n_big_obs),
+                                                                  P->imp_params.p + kTrkParams * P->Tv_small, P->y.p, P->Xc.p,
+                                                                  want_steps ? P->pt_step.p : nullptr,
+                                                                  P->batch_out.p + 4 * (int64_t)P->n_batches}, &P->launches);
+    else if (P->n_big > 0)
       wide_pass(s, P->n_big, vbig::BacksubPass<kLoss>{P->view(), P->big_view(), P->state(), lm, P->big_obs.p, P->big_params.p, P->y.p,
                                                       P->Xc.p, want_steps ? P->pt_step.p : nullptr,
                                                       P->batch_out.p + 4 * (int64_t)P->n_batches}, &P->launches);
@@ -896,6 +1090,8 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   LVBA_CUDA(cudaStreamSynchronize(s));
   if (P->n_rows == 0) *reinterpret_cast<int*>(P->h_scal + 15) = 0;   // every camera constant: nothing was factorised
   P->d2h += 16 * sizeof(double);
+  P->cg_sys = P->iterative() && P->n_rows > 0;
+  P->imp_sys = imp;
   if (intr) {        // the block in the gradient max-norm, the status and the norms (Ceres: ||x|| over all 8 entries of the block)
     double* h = P->h_scal;
     h[1] = std::max(h[1], h[9]);
@@ -1196,6 +1392,7 @@ int lvba_visual_get_system(lvba_visual_problem* p, double* rhs, double* blocks) 
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
   LVBA_TRY(lvba::visual_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
+  if (blocks && p->imp_sys) return lvba::fail(LVBA_ERR_UNSUPPORTED, "the last pass ran the matrix-free product of ITERATIVE_SCHUR: there is no S");
   if (rhs && p->n_rows > 0) LVBA_CUDA(cudaMemcpyAsync(rhs, p->rhs.p, (size_t)p->n_rows * 6 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
   if (blocks && p->env.nblocks > 0) LVBA_CUDA(cudaMemcpyAsync(blocks, p->S.p, (size_t)p->env.nblocks * 36 * sizeof(double), cudaMemcpyDeviceToHost, p->stream));
   LVBA_CUDA(cudaStreamSynchronize(p->stream));
@@ -1211,6 +1408,7 @@ int lvba_visual_reset_lm(lvba_visual_problem* p, const lvba_visual_opts* opts) L
   p->opts = o;
   p->lm.reset(o);
   p->cg_total = 0; p->cg_last = 0; p->cg_term = 0;
+  p->cg_sys = false;
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_reset_lm")
 
@@ -1357,6 +1555,37 @@ int lvba_visual_get_intrinsics_system(lvba_visual_problem* p, int32_t* k, double
   }
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_get_intrinsics_system")
+
+int lvba_visual_schur_product(lvba_visual_problem* p, int32_t* matrix_free) LVBA_ABI_BEGIN {
+  if (!p || !matrix_free) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
+  *matrix_free = p->matrix_free ? 1 : 0;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_schur_product")
+
+int lvba_visual_apply_system(lvba_visual_problem* p, const double* x, double* y) LVBA_ABI_BEGIN {
+  if (!p || !x || !y) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  LVBA_TRY(lvba::visual_check_usable(p));
+  if (!p->cg_sys) return lvba::fail(LVBA_ERR_INVALID_ARG, "no system: the last pass since the last reset or re-plan did not run ITERATIVE_SCHUR");
+  LVBA_CUDA(cudaSetDevice(p->device));
+  cudaStream_t s = p->stream;
+  const size_t n6 = (size_t)p->n_rows * 6;
+  lvba::DevBuf<double> d;
+  LVBA_TRY(d.alloc(2 * n6));
+  LVBA_TRY(d.upload(x, n6, s, &p->h2d));
+  if (p->imp_zero.n == 0) { LVBA_TRY(p->imp_zero.alloc(1)); LVBA_TRY(p->imp_zero.zero(s)); }
+  if (p->imp_sys) {
+    LVBA_TRY(lvba::visual_imp_product(p, d.p, d.p + n6, p->imp_zero.p, &p->launches));
+  } else {
+    lvba::visual_pcg_product_kernel<<<(unsigned)((p->n_rows + 7) / 8), 256, 0, s>>>(p->env.view(), p->S.p, p->dadd.p, d.p, d.p + n6, p->imp_zero.p);
+    LVBA_CUDA(cudaGetLastError());
+    ++p->launches;
+  }
+  LVBA_CUDA(cudaMemcpyAsync(y, d.p + n6, n6 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  LVBA_CUDA(cudaStreamSynchronize(s));
+  p->d2h += (int64_t)(n6 * sizeof(double));
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_apply_system")
 
 int lvba_visual_linear_stats(lvba_visual_problem* p, int64_t* cg_iters_total, int32_t* cg_iters_last, int32_t* term_last) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");

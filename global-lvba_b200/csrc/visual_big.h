@@ -89,6 +89,37 @@ struct ObsPass {               // one item per observation of the big landmarks
   }
 };
 
+// The landmark step of local landmark k at X, from acc = sum J_X^T J_X (xx xy xz yy yz zz) | sum J_X^T r and c = sum r^2 (kLoss:
+// sum rho) over its observations: the plane term, the LM diagonal of the point columns, C^-1, g_p and w = C^-1 g_p into
+// params + kTrkParams b (kTrkParams layout), 1/2 (c + the plane's term) into cost[b] and max |g_p| (unscaled) into gmax[b].
+// TrackPass and the matrix-free linearisation (visual_implicit.h) share it.
+template <bool kLoss>
+LVBA_BHD void landmark_step(const VisualView& vv, const VisualLM& lm, int64_t k, const double* X, double* acc, double c, double* params,
+                            double* cost, double* gmax, int64_t b) {
+  double rp, Jpl[3];
+  plane_eval(vv, vv.plane + 4 * k, X, rp, Jpl);
+  if constexpr (kLoss) c += plane_loss(vv, rp, Jpl);
+  else c += rp * rp;
+  const double* sp = lm.s_pt + 3 * k;
+  Jpl[0] *= sp[0]; Jpl[1] *= sp[1]; Jpl[2] *= sp[2];
+  acc[0] += Jpl[0] * Jpl[0]; acc[1] += Jpl[0] * Jpl[1]; acc[2] += Jpl[0] * Jpl[2];
+  acc[3] += Jpl[1] * Jpl[1]; acc[4] += Jpl[1] * Jpl[2]; acc[5] += Jpl[2] * Jpl[2];
+  acc[6] += Jpl[0] * rp; acc[7] += Jpl[1] * rp; acc[8] += Jpl[2] * rp;
+  // LM diagonal of the point columns: clamp(||J~[:,j]||^2)/radius   (Ceres LevenbergMarquardtStrategy)
+  const double ir = 1.0 / lm.radius;
+  acc[0] += fmin(fmax(acc[0], lm.min_diag), lm.max_diag) * ir;
+  acc[3] += fmin(fmax(acc[3], lm.min_diag), lm.max_diag) * ir;
+  acc[5] += fmin(fmax(acc[5], lm.min_diag), lm.max_diag) * ir;
+  double* p = params + kTrkParams * b;
+  sym3_inverse(acc, p);
+  p[6] = acc[6]; p[7] = acc[7]; p[8] = acc[8];
+  p[9] = p[0] * acc[6] + p[1] * acc[7] + p[2] * acc[8];
+  p[10] = p[1] * acc[6] + p[3] * acc[7] + p[4] * acc[8];
+  p[11] = p[2] * acc[6] + p[4] * acc[7] + p[5] * acc[8];
+  cost[b] = 0.5 * c;
+  gmax[b] = fmax(fabs(p[6] / sp[0]), fmax(fabs(p[7] / sp[1]), fabs(p[8] / sp[2])));
+}
+
 template <bool kLoss>
 struct TrackPass {             // one item per big landmark; cost[b] = 1/2 sum r^2 (kLoss: 1/2 sum rho), gmax[b] = max |g_p| (unscaled)
   VisualView vv; View bv; VisualState st; VisualLM lm; const double* obs; double* params; double* cost; double* gmax;
@@ -105,28 +136,7 @@ struct TrackPass {             // one item per big landmark; cost[b] = 1/2 sum r
       else c += f[kObR] * f[kObR] + f[kObR + 1] * f[kObR + 1];
       for (int q = 0; q < 9; ++q) acc[q] += f[kObStage + q];
     }
-    double rp, Jpl[3];
-    plane_eval(vv, vv.plane + 4 * k, X, rp, Jpl);
-    if constexpr (kLoss) c += plane_loss(vv, rp, Jpl);
-    else c += rp * rp;
-    const double* sp = lm.s_pt + 3 * k;
-    Jpl[0] *= sp[0]; Jpl[1] *= sp[1]; Jpl[2] *= sp[2];
-    acc[0] += Jpl[0] * Jpl[0]; acc[1] += Jpl[0] * Jpl[1]; acc[2] += Jpl[0] * Jpl[2];
-    acc[3] += Jpl[1] * Jpl[1]; acc[4] += Jpl[1] * Jpl[2]; acc[5] += Jpl[2] * Jpl[2];
-    acc[6] += Jpl[0] * rp; acc[7] += Jpl[1] * rp; acc[8] += Jpl[2] * rp;
-    // LM diagonal of the point columns: clamp(||J~[:,j]||^2)/radius   (Ceres LevenbergMarquardtStrategy)
-    const double ir = 1.0 / lm.radius;
-    acc[0] += fmin(fmax(acc[0], lm.min_diag), lm.max_diag) * ir;
-    acc[3] += fmin(fmax(acc[3], lm.min_diag), lm.max_diag) * ir;
-    acc[5] += fmin(fmax(acc[5], lm.min_diag), lm.max_diag) * ir;
-    double* p = params + kTrkParams * b;
-    sym3_inverse(acc, p);
-    p[6] = acc[6]; p[7] = acc[7]; p[8] = acc[8];
-    p[9] = p[0] * acc[6] + p[1] * acc[7] + p[2] * acc[8];
-    p[10] = p[1] * acc[6] + p[3] * acc[7] + p[4] * acc[8];
-    p[11] = p[2] * acc[6] + p[4] * acc[7] + p[5] * acc[8];
-    cost[b] = 0.5 * c;
-    gmax[b] = fmax(fabs(p[6] / sp[0]), fmax(fabs(p[7] / sp[1]), fabs(p[8] / sp[2])));
+    landmark_step<kLoss>(vv, lm, k, X, acc, c, params, cost, gmax, b);
   }
 };
 
@@ -284,8 +294,10 @@ struct ColTrackPass {          // one item per big landmark: its three point col
 
 // one item per big landmark, after ObsPass / TrackPass at the same state and scale: out[4 b ..] = model-cost change, step^2,
 // x^2, 0
-template <bool kLoss>
-struct BacksubPass {
+// kStride: the doubles per observation record of obs (r, J_c and J_X at kObR, kObJc and kObJX): kObs for ObsPass' records
+// (BacksubPass), vimp::kRec for those of the matrix-free linearisation (visual_implicit.h)
+template <bool kLoss, int kStride>
+struct BacksubStridePass {
   VisualView vv; View bv; VisualState st; VisualLM lm; const double* obs; double* params; const double* y_cam;
   double* X_cand; double* pt_step; double* out;
   LVBA_BHD void operator()(int64_t b) const {
@@ -293,7 +305,7 @@ struct BacksubPass {
     const int64_t lo = vv.trk_ptr[k] - base, hi = vv.trk_ptr[k + 1] - base;
     double a0 = 0, a1 = 0, a2 = 0;
     for (int64_t i = lo; i < hi; ++i) {                 // E^T y_c = J_X^T (J_c y_c)
-      const double* f = obs + kObs * i;
+      const double* f = obs + kStride * i;
       double j0, j1;
       camera_part(f, vv.obs_row[base + i], j0, j1);
       const double* JX = f + kObJX;
@@ -316,7 +328,7 @@ struct BacksubPass {
     const double jy = Jpl[0] * d[0] + Jpl[1] * d[1] + Jpl[2] * d[2];   // J~ y = J (s o y)
     double model = -jy * (rp + 0.5 * jy);
     for (int64_t i = lo; i < hi; ++i) {
-      const double* f = obs + kObs * i;
+      const double* f = obs + kStride * i;
       double j0, j1;
       camera_part(f, vv.obs_row[base + i], j0, j1);
       const double* JX = f + kObJX;
@@ -359,6 +371,9 @@ struct CostPass {              // one item per big landmark: cost[b] = 1/2 (sum 
     else cost[b] = 0.5 * (c + rp * rp);
   }
 };
+
+template <bool kLoss>
+struct BacksubPass : BacksubStridePass<kLoss, kObs> {};
 
 using ColTrackF = ColTrackPass<false>;
 using BacksubF = BacksubPass<false>;

@@ -23,7 +23,8 @@
 // reads the word once per group; the iteration count and the bits do not depend on the group size.  Every dot product is a
 // fixed-order two-level sum (chunks of kChunk elements in index order, then the chunks in order), so, given S, the solve has the
 // same bits on every run.  The product q = A p is ProdF here; the device runs the warp-per-row visual_pcg_product_kernel
-// instead (visual_api.cuh), which agrees with it to rounding.
+// instead (visual_api.cuh), which agrees with it to rounding.  On a plan that chose the matrix-free product (visual_implicit.h)
+// solve_with takes that product and PrecDF, which reads the diagonal blocks that product's build makes instead of S.
 #pragma once
 #include "env_types.h"
 #include "lidar_big.h"     // LVBA_BHD
@@ -63,40 +64,52 @@ struct StartF {
   }
 };
 
+// out = (d + diag(dadd_r))^-1 of the symmetric 6x6 block d (read through its lower triangle) through its Cholesky factor;
+// false for a pivot that is not finite and > 0
+LVBA_BHD bool prec_block(const double* d, const double* dadd_r, double* out) {
+  double L[36], Li[36];
+  for (int i = 0; i < 36; ++i) { L[i] = 0.0; Li[i] = 0.0; }
+  bool ok = true;
+  for (int j = 0; j < 6; ++j) {
+    double v = sym(d, j, j) + dadd_r[j];
+    for (int m = 0; m < j; ++m) v -= L[j * 6 + m] * L[j * 6 + m];
+    if (!(v > 0.0 && v <= 1.7976931348623157e308)) { ok = false; v = 1.0; }
+    const double l = sqrt(v);
+    L[j * 6 + j] = l;
+    for (int i = j + 1; i < 6; ++i) {
+      double w = sym(d, i, j);
+      for (int m = 0; m < j; ++m) w -= L[i * 6 + m] * L[j * 6 + m];
+      L[i * 6 + j] = w / l;
+    }
+  }
+  for (int j = 0; j < 6; ++j)                          // Li = L^-1, column by column
+    for (int i = j; i < 6; ++i) {
+      double w = i == j ? 1.0 : 0.0;
+      for (int m = j; m < i; ++m) w -= L[i * 6 + m] * Li[m * 6 + j];
+      Li[i * 6 + j] = w / L[i * 6 + i];
+    }
+  for (int a = 0; a < 6; ++a)                          // L^-T L^-1
+    for (int b = 0; b < 6; ++b) {
+      double w = 0.0;
+      for (int m = a > b ? a : b; m < 6; ++m) w += Li[m * 6 + a] * Li[m * 6 + b];
+      out[a * 6 + b] = w;
+    }
+  return ok;
+}
+
 // minv[36 r] = (S_rr + diag(dadd_r))^-1 through its Cholesky factor; a pivot that is not finite and > 0 sets kBadPrec
 struct PrecF {
   EnvView e; const double* S; const double* dadd; double* minv; Ctl c;
   LVBA_BHD void operator()(int64_t r) const {
-    const double* d = S + 36 * (e.row_start[r] + (r - e.first[r]));
-    double L[36], Li[36];
-    for (int i = 0; i < 36; ++i) { L[i] = 0.0; Li[i] = 0.0; }
-    bool ok = true;
-    for (int j = 0; j < 6; ++j) {
-      double v = sym(d, j, j) + dadd[6 * r + j];
-      for (int m = 0; m < j; ++m) v -= L[j * 6 + m] * L[j * 6 + m];
-      if (!(v > 0.0 && v <= 1.7976931348623157e308)) { ok = false; v = 1.0; }
-      const double l = sqrt(v);
-      L[j * 6 + j] = l;
-      for (int i = j + 1; i < 6; ++i) {
-        double w = sym(d, i, j);
-        for (int m = 0; m < j; ++m) w -= L[i * 6 + m] * L[j * 6 + m];
-        L[i * 6 + j] = w / l;
-      }
-    }
-    for (int j = 0; j < 6; ++j)                          // Li = L^-1, column by column
-      for (int i = j; i < 6; ++i) {
-        double w = i == j ? 1.0 : 0.0;
-        for (int m = j; m < i; ++m) w -= L[i * 6 + m] * Li[m * 6 + j];
-        Li[i * 6 + j] = w / L[i * 6 + i];
-      }
-    double* out = minv + 36 * r;
-    for (int a = 0; a < 6; ++a)                          // L^-T L^-1
-      for (int b = 0; b < 6; ++b) {
-        double w = 0.0;
-        for (int m = a > b ? a : b; m < 6; ++m) w += Li[m * 6 + a] * Li[m * 6 + b];
-        out[a * 6 + b] = w;
-      }
-    if (!ok) c.si[kBadPrec] = 1;
+    if (!prec_block(S + 36 * (e.row_start[r] + (r - e.first[r])), dadd + 6 * r, minv + 36 * r)) c.si[kBadPrec] = 1;
+  }
+};
+
+// the same from the diagonal blocks D [n][36] of the matrix-free product (visual_implicit.h)
+struct PrecDF {
+  const double* D; const double* dadd; double* minv; Ctl c;
+  LVBA_BHD void operator()(int64_t r) const {
+    if (!prec_block(D + 36 * r, dadd + 6 * r, minv + 36 * r)) c.si[kBadPrec] = 1;
   }
 };
 
@@ -252,17 +265,18 @@ struct Bufs {
 };
 struct Params { double eta; int min_iter, max_iter; };
 
-// The whole solve of A x = b over n block rows.  prod(in, out) enqueues out = A in (a no-op once the solve is done).  The
-// status words come to the host once before the first iteration and once per kGroup iterations; si_host [kNInt] holds the
-// last copy, so after the return si_host[kIter] / [kTerm] / [kFail] describe the solve.
-template <class Exec, class Prod>
-int solve(Exec& ex, const EnvView& e, const double* S, const double* dadd, const double* b, double* x, const Bufs& B,
-          const Params& o, const Prod& prod, int* si_host, int64_t* d2h) {
-  const int64_t n = e.n, n6 = 6 * n, nch = chunks(n6);
+// The whole solve of A x = b over n block rows.  prec is the preconditioner's pass (PrecF or PrecDF, one item per row),
+// prod(in, out) enqueues out = A in (a no-op once the solve is done).  The status words come to the host once before the first
+// iteration and once per kGroup iterations; si_host [kNInt] holds the last copy, so after the return si_host[kIter] / [kTerm] /
+// [kFail] describe the solve.
+template <class Exec, class Prec, class Prod>
+int solve_with(Exec& ex, int64_t n, const Prec& prec, const double* b, double* x, const Bufs& B, const Params& o, const Prod& prod,
+               int* si_host, int64_t* d2h) {
+  const int64_t n6 = 6 * n, nch = chunks(n6);
   const Ctl& c = B.c;
   int rc;
   if ((rc = ex.for_each(1, StartF{c}))) return rc;
-  if ((rc = ex.for_each(n, PrecF{e, S, dadd, B.minv, c}))) return rc;
+  if ((rc = ex.for_each(n, prec))) return rc;
   if ((rc = ex.for_each(n6, InitF{b, x, B.r}))) return rc;
   if ((rc = ex.for_each(nch, DotF{c, n6, b, b, nullptr, true}))) return rc;
   if ((rc = ex.for_each(1, CheckF{c, nch}))) return rc;
@@ -290,6 +304,13 @@ int solve(Exec& ex, const EnvView& e, const double* S, const double* dadd, const
     }
   }
   return 0;
+}
+
+// the solve on the explicit S in envelope storage
+template <class Exec, class Prod>
+int solve(Exec& ex, const EnvView& e, const double* S, const double* dadd, const double* b, double* x, const Bufs& B,
+          const Params& o, const Prod& prod, int* si_host, int64_t* d2h) {
+  return solve_with(ex, e.n, PrecF{e, S, dadd, B.minv, B.c}, b, x, B, o, prod, si_host, d2h);
 }
 
 }  // namespace vpcg

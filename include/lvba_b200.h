@@ -351,6 +351,8 @@ int lvba_visual_step(lvba_visual_problem* p, double radius, int32_t jacobi_scali
 /* Reduced camera system of the last lvba_visual_step: block structure + values + rhs (for parity tests). */
 int lvba_visual_structure(lvba_visual_problem* p, int32_t* n_active, int32_t* cam_of_row /* [n_active] */,
                           int64_t* nblocks, int32_t* brow, int32_t* bcol);
+/* After a pass of ITERATIVE_SCHUR on the matrix-free product (lvba_visual_schur_product) there is no S: a call with blocks !=
+ * NULL returns LVBA_ERR_UNSUPPORTED and writes nothing; with blocks == NULL it writes rhs as after any pass. */
 int lvba_visual_get_system(lvba_visual_problem* p, double* rhs /* [n_active*6] */, double* blocks /* [nblocks*36] */);
 int lvba_visual_reset_lm(lvba_visual_problem* p, const lvba_visual_opts* opts);
 /* restore q, t, X and the intrinsics passed to lvba_visual_create (device-to-device) */
@@ -372,6 +374,17 @@ int lvba_visual_get_intrinsics_system(lvba_visual_problem* p, int32_t* k, double
  * lvba_visual_reset_lm or removal; cg_iters_last and term_last, the iteration count and termination of the last solve
  * (0 SUCCESS, 1 NO_CONVERGENCE, 2 FAILURE).  All zero until a solve has run.  Any pointer may be NULL. */
 int lvba_visual_linear_stats(lvba_visual_problem* p, int64_t* cg_iters_total, int32_t* cg_iters_last, int32_t* term_last);
+/* The product ITERATIVE_SCHUR runs its conjugate gradients on, chosen for the handle's plan from its structure at create and at
+ * every re-plan (a new cam_fixed, a removal), whatever the linear solver: *matrix_free = 0 for the explicit reduced camera
+ * system S in envelope storage, 1 for the matrix-free product through the Jacobian blocks, which never forms S.  The
+ * matrix-free product costs O(observations) per product where the explicit S costs O(sum of squared track lengths) to build:
+ * long tracks and loop closures take it.  The two are the same algorithm (the same CG on the same S + D, with sums in another
+ * order); DENSE_SCHUR always builds S. */
+int lvba_visual_schur_product(lvba_visual_problem* p, int32_t* matrix_free);
+/* y = (S + D) x [n_active*6] for the damped reduced camera system of the last lvba_visual_step or iteration, through the product
+ * its conjugate gradients used (for parity tests).  LVBA_ERR_INVALID_ARG unless that pass ran ITERATIVE_SCHUR: before any pass,
+ * after lvba_visual_reset_lm or a re-plan, and under DENSE_SCHUR. */
+int lvba_visual_apply_system(lvba_visual_problem* p, const double* x, double* y);
 int lvba_visual_iterate(lvba_visual_problem* p, int32_t n_iter, lvba_summary* summary);
 int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_valid_tracks,
                        int64_t* n_blocks_env, int64_t* n_pairs);
