@@ -256,7 +256,7 @@ def system(lin, cam_row, radius=1e4, scaling=True, loss_px=None, loss_pl=None, m
     one = mpf(1)
     s_cam = [[one / (1 + mp.sqrt(c)) if scaling else one for c in row] for row in colsq]
     lms = [_landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag) for L in lin]
-    return dict(n_rows=n_rows, s_cam=s_cam, lm=lms, cam_row=cam_row)
+    return dict(n_rows=n_rows, s_cam=s_cam, lm=lms, cam_row=cam_row, radius=radius, min_diag=min_diag, max_diag=max_diag)
 
 
 def _landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag):
@@ -289,6 +289,7 @@ def _landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag):
     ix = {x: i for i, x in enumerate(urows)}
     R = len(urows)
     U = [[[mpf(0)] * 6 for _ in range(6)] for _ in range(R)]
+    csq = [[mpf(0)] * 6 for _ in range(R)]
     W = [[[mpf(0)] * 3 for _ in range(6)] for _ in range(R)]
     gc = [[mpf(0)] * 6 for _ in range(R)]
     for k in range(K):
@@ -299,6 +300,7 @@ def _landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag):
             jc, jx = Jc[k][a], JX[k][a]
             for c in range(6):
                 gc[i][c] += jc[c] * r[k][a]
+                csq[i][c] += jc[c] * jc[c]
                 for d in range(6):
                     U[i][c][d] += jc[c] * jc[d]
                 for m in range(3):
@@ -330,11 +332,12 @@ def _landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag):
     ECi = VCi @ EC @ VCi
     Vgp = sum((VX[k].T @ Vr[k] for k in range(K)), np.zeros(3)) + Vp * Vrp
     Egp = sum((EX[k].T @ Vr[k] + VX[k].T @ Er[k] for k in range(K)), np.zeros(3)) + Ep * Vrp + Vp * Erp
-    EU = np.zeros((R, 6, 6)); VW = np.zeros((R, 6, 3)); EW = np.zeros((R, 6, 3)); Egc = np.zeros((R, 6))
+    EU = np.zeros((R, 6, 6)); VU = np.zeros((R, 6, 6)); VW = np.zeros((R, 6, 3)); EW = np.zeros((R, 6, 3)); Egc = np.zeros((R, 6))
     for k in range(K):
         if rows[k] >= 0:
             i = ix[rows[k]]
             EU[i] += Ec[k].T @ Vc[k] + Vc[k].T @ Ec[k]
+            VU[i] += Vc[k].T @ Vc[k]
             VW[i] += Vc[k].T @ VX[k]; EW[i] += Ec[k].T @ VX[k] + Vc[k].T @ EX[k]
             Egc[i] += Ec[k].T @ Vr[k] + Vc[k].T @ Er[k]
     VY = VW @ VCi
@@ -342,6 +345,9 @@ def _landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag):
     pair_e = (np.einsum("icm,jdm->ijcd", EY, VW) + np.einsum("icm,jdm->ijcd", VY, EW)).max(axis=(2, 3)) if R else np.zeros((0, 0))
     Sh = {(urows[i], urows[j]): pair_e[i, j] + (EU[i].max() if i == j else 0.0) for i in range(R) for j in range(i + 1)}
     rhsh = [(Egc[i] + EY[i] @ Vgp + VY[i] @ Egp).max() for i in range(R)]
+    # the term scale of every entry: sum |J_c|^T |J_c| (diagonal blocks) + sum_o |E_o| |C^-1| sum_o |E_o|^T
+    Tp = np.einsum("icm,jdm->ijcd", VY, VW) if R else np.zeros((0, 0, 6, 6))
+    Tl = {(urows[i], urows[j]): Tp[i, j] + (VU[i] if i == j else 0.0) for i in range(R) for j in range(i + 1)}
     S = {(urows[i], urows[i]): diag[i] for i in range(R)}
     for (i, j), blk in off.items():
         S[(urows[i], urows[j])] = blk
@@ -349,7 +355,8 @@ def _landmark(L, cam_row, s_cam, radius, scaling, min_diag, max_diag):
     costh = sum(w[k] * float(abs(obs[k]["r"][a])) * Er[k][a] for k in range(K) for a in range(2)) \
         + float(P["w"] * abs(P["r"])) * Erp + float(abs(cost))
     kappa = float(VC.sum(1).max() * VCi.sum(1).max())
-    return dict(track=L["track"], rows=rows, urows=urows, S=S, S_hat=Sh, rhs=dict(zip(urows, rhs)), rhs_hat=dict(zip(urows, rhsh)),
+    return dict(track=L["track"], rows=rows, urows=urows, S=S, S_hat=Sh, T=Tl, csq=dict(zip(urows, csq)),
+                csq_hat=dict(zip(urows, (np.diag(EU[i]) for i in range(R)))), rhs=dict(zip(urows, rhs)), rhs_hat=dict(zip(urows, rhsh)),
                 cost=float(cost / 2), cost_hat=costh, kappa=kappa, amp=max([float(o["amp"]) for o in obs] + [1.0]),
                 z_min=min([float(o["z"]) for o in obs]), e=float(P["e"]), C=np.array([[float(x) for x in row] for row in C]), s_pt=s_pt, Ci=Ci, gp=gp, JX=JX, r=r, Jps=Jps, rp=rp,
                 V=dict(X=VX, r=Vr, p=Vp, rp=Vrp, Ci=VCi, gp=Vgp), E=dict(X=EX, r=Er, p=Ep, rp=Erp, Ci=ECi, gp=Egp),
@@ -418,6 +425,93 @@ def assemble(sysm, lms=None):
             rhs[i] += v; rhsh[i] += L["rhs_hat"][i]; touched[i] = True
     return dict(S=S, S_hat=Sh, rhs=rhs, rhs_hat=rhsh, rows=touched, cost=math.fsum(L["cost"] for L in lms),
                 cost_hat=math.fsum(L["cost_hat"] for L in lms))
+
+
+def damped(sysm, lms=None):
+    """The damped operator A = S + diag(dadd) that ITERATIVE_SCHUR applies, summed over the landmarks `lms` (default: all), as
+    full 6x6 blocks in both triangles (A_ji = A_ij^T): dadd = clamp(sum J~_c^2, min_diag, max_diag) / radius per camera column
+    (visual_cam_diag_kernel), each block with its error scale, and T, the sum of the absolute values of the terms of every
+    entry (sum |J_c|^T |J_c| on the diagonal blocks, plus dadd, plus sum_l |W_il| |C_l^-1| |W_jl|^T, |W_il| = sum_o |E_o|).
+    Returns dict(S, S_hat, T) keyed (i, j) over both triangles, so that ratios(damped(...), A_block) applies, and dadd,
+    dadd_hat [n_rows, 6]."""
+    lms = sysm["lm"] if lms is None else lms
+    ref = assemble(sysm, lms)
+    n = sysm["n_rows"]
+    csq = {}; csqh = np.zeros((n, 6))
+    T = {}
+    for L in lms:
+        for i, v in L["csq"].items():
+            c = csq.setdefault(i, [mpf(0)] * 6)
+            for a in range(6):
+                c[a] += v[a]
+            csqh[i] += L["csq_hat"][i]
+        for k, b in L["T"].items():
+            T[k] = T.get(k, 0.0) + b
+    rad, lo, hi = mpf(float(sysm["radius"])), mpf(float(sysm["min_diag"])), mpf(float(sysm["max_diag"]))
+    dadd = np.zeros((n, 6)); daddh = np.zeros((n, 6))
+    for i, c in csq.items():
+        for a in range(6):
+            dadd[i, a] = float(min(max(c[a], lo), hi) / rad)
+            daddh[i, a] = (csqh[i, a] / float(rad) if lo < c[a] < hi else 0.0) + dadd[i, a]
+    A, Ah, At = {}, {}, {}
+    for (i, j), b in ref["S"].items():
+        if i == j:
+            A[(i, i)] = b + np.diag(dadd[i])
+            Ah[(i, i)] = ref["S_hat"][(i, i)] + daddh[i].max()
+            At[(i, i)] = T[(i, i)] + np.diag(dadd[i])
+        else:
+            A[(i, j)], A[(j, i)] = b, b.T
+            Ah[(i, j)] = Ah[(j, i)] = ref["S_hat"][(i, j)]
+            At[(i, j)], At[(j, i)] = T[(i, j)], T[(i, j)].T
+    return dict(S=A, S_hat=Ah, T=At, dadd=dadd, dadd_hat=daddh)
+
+
+def dense(blocks, n):
+    """{(i, j): 6x6} -> the [6n, 6n] matrix"""
+    M = np.zeros((6 * n, 6 * n))
+    for (i, j), b in blocks.items():
+        M[6 * i:6 * i + 6, 6 * j:6 * j + 6] = b
+    return M
+
+
+# The symmetry bound of an operator applied through the Jacobian blocks in double-double (visual_implicit.h, vimp::DD): each
+# entry is the exact operator of the rounded records, which is symmetric, rounded once, so that
+#   |A_ij - A_ji| <= ulp(max(|A_ij|, |A_ji|)) + C_SYM eps^2 T_ij
+# with T_ij the sum of the absolute values of the entry's terms (damped(), term_scale_f64()).  A product rounded in plain
+# double misses it by the cancellation in its terms, ~eps T_ij.
+C_SYM = 64.0
+
+
+def symmetry_ratio(A, T):
+    """max over the off-diagonal entries of |A_ij - A_ji| / (ulp(max(|A_ij|, |A_ji|)) + C_SYM eps^2 T_ij), for the dense
+    operator A and its term scale T (a ratio <= 1 meets the bound); NaN anywhere gives NaN"""
+    d = np.abs(A - A.T)
+    bound = np.spacing(np.maximum(np.abs(A), np.abs(A.T))) + C_SYM * EPS * EPS * np.maximum(T, T.T)
+    np.fill_diagonal(d, 0.0)
+    return float(np.max(d / bound)) if d.size else 0.0
+
+
+def term_scale_f64(prob, radius=1e4, scaling=True, min_diag=1e-6, max_diag=1e32):
+    """T of damped() in float64, from the absolute values of the float64 oracle's Jacobian (visual_oracle.VisualProblem or
+    visual_loss_oracle.RobustProblem: corrected with a loss): |J_c|^T |J_c| + diag(dadd) + |E| |C^-1| |E|^T, with E per
+    observation as |J_c|^T |J_X| and C the damped point blocks.  For scenes too large for the 50-digit linearisation; T is
+    needed to its order of magnitude only.  Returns the dense [6 nc, 6 nc] matrix."""
+    import scipy.sparse as sp
+    res, J = prob.residuals(jac=True)
+    scale = 1.0 / (1.0 + np.sqrt(np.asarray(J.multiply(J).sum(0)).ravel())) if scaling else np.ones(prob.ncols)
+    Js = (J @ sp.diags(scale)).tocsc()
+    nc6 = 6 * prob.nc
+    diag = np.clip(np.asarray(Js.multiply(Js).sum(0)).ravel(), min_diag, max_diag) / radius
+    Jc, Jp = abs(Js[:, :nc6]), Js[:, nc6:]
+    CC = (Jp.T @ Jp).tocoo()                                  # block diagonal: a residual row touches one landmark
+    Cb = np.zeros((prob.npt, 3, 3))
+    np.add.at(Cb, (CC.row // 3, CC.row % 3, CC.col % 3), CC.data)
+    Cb += np.einsum("la,ab->lab", diag[nc6:].reshape(-1, 3), np.eye(3))
+    Ci = np.abs(np.linalg.inv(Cb)) if prob.npt else Cb
+    E = (Jc.T @ abs(Jp)).tocsc()
+    Cib = sp.block_diag(list(Ci), format="csc")
+    T = (Jc.T @ Jc).toarray() + np.diag(diag[:nc6]) + (E @ Cib @ E.T).toarray()
+    return T
 
 
 def ratios(ref, S_block=None, rhs=None, cost=None):

@@ -12,6 +12,12 @@ is labelled with its class:
   cancel    cameras that see only one or two landmarks, so that U - W C^-1 W^T nearly cancels
   big       far / pair geometry with 128 observations (the tile path) and with 129 and 300 (visual_big.h)
   ordinary  3 - 5 views at 5 - 20 m (a reference point for the others)
+  repeat    a far facade at a grazing angle that one camera sees two or three times (not in CLASSES: isolated(classes=...)
+            adds it), so that the repeated views' terms, which nearly cancel, are summed as one run of the camera's row
+
+`ballast` adds a few long tracks on cameras of their own, every camera seen several times, so that the matrix-free product
+(visual_implicit.h) sums RowPartF runs on long tracks, without touching the cameras of any other class.  (The rule moves every
+problem of the family to the matrix-free product with or without them; `EXPLICIT` ballast holds a problem on the explicit S.)
 
 and problems of their own for what is global to a problem: `distort` (large k1 k2 p1 p2, landmarks near the corners, where the
 radial factor approaches 0), `huber_edge` (reprojection s within a few ulps of a^2 on both sides, a = 1.7, and far beyond) and
@@ -25,6 +31,7 @@ from oracle import visual_mp as vm
 
 BASE = np.array([[1.0, 0.0, 0.0], [0.0, 0.0, -1.0], [0.0, 1.0, 0.0]])      # camera z = world +y, camera x = world +x
 CLASSES = ("ordinary", "far", "pair", "rotation", "near_z", "plane0", "offset", "cancel")
+REPEAT = CLASSES + ("repeat",)
 
 
 class _Scene:
@@ -137,18 +144,24 @@ def _add_class(S, cls, i, cams=None, x0=0.0):
         cl = street(4, offset=off) if cams is None else cams[:4]
         X = S.at(cl[0], rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3), 20.0)
         S.track(cl, X, cls)
+    elif cls == "repeat":
+        D = 10.0 ** (2 + 3 * (i % 4) / 3)                   # 1e2 .. 1e5 m
+        cl = street(5)
+        X = S.at(cl[2], rng.uniform(-0.1, 0.1), rng.uniform(-0.1, 0.1), D)
+        ray = X - np.mean([S.c[k] for k in cl], 0)
+        S.track(cl + [cl[1]] * (1 + i % 2), X, cls, normal=_perp(ray / np.linalg.norm(ray), rng))
     elif cls == "cancel":
         cl = street(2)
         for k in range(1 + i % 2):
             S.track(cl, S.at(cl[0], rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3), 12.0), cls)
 
 
-def isolated(per_class=6, seed=7):
+def isolated(per_class=6, seed=7, classes=CLASSES):
     """every landmark on cameras of its own (the offset landmarks' cameras translated with them), so that every S block and
-    rhs row belongs to one class"""
+    rhs row belongs to one class; classes=REPEAT adds the repeat class after the others (the rest unchanged)"""
     S = _Scene(seed)
     x0 = 0.0
-    for cls in CLASSES:
+    for cls in classes:
         for i in range(per_class):
             _add_class(S, cls, i, x0=x0)
             x0 += 10.0
@@ -264,3 +277,42 @@ def cauchy_far(seed=41, a=0.05):
         p["obs_uv"][k] += np.float32(10.0 ** (-1 + 3.9 * i / 15))
     p["loss_px"], p["loss_pl"] = (vm.CAUCHY, a), (vm.CAUCHY, 0.5)
     return p
+
+
+def ballast(p, n_tracks=2, n_cams=20, views=3, seed=99, one_street=False):
+    """p with n_tracks ordinary landmarks 20 m deep appended, each on n_cams new cameras of its own (a street 0.5 m apart, 5 km
+    from the origin along x) and seeing each of them `views` times, n_cams views apart (class "ballast").  The new cameras and
+    landmarks come after p's, so every other camera keeps its index and its system row.  one_street: every track on the same
+    n_cams new cameras (many short tracks on a few cameras hold a problem under the rule, on the explicit S)."""
+    rng = np.random.Generator(np.random.Philox(key=seed))
+    S = _Scene(seed)
+    S.rng = rng
+    q, t, X, Xg = [p["q"]], [p["t"]], [p["X"]], [p["X_gt"]]
+    planes, obs_cam, obs_uv = [p["plane_nd"]], [p["obs_cam"]], [p["obs_uv"]]
+    M = len(p["q"])
+    for k in range(n_tracks):
+        cl = S.street(-5e3 + 50.0 * k, n_cams) if not (one_street and k) else cl
+        Xk = S.at(cl[n_cams // 2], rng.uniform(-0.2, 0.2), rng.uniform(-0.2, 0.2), 20.0)
+        cams = np.tile(np.asarray(cl), views)
+        R = np.array([S.R[c] for c in cams]); tt = -np.einsum("nij,nj->ni", R, np.array([S.c[c] for c in cams]))
+        uv, _ = synth.project(R, tt, np.repeat(Xk[None], len(cams), 0), p["intr"])
+        obs_uv.append((uv + rng.normal(0, 0.5, uv.shape)).astype(np.float32))
+        obs_cam.append((M + cams).astype(np.int32))
+        n = rng.normal(size=3); n /= np.linalg.norm(n)
+        planes.append(np.array([[*n, -n @ Xk]]))
+        X.append((Xk + rng.normal(0, 0.05, 3))[None]); Xg.append(Xk[None])
+    Rb = np.array(S.R); tb = -np.einsum("nij,nj->ni", Rb, np.array(S.c))
+    q.append(synth.rot_to_quat_wxyz(Rb)); t.append(tb)
+    out = dict(p)
+    K = [len(c) for c in obs_cam[1:]]
+    out.update(q=np.concatenate(q), t=np.concatenate(t), X=np.concatenate(X), X_gt=np.concatenate(Xg),
+               plane_nd=np.concatenate(planes), obs_cam=np.concatenate(obs_cam).astype(np.int32),
+               obs_uv=np.concatenate(obs_uv).astype(np.float32),
+               obs_ptr=np.concatenate([p["obs_ptr"], p["obs_ptr"][-1] + np.cumsum(K)]).astype(np.int64),
+               cls=np.concatenate([p["cls"], np.array(["ballast"] * n_tracks)]))
+    out.pop("lin", None)
+    return out
+
+
+# ballast() arguments that keep a problem of the family on the explicit S: 400 three-view tracks on three cameras
+EXPLICIT = dict(n_tracks=400, n_cams=3, views=1, one_street=True)
