@@ -37,7 +37,7 @@ EXPORTS = [
     "lvba_visual_get_system", "lvba_visual_reset_lm", "lvba_visual_reset_state", "lvba_visual_iterate", "lvba_visual_counts",
     "lvba_visual_big_counts", "lvba_visual_obs_residuals", "lvba_visual_remove_observations", "lvba_visual_remove_outliers",
     "lvba_visual_get_intrinsics", "lvba_visual_set_intrinsics", "lvba_visual_get_intrinsics_system", "lvba_visual_linear_stats",
-    "lvba_visual_schur_product", "lvba_visual_apply_system",
+    "lvba_visual_schur_product", "lvba_visual_apply_system", "lvba_visual_dogleg_state",
     "lvba_voxel_default_opts", "lvba_voxel_map_create", "lvba_voxel_map_create_windows", "lvba_voxel_map_windows",
     "lvba_voxel_map_lidar_lm_batch", "lvba_voxel_map_summary", "lvba_voxel_map_export",
     "lvba_voxel_map_lookup", "lvba_voxel_map_lidar_create", "lvba_voxel_map_lidar_lm", "lvba_voxel_map_destroy",
@@ -74,6 +74,7 @@ class VisualOpts(C.Structure):
                 ("reproj_loss", C.c_int32), ("reproj_loss_scale", C.c_double),
                 ("plane_loss", C.c_int32), ("plane_loss_scale", C.c_double),
                 ("linear_solver", C.c_int32), ("eta", C.c_double), ("min_linear_iter", C.c_int32), ("max_linear_iter", C.c_int32),
+                ("trust_region_strategy", C.c_int32),
                 ("cam_fixed", C.POINTER(C.c_uint8))]
 
 
@@ -81,6 +82,10 @@ class VisualOpts(C.Structure):
 LINEAR_DENSE_SCHUR, LINEAR_ITERATIVE_SCHUR = 0, 1
 # the termination of one conjugate-gradients solve (VisualProblem.linear_stats)
 CG_SUCCESS, CG_NO_CONVERGENCE, CG_FAILURE = 0, 1, 2
+# lvba_trust_region: the trust-region strategy (VisualOpts.trust_region_strategy)
+TR_LEVENBERG_MARQUARDT, TR_DOGLEG = 0, 1
+# lvba_dogleg_case: the step of the last dogleg pass (VisualProblem.dogleg_state)
+DOGLEG_NONE, DOGLEG_GAUSS_NEWTON, DOGLEG_CAUCHY, DOGLEG_INTERPOLATED = 0, 1, 2, 3
 
 # lvba_visual_opts::refine_intrinsics: bit i frees intr[i] of (fx fy cx cy k1 k2 p1 p2)
 INTR_FOCAL, INTR_PRINCIPAL, INTR_DISTORTION = 0x03, 0x0C, 0xF0
@@ -419,10 +424,12 @@ def _with_cam_fixed(opts, cam_fixed, M):
     return o, m
 
 
-def _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter):
-    """opts (None: the defaults) with those of the linear-solver fields that are not None set (lvba_visual_opts::linear_solver,
-    eta, min_linear_iter, max_linear_iter); opts as they are when all four are None."""
-    kw = dict(linear_solver=linear_solver, eta=eta, min_linear_iter=min_linear_iter, max_linear_iter=max_linear_iter)
+def _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter, trust_region_strategy=None):
+    """opts (None: the defaults) with those of the linear-solver and trust-region fields that are not None set
+    (lvba_visual_opts::linear_solver, eta, min_linear_iter, max_linear_iter, trust_region_strategy); opts as they are when all
+    are None."""
+    kw = dict(linear_solver=linear_solver, eta=eta, min_linear_iter=min_linear_iter, max_linear_iter=max_linear_iter,
+              trust_region_strategy=trust_region_strategy)
     if all(v is None for v in kw.values()):
         return opts
     o = visual_default_opts() if opts is None else VisualOpts.from_buffer_copy(opts)
@@ -433,12 +440,13 @@ def _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter):
 
 
 def visual_lm(q, t, X, plane_nd, obs_ptr, obs_cam, obs_uv, intr, sigma_px, sigma_plane, fixed_cam=0, opts=None, cam_fixed=None,
-              linear_solver=None, eta=None, min_linear_iter=None, max_linear_iter=None):
+              linear_solver=None, eta=None, min_linear_iter=None, max_linear_iter=None, trust_region_strategy=None):
     """One-shot drop-in for the Ceres block of optimizeCameraPoses (lvba_system.cpp:1571-1656).  cam_fixed: boolean mask
     [M] of further constant cameras (lvba_visual_opts::cam_fixed), or None.  linear_solver (LINEAR_*), eta, min_linear_iter,
-    max_linear_iter: the solver of the reduced camera system, None for what opts says."""
+    max_linear_iter: the solver of the reduced camera system, trust_region_strategy (TR_*): LM or dogleg; None for what opts
+    says."""
     lib = load_library()
-    opts = _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter)
+    opts = _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter, trust_region_strategy)
     q = _f64(q).copy(); t = _f64(t).copy(); X = _f64(X).copy(); pl = _f64(plane_nd)
     op = np.ascontiguousarray(obs_ptr, np.int64); oc = np.ascontiguousarray(obs_cam, np.int32)
     uv = np.ascontiguousarray(obs_uv, np.float32); it = _f64(intr)
@@ -511,12 +519,13 @@ class VisualProblem:
         return cam, rhs, br, bc, blocks
 
     def reset_lm(self, opts=None, cam_fixed=None, refine_intrinsics=None, linear_solver=None, eta=None, min_linear_iter=None,
-                 max_linear_iter=None):
+                 max_linear_iter=None, trust_region_strategy=None):
         """lvba_visual_reset_lm; cam_fixed: boolean mask [M] of further constant cameras (a mask that differs from the
         handle's re-plans it), or None for what opts.cam_fixed says; refine_intrinsics: the mask of free intrinsics
         (INTR_* bits), or None for what opts.refine_intrinsics says; linear_solver (LINEAR_*), eta, min_linear_iter,
-        max_linear_iter: the solver of the reduced camera system, None for what opts says."""
-        opts = _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter)
+        max_linear_iter: the solver of the reduced camera system, trust_region_strategy (TR_*): LM or dogleg; None for what
+        opts says."""
+        opts = _with_linear(opts, linear_solver, eta, min_linear_iter, max_linear_iter, trust_region_strategy)
         opts, mask = _with_cam_fixed(opts, cam_fixed, self.M)
         if refine_intrinsics is not None:
             opts = visual_default_opts() if opts is None else VisualOpts.from_buffer_copy(opts)
@@ -553,6 +562,15 @@ class VisualProblem:
         a, b, c = C.c_int64(), C.c_int32(), C.c_int32()
         _chk(self._lib.lvba_visual_linear_stats(self._h, C.byref(a), C.byref(b), C.byref(c)))
         return dict(cg_iters_total=a.value, cg_iters_last=b.value, term_last=c.value)
+
+    def dogleg_state(self):
+        """lvba_visual_dogleg_state: dict(radius, mu, alpha, grad_norm, gn_norm, case (DOGLEG_*), reused (passes since the
+        last reset_lm or removal that reused a linearisation)).  LvbaError unless the last reset_lm chose TR_DOGLEG."""
+        d = [C.c_double() for _ in range(5)]
+        c, r = C.c_int32(), C.c_int64()
+        _chk(self._lib.lvba_visual_dogleg_state(self._h, *[C.byref(v) for v in d], C.byref(c), C.byref(r)))
+        return dict(radius=d[0].value, mu=d[1].value, alpha=d[2].value, grad_norm=d[3].value, gn_norm=d[4].value, case=c.value,
+                    reused=r.value)
 
     def schur_product(self):
         """lvba_visual_schur_product: 1 when ITERATIVE_SCHUR runs on the matrix-free product for this plan, 0 on the explicit S."""

@@ -8,22 +8,30 @@
 #include "exec.cuh"
 #include "runtime.cuh"   // (pulls comm.cuh in)
 #include "visual.cuh"
+#include "visual_dogleg.h"
 #include "visual_outliers.h"
 #include "visual_implicit.h"
 #include "visual_pcg.h"
 #include "visual_plan.h"
 
 namespace lvba {
-// the trust-region state of one solve (Ceres TrustRegionMinimizer + LevenbergMarquardtStrategy)
+// the trust-region state of one solve (Ceres TrustRegionMinimizer + LevenbergMarquardtStrategy, or DoglegStrategy)
 struct TrustRegionState {
   double radius = 1e4, nu = 2.0, cost = 0.0, cost_first = 0.0;
   bool have_scale = false, have_first = false, converged = false;
   int iters = 0, accepted = 0, builds = 0, invalid = 0, termination = LVBA_TERM_MAX_ITER;
+  // DOGLEG (visual_dogleg.h): mu, whether the next pass reuses the linearisation, the passes that did since the reset, and
+  // alpha, |g|, |GN|, the case and |s| of the last step (lvba_visual_dogleg_state)
+  double mu = vdog::kMinMu, alpha = 0.0, grad_norm = 0.0, gn_norm = 0.0, dl_norm = 0.0;
+  bool reuse = false;
+  int dl_case = vdog::kNone;
+  int64_t reused = 0;
   // a new solve from the options; cost and cost_first keep their values until its first pass sets them
   void reset(const lvba_visual_opts& o) {
     radius = o.initial_radius; nu = 2.0;
     have_scale = have_first = converged = false;
     iters = accepted = builds = invalid = 0; termination = LVBA_TERM_MAX_ITER;
+    mu = vdog::kMinMu; alpha = grad_norm = gn_norm = dl_norm = 0.0; reuse = false; dl_case = vdog::kNone; reused = 0;
   }
 };
 }  // namespace lvba
@@ -108,6 +116,12 @@ struct lvba_visual_problem {
   lvba::DevBuf<double> imp_rec, imp_params, imp_cost, imp_gmax, imp_u, imp_part, imp_D;
   lvba::DevBuf<int> imp_zero;                       // an int 0: the "done" word of a product outside a solve
   bool implicit_pass() const { return iterative() && matrix_free; }
+  // ---- DOGLEG (lvba_visual_opts::trust_region_strategy, visual_dogleg.h): D, g, GN, the step v, the per-entry and
+  // per-landmark terms, the sums' partials and the device scalars (vdog::Bufs), set up when a dogleg pass first needs them, and
+  // the host copy of the scalars after a pass
+  lvba::DevBuf<double> dl_buf;
+  double h_dl[lvba::vdog::kNScal] = {};
+  bool dogleg() const { return opts.trust_region_strategy == LVBA_TR_DOGLEG; }
   // LM state
   lvba_visual_opts opts;
   lvba::TrustRegionState lm;
@@ -536,6 +550,19 @@ inline int visual_check_linear(const lvba_visual_opts& o) {
   return LVBA_OK;
 }
 
+// the trust-region strategy of lvba_visual_opts: a known one; DOGLEG needs the exact Gauss-Newton step of DENSE_SCHUR and runs
+// without the intrinsics block, on one GPU (checked before any device work)
+inline int visual_check_trust(const lvba_visual_opts& o) {
+  if (o.trust_region_strategy != LVBA_TR_LEVENBERG_MARQUARDT && o.trust_region_strategy != LVBA_TR_DOGLEG)
+    return fail(LVBA_ERR_INVALID_ARG, "trust_region_strategy = %d is not an lvba_trust_region", (int)o.trust_region_strategy);
+  if (o.trust_region_strategy != LVBA_TR_DOGLEG) return LVBA_OK;
+  if (o.linear_solver == LVBA_LINEAR_ITERATIVE_SCHUR)
+    return fail(LVBA_ERR_INVALID_ARG, "DOGLEG needs an exact Gauss-Newton step: not with ITERATIVE_SCHUR");
+  if (o.refine_intrinsics) return fail(LVBA_ERR_UNSUPPORTED, "DOGLEG does not solve the intrinsics block: refine_intrinsics needs the LM");
+  if (comm().active()) return fail(LVBA_ERR_UNSUPPORTED, "DOGLEG runs on one GPU: not with an active communicator");
+  return LVBA_OK;
+}
+
 // a handle whose failed re-plan could not be undone (visual_replan) takes no further calls but destroy and the state copies
 inline int visual_check_usable(const lvba_visual_problem* P) {
   if (P->unusable) return fail(LVBA_ERR_INVALID_ARG, "this handle lost its plan in a failed lvba_visual_reset_lm: destroy it");
@@ -560,6 +587,7 @@ inline void visual_intr_forget(lvba_visual_problem* P) {
 inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   LVBA_TRY(visual_check_loss(o));
   LVBA_TRY(visual_check_linear(o));
+  LVBA_TRY(visual_check_trust(o));
   if (o.refine_intrinsics >> 8)
     return fail(LVBA_ERR_INVALID_ARG, "refine_intrinsics = 0x%x: only bits 0..7 name intrinsics", (unsigned)o.refine_intrinsics);
   if (o.refine_intrinsics && comm().active())
@@ -588,6 +616,10 @@ inline int visual_set_mode(lvba_visual_problem* P, const lvba_visual_opts& o) {
   visual_intr_forget(P);
   return LVBA_OK;
 }
+
+// The dogleg's linearisation (D, g, alpha, GN and the cost it was taken at) belongs to the state, the intrinsics and the Jacobi
+// scale of its pass: a call that changes any of them makes the next dogleg pass linearise again
+inline void visual_dogleg_forget(lvba_visual_problem* P) { P->lm.reuse = false; }
 
 // ---------------------------------------------------------------- the row CSR
 // The observations of every camera row in ascending order (row_ptr / row_obs), for the current plan: the border gather of the
@@ -937,7 +969,7 @@ inline int visual_pcg_solve(lvba_visual_problem* P) {
 // scal layout: [0] cost  [1] gmax  [2] model  [3] step^2 (pts)  [4] x^2 (pts)  [5] -  [6] step^2 (cams) [7] x^2 (cams)
 //              [8] candidate cost
 template <bool kLoss>
-inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool want_steps) {
+inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool want_steps, bool cand) {
   cudaStream_t s = P->stream;
   const VisualLM lm = visual_lm_params(P, radius);
   const EnvView ev = P->env.view();
@@ -1079,8 +1111,10 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   reduce_cols_kernel<<<1, 256, 0, s>>>(P->cam_out.p, ncb, 2, 2, P->scal.p + 6);
   ++P->launches;
   if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 2, 3, s));   // model, step^2, x^2 of the landmark shard
-  visual_cost_t<kLoss>(P, P->cand(), P->scal.p + 8, intr ? P->intr_c : nullptr);   // candidate cost
-  if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 8, 1, s));
+  if (cand) {
+    visual_cost_t<kLoss>(P, P->cand(), P->scal.p + 8, intr ? P->intr_c : nullptr);   // candidate cost
+    if (cm.active()) LVBA_TRY(cm.allreduce_sum(P->scal.p + 8, 1, s));
+  }
   P->timers.end();
   LVBA_CUDA(cudaGetLastError());
   LVBA_CUDA(cudaMemcpyAsync(P->h_scal, P->scal.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -1100,17 +1134,15 @@ inline int visual_linearize_solve_t(lvba_visual_problem* P, double radius, bool 
   }
   return LVBA_OK;
 }
-inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool want_steps) {
-  return P->robust() ? visual_linearize_solve_t<true>(P, radius, want_steps) : visual_linearize_solve_t<false>(P, radius, want_steps);
+// cand = false: no candidate cost (scal[8] keeps its value), for the Gauss-Newton step of the dogleg, whose candidate is another
+inline int visual_linearize_solve(lvba_visual_problem* P, double radius, bool want_steps, bool cand = true) {
+  return P->robust() ? visual_linearize_solve_t<true>(P, radius, want_steps, cand) : visual_linearize_solve_t<false>(P, radius, want_steps, cand);
 }
 
-inline int visual_iterate_impl(lvba_visual_problem* P, int n_iter, lvba_summary* sum) {
-  const double t0 = wall_ms();
-  const int64_t l0 = P->launches, h0 = P->h2d, d0 = P->d2h;
+// n_iter passes of the LM (LevenbergMarquardtStrategy)
+inline int visual_lm_passes(lvba_visual_problem* P, int n_iter) {
   TrustRegionState& lm = P->lm;
-  const int iters0 = lm.iters, acc0 = lm.accepted, builds0 = lm.builds;
   const lvba_visual_opts& o = P->opts;
-  if (!lm.have_scale) LVBA_TRY(visual_compute_scale(P, o.jacobi_scaling));
   for (int it = 0; it < n_iter && !lm.converged; ++it) {
     LVBA_TRY(visual_linearize_solve(P, lm.radius, false));
     const double* h = P->h_scal;
@@ -1154,6 +1186,132 @@ inline int visual_iterate_impl(lvba_visual_problem* P, int n_iter, lvba_summary*
       if (lm.radius < o.min_radius) { lm.converged = true; lm.termination = LVBA_TERM_RADIUS; }
     }
   }
+  return LVBA_OK;
+}
+
+// ---------------------------------------------------------------- DOGLEG (visual_dogleg.h)
+// The buffers of a dogleg pass for the current plan (kept while their size fits; a re-plan resets the state, so nothing stale
+// is reused)
+inline int visual_dogleg_bufs(lvba_visual_problem* P, vdog::Bufs& B) {
+  const int64_t n = 6 * (int64_t)P->n_rows + 3 * P->Tv, ps = vdog::prod_size(n, P->Tv), pp = vdog::part_size(n, P->Tv);
+  const size_t need = (size_t)(4 * n + ps + pp + vdog::kNScal);
+  if (P->dl_buf.n < need) LVBA_TRY(P->dl_buf.alloc(need));
+  double* b = P->dl_buf.p;
+  B = vdog::Bufs{b, b + n, b + 2 * n, b + 3 * n, b + 4 * n, b + 4 * n + ps, b + 4 * n + ps + pp};
+  return LVBA_OK;
+}
+
+// One dogleg step after the Gauss-Newton solve (fresh: the first on this linearisation): D, g, GN and alpha when fresh, the
+// case and the step, the candidate into qc / tc / Xc, the model, the step norms and the candidate cost into scal as
+// visual_linearize_solve leaves them; both scalar sets to the host
+template <bool kLoss>
+inline int visual_dogleg_pass_t(lvba_visual_problem* P, bool fresh) {
+  cudaStream_t s = P->stream;
+  vdog::Bufs B;
+  LVBA_TRY(visual_dogleg_bufs(P, B));
+  const VisualLM lmp = visual_lm_params(P, 1.0 / P->lm.mu);
+  P->timers.begin(PH_RESID);
+  CudaExec ex;
+  ex.stream = s;
+  if (fresh)
+    LVBA_TRY(vdog::linearised<kLoss>(ex, P->view(), P->state(), lmp, P->n_rows, P->Tv, P->cam_colsq.p, P->cam_grad.p, P->y.p, P->pt_step.p, B));
+  LVBA_TRY(vdog::step<kLoss>(ex, P->view(), P->state(), lmp, P->n_rows, P->Tv, P->lm.radius, fresh, P->Xc.p, B, P->scal.p));
+  P->launches += ex.launches;
+  const int ncb = (P->n_rows + 127) / 128;
+  if (ncb > 0) {
+    visual_cam_update_kernel<<<ncb, 128, 0, s>>>(P->n_rows, P->d_cam_of_row.p, P->q.p, P->t.p, B.v, P->s_cam.p, P->qc.p, P->tc.p, nullptr,
+                                                 P->cam_out.p);
+    ++P->launches;
+  }
+  reduce_cols_kernel<<<1, 256, 0, s>>>(P->cam_out.p, ncb, 2, 2, P->scal.p + 6);
+  ++P->launches;
+  visual_cost_t<kLoss>(P, P->cand(), P->scal.p + 8);
+  P->timers.end();
+  LVBA_CUDA(cudaGetLastError());
+  LVBA_CUDA(cudaMemcpyAsync(P->h_scal, P->scal.p, 16 * sizeof(double), cudaMemcpyDeviceToHost, s));
+  LVBA_CUDA(cudaMemcpyAsync(P->h_dl, B.sc, sizeof(P->h_dl), cudaMemcpyDeviceToHost, s));
+  LVBA_CUDA(cudaStreamSynchronize(s));
+  P->d2h += 16 * sizeof(double) + sizeof(P->h_dl);
+  TrustRegionState& lm = P->lm;
+  const double* d = P->h_dl;
+  lm.alpha = d[vdog::kAlpha]; lm.grad_norm = std::sqrt(d[vdog::kGG]); lm.gn_norm = std::sqrt(d[vdog::kNN]);
+  lm.dl_case = (int)d[vdog::kCase]; lm.dl_norm = d[vdog::kStepNorm];
+  return LVBA_OK;
+}
+
+// n_iter passes of the dogleg (DoglegStrategy; the rule in visual_dogleg.h).  A pass after a rejected step reuses the
+// linearisation: no build and no solve.
+inline int visual_dogleg_passes(lvba_visual_problem* P, int n_iter) {
+  TrustRegionState& lm = P->lm;
+  const lvba_visual_opts& o = P->opts;
+  for (int it = 0; it < n_iter && !lm.converged; ++it) {
+    const bool fresh = !lm.reuse;
+    bool solved = !fresh, linearised = false;
+    for (; fresh && lm.mu < vdog::kMaxMu; lm.mu *= vdog::kMuIncrease) {   // the Gauss-Newton step at radius 1 / mu
+      LVBA_TRY(visual_linearize_solve(P, 1.0 / lm.mu, true, false));
+      const double* h = P->h_scal;
+      if (!linearised) {
+        linearised = true;
+        lm.cost = h[0];
+        if (!lm.have_first) { lm.cost_first = lm.cost; lm.have_first = true; }
+        const double gmax = std::max(h[1], h[5]);
+        if (o.gradient_tolerance >= 0 && gmax <= o.gradient_tolerance) { lm.converged = true; lm.termination = LVBA_TERM_GRADIENT_TOL; break; }
+      }
+      if (*reinterpret_cast<const int*>(h + 15) == 0 && std::isfinite(h[3]) && std::isfinite(h[6])) { solved = true; break; }
+    }
+    if (lm.converged) break;
+    ++lm.iters;
+    if (!fresh) ++lm.reused;
+    lm.reuse = true;                                  // DoglegStrategy::ComputeStep: reuse_ = true once a step is computed
+    if (solved) {
+      if (P->robust()) LVBA_TRY(visual_dogleg_pass_t<true>(P, fresh));
+      else LVBA_TRY(visual_dogleg_pass_t<false>(P, fresh));
+    }
+    const double* h = P->h_scal;
+    const double model = h[2], cand = h[8];
+    const double step_norm = std::sqrt(h[3] + h[6]), x_norm = std::sqrt(h[4] + h[7]);
+    const bool valid = solved && std::isfinite(model) && std::isfinite(step_norm) && model > 0.0;
+    if (o.verbose)
+      fprintf(stderr, "[lvba visual dogleg] iter %d: cost %.9g cand %.9g model %.6g radius %.3g mu %.3g case %d reuse %d valid %d\n", lm.iters,
+              lm.cost, cand, model, lm.radius, lm.mu, lm.dl_case, (int)!fresh, (int)valid);
+    if (!valid) {                                    // DoglegStrategy::StepIsInvalid: the radius stays
+      ++lm.invalid;
+      lm.mu *= vdog::kMuIncrease;
+      lm.reuse = false;
+      if (lm.invalid >= 5) { lm.converged = true; lm.termination = LVBA_TERM_INVALID_STEPS; }
+      continue;
+    }
+    lm.invalid = 0;
+    const double rho = (lm.cost - cand) / model;
+    if (o.parameter_tolerance >= 0 && step_norm <= o.parameter_tolerance * (x_norm + o.parameter_tolerance)) {
+      lm.converged = true; lm.termination = LVBA_TERM_PARAMETER_TOL; break;
+    }
+    if (o.function_tolerance >= 0 && std::fabs(lm.cost - cand) <= o.function_tolerance * lm.cost) {
+      lm.converged = true; lm.termination = LVBA_TERM_FUNCTION_TOL; break;
+    }
+    if (std::isfinite(cand) && rho > o.min_relative_decrease) {             // StepAccepted
+      std::swap(P->q.p, P->qc.p); std::swap(P->t.p, P->tc.p); std::swap(P->X.p, P->Xc.p);
+      lm.cost = cand;
+      ++lm.accepted;
+      if (rho < vdog::kDecrease) lm.radius *= 0.5;
+      if (rho > vdog::kIncrease) lm.radius = std::max(lm.radius, 3.0 * lm.dl_norm);
+      lm.mu = std::max(vdog::kMinMu, 2.0 * lm.mu / vdog::kMuIncrease);
+      lm.reuse = false;
+    } else {                                                                  // StepRejected
+      lm.radius *= 0.5;
+    }
+    if (lm.radius < o.min_radius) { lm.converged = true; lm.termination = LVBA_TERM_RADIUS; }
+  }
+  return LVBA_OK;
+}
+
+inline int visual_iterate_impl(lvba_visual_problem* P, int n_iter, lvba_summary* sum) {
+  const double t0 = wall_ms();
+  const int64_t l0 = P->launches, h0 = P->h2d, d0 = P->d2h;
+  TrustRegionState& lm = P->lm;
+  const int iters0 = lm.iters, acc0 = lm.accepted, builds0 = lm.builds;
+  if (!lm.have_scale) LVBA_TRY(visual_compute_scale(P, P->opts.jacobi_scaling));
+  LVBA_TRY(P->dogleg() ? visual_dogleg_passes(P, n_iter) : visual_lm_passes(P, n_iter));
   if (sum) {
     LVBA_CUDA(cudaStreamSynchronize(P->stream));
     double ms[PH_COUNT] = {0, 0, 0};
@@ -1291,6 +1449,7 @@ void lvba_visual_default_opts(lvba_visual_opts* o) {
   // Ceres' Solver::Options: DENSE_SCHUR (src/lvba_system.cpp:1574); eta, min / max_linear_solver_iterations
   o->linear_solver = LVBA_LINEAR_DENSE_SCHUR;
   o->eta = 1e-1; o->min_linear_iter = 0; o->max_linear_iter = 500;
+  o->trust_region_strategy = LVBA_TR_LEVENBERG_MARQUARDT;       // Ceres' default
 }
 
 int lvba_visual_create(int32_t M, int64_t T, const double* q, const double* t, const double* X, const double* plane_nd,
@@ -1313,6 +1472,7 @@ int lvba_visual_set_state(lvba_visual_problem* p, const double* q, const double*
   LVBA_TRY(p->t.upload(t, (size_t)p->M * 3, p->stream, &p->h2d)); LVBA_TRY(p->tc.upload(t, (size_t)p->M * 3, p->stream));
   LVBA_TRY(p->X.upload(X, (size_t)p->T * 3, p->stream, &p->h2d)); LVBA_TRY(p->Xc.upload(X, (size_t)p->T * 3, p->stream));
   LVBA_CUDA(cudaStreamSynchronize(p->stream));
+  lvba::visual_dogleg_forget(p);
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_set_state")
 
@@ -1361,7 +1521,10 @@ int lvba_visual_step(lvba_visual_problem* p, double radius, int32_t jacobi_scali
   if (!p || !(radius > 0)) return lvba::fail(LVBA_ERR_INVALID_ARG, "bad argument");
   LVBA_TRY(lvba::visual_check_usable(p));
   LVBA_CUDA(cudaSetDevice(p->device));
-  if (recompute_scale || !p->lm.have_scale) LVBA_TRY(lvba::visual_compute_scale(p, jacobi_scaling));
+  if (recompute_scale || !p->lm.have_scale) {
+    LVBA_TRY(lvba::visual_compute_scale(p, jacobi_scaling));
+    lvba::visual_dogleg_forget(p);
+  }
   LVBA_CUDA(cudaMemsetAsync(p->cam_step.p, 0, (size_t)p->M * 6 * sizeof(double), p->stream));
   if (p->T > 0) LVBA_CUDA(cudaMemsetAsync(p->pt_step.p, 0, (size_t)p->T * 3 * sizeof(double), p->stream));
   LVBA_TRY(lvba::visual_linearize_solve(p, radius, true));
@@ -1423,6 +1586,7 @@ int lvba_visual_reset_state(lvba_visual_problem* p) LVBA_ABI_BEGIN {
   std::copy(p->intr0, p->intr0 + 8, p->intr);
   std::copy(p->intr0, p->intr0 + 8, p->intr_c);
   lvba::visual_intr_forget(p);
+  lvba::visual_dogleg_forget(p);
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_reset_state")
 
@@ -1460,6 +1624,7 @@ int lvba_visual_lm(int32_t M, int64_t T, double* q, double* t, double* X, const 
   if (opts) o = *opts; else lvba_visual_default_opts(&o);
   LVBA_TRY(lvba::visual_check_loss(o));                       // before any device work: the buffers stay untouched
   LVBA_TRY(lvba::visual_check_linear(o));
+  LVBA_TRY(lvba::visual_check_trust(o));
   if (o.refine_intrinsics)
     return lvba::fail(LVBA_ERR_INVALID_ARG, "refine_intrinsics needs a handle (lvba_visual_reset_lm): the one-shot call's intr is const");
   LVBA_TRY(lvba::visual_check_mask(M > 0 && !lvba::visual_mask(M, o.cam_fixed).empty()));
@@ -1526,6 +1691,7 @@ int lvba_visual_set_intrinsics(lvba_visual_problem* p, const double intr[8]) LVB
     if (!std::isfinite(intr[i])) return lvba::fail(LVBA_ERR_INVALID_ARG, "intr[%d] = %g is not finite", i, intr[i]);
   std::copy(intr, intr + 8, p->intr);
   std::copy(intr, intr + 8, p->intr_c);
+  lvba::visual_dogleg_forget(p);
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_set_intrinsics")
 
@@ -1586,6 +1752,21 @@ int lvba_visual_apply_system(lvba_visual_problem* p, const double* x, double* y)
   p->d2h += (int64_t)(n6 * sizeof(double));
   return LVBA_OK;
 } LVBA_ABI_END("lvba_visual_apply_system")
+
+int lvba_visual_dogleg_state(lvba_visual_problem* p, double* radius, double* mu, double* alpha, double* grad_norm, double* gn_norm,
+                             int32_t* step_case, int64_t* reused) LVBA_ABI_BEGIN {
+  if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");
+  if (!p->dogleg()) return lvba::fail(LVBA_ERR_INVALID_ARG, "the last lvba_visual_reset_lm chose the LM: no dogleg state");
+  const lvba::TrustRegionState& s = p->lm;
+  if (radius) *radius = s.radius;
+  if (mu) *mu = s.mu;
+  if (alpha) *alpha = s.alpha;
+  if (grad_norm) *grad_norm = s.grad_norm;
+  if (gn_norm) *gn_norm = s.gn_norm;
+  if (step_case) *step_case = s.dl_case;
+  if (reused) *reused = s.reused;
+  return LVBA_OK;
+} LVBA_ABI_END("lvba_visual_dogleg_state")
 
 int lvba_visual_linear_stats(lvba_visual_problem* p, int64_t* cg_iters_total, int32_t* cg_iters_last, int32_t* term_last) LVBA_ABI_BEGIN {
   if (!p) return lvba::fail(LVBA_ERR_INVALID_ARG, "null argument");

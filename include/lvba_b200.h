@@ -147,6 +147,20 @@ typedef struct lvba_visual_opts {
   double eta;                    /* 0.1   Solver::Options::eta */
   int32_t min_linear_iter;       /* 0     min_linear_solver_iterations */
   int32_t max_linear_iter;       /* 500   max_linear_solver_iterations */
+  /* The trust-region strategy (Ceres' trust_region_strategy_type), lvba_trust_region:
+   *   LVBA_TR_LEVENBERG_MARQUARDT (the default, the reference's choice): initial_radius, max_radius, min_lm_diagonal and
+   *     max_lm_diagonal as documented above.
+   *   LVBA_TR_DOGLEG: Ceres' TRADITIONAL_DOGLEG, restated from ceres-solver 2.1.0 (csrc/visual_dogleg.h): the Gauss-Newton step
+   *     (the DENSE_SCHUR solve with the small regularisation mu D^2), the Cauchy point and the dogleg between them inside the
+   *     radius, which starts at initial_radius (max_radius does not bound it, as in Ceres).  A rejected step keeps the
+   *     linearisation and only moves the dogleg point, so a rejected pass costs no build and no solve: hessian_builds is then
+   *     lower than iterations.  lvba_visual_set_state, _reset_state, _set_intrinsics and an lvba_visual_step that recomputes the
+   *     Jacobi scale change what that linearisation was taken at: the next pass linearises again.
+   * As linear_solver: the one-shot call takes it from its opts, a handle from lvba_visual_reset_lm.  Refused before any device
+   * work: an unknown value, and DOGLEG with ITERATIVE_SCHUR (LVBA_ERR_INVALID_ARG: the dogleg needs an exact Gauss-Newton step);
+   * DOGLEG with refine_intrinsics != 0 or an active communicator (LVBA_ERR_UNSUPPORTED).  lvba_visual_dogleg_state reports the
+   * state.  Sits before cam_fixed, which stays the last field. */
+  int32_t trust_region_strategy; /* LVBA_TR_LEVENBERG_MARQUARDT */
   /* Constant cameras (ceres::Problem::SetParameterBlockConstant, which the reference calls on camera 0 at
    * src/lvba_system.cpp:1582-1583): NULL (the default) or M bytes, nonzero = camera held constant.  The constant cameras are
    * fixed_cam and every camera c with cam_fixed[c] != 0; they get no row in the reduced camera system and come back
@@ -168,6 +182,19 @@ typedef enum lvba_linear_solver {
   LVBA_LINEAR_DENSE_SCHUR = 0,
   LVBA_LINEAR_ITERATIVE_SCHUR = 1
 } lvba_linear_solver;
+
+typedef enum lvba_trust_region {
+  LVBA_TR_LEVENBERG_MARQUARDT = 0,
+  LVBA_TR_DOGLEG = 1              /* Ceres' TRADITIONAL_DOGLEG */
+} lvba_trust_region;
+
+/* the step of the last dogleg pass (lvba_visual_dogleg_state) */
+typedef enum lvba_dogleg_case {
+  LVBA_DOGLEG_NONE = 0,           /* no step since the last reset */
+  LVBA_DOGLEG_GAUSS_NEWTON = 1,   /* the Gauss-Newton step lies inside the radius */
+  LVBA_DOGLEG_CAUCHY = 2,         /* the gradient step cut at the radius */
+  LVBA_DOGLEG_INTERPOLATED = 3    /* the point between the Cauchy point and the Gauss-Newton step on the radius */
+} lvba_dogleg_case;
 
 #define LVBA_INTR_FOCAL      0x03u   /* fx fy */
 #define LVBA_INTR_PRINCIPAL  0x0Cu   /* cx cy */
@@ -385,6 +412,12 @@ int lvba_visual_schur_product(lvba_visual_problem* p, int32_t* matrix_free);
  * its conjugate gradients used (for parity tests).  LVBA_ERR_INVALID_ARG unless that pass ran ITERATIVE_SCHUR: before any pass,
  * after lvba_visual_reset_lm or a re-plan, and under DENSE_SCHUR. */
 int lvba_visual_apply_system(lvba_visual_problem* p, const double* x, double* y);
+/* The dogleg state of a handle whose last lvba_visual_reset_lm chose LVBA_TR_DOGLEG (else LVBA_ERR_INVALID_ARG): the radius
+ * Delta and mu as the next pass will use them; alpha, |g| and |GN| of the current linearisation and the lvba_dogleg_case of the
+ * last step (all 0 before the first pass); the passes since the last reset that reused a linearisation.  In the D-scaled
+ * space of csrc/visual_dogleg.h.  Any pointer may be NULL.  A reset, a removal and a cam_fixed re-plan start it again. */
+int lvba_visual_dogleg_state(lvba_visual_problem* p, double* radius, double* mu, double* alpha, double* grad_norm,
+                             double* gn_norm, int32_t* step_case, int64_t* reused);
 int lvba_visual_iterate(lvba_visual_problem* p, int32_t n_iter, lvba_summary* summary);
 int lvba_visual_counts(lvba_visual_problem* p, int64_t* nnz_valid, int64_t* n_valid_tracks,
                        int64_t* n_blocks_env, int64_t* n_pairs);

@@ -55,6 +55,9 @@
 //   --linear-solver dense_schur|iterative_schur   the solver of the visual stage's reduced camera system
 //                (lvba_visual_opts::linear_solver): the envelope LDL^T (the default) or Ceres' ITERATIVE_SCHUR, conjugate gradients at
 //                Ceres' default forcing tolerance.  Checked when parsed (--check included); without the flag the output is as before.
+//   --trust-region lm|dogleg   the trust-region strategy of the visual stage (lvba_visual_opts::trust_region_strategy):
+//                Levenberg-Marquardt (the default) or Ceres' TRADITIONAL_DOGLEG, which needs --linear-solver dense_schur.  Checked
+//                when parsed (--check included); without the flag the output is as before.
 #include <climits>
 #include <cmath>
 #include <cstdio>
@@ -152,6 +155,15 @@ int main(int argc, char** argv) {
       else if (v == "iterative_schur") visual_opts.linear_solver = LVBA_LINEAR_ITERATIVE_SCHUR;
       else {
         std::fprintf(stderr, "--linear-solver: '%s' is not dense_schur or iterative_schur\n", v.c_str());
+        return 64;
+      }
+    }
+    else if (a == "--trust-region") {
+      const std::string v = next();
+      if (v == "lm") visual_opts.trust_region_strategy = LVBA_TR_LEVENBERG_MARQUARDT;
+      else if (v == "dogleg") visual_opts.trust_region_strategy = LVBA_TR_DOGLEG;
+      else {
+        std::fprintf(stderr, "--trust-region: '%s' is not lm or dogleg\n", v.c_str());
         return 64;
       }
     }
